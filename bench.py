@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py - depth-maps/s of the MVSFormer++ depth-inference hot path on B200 (BASELINE.json metric).
+"""bench.py - depth-maps/s of the MVSFormer++ depth-inference hot path on H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            # our arm (CUDA library behind the reference seams)
   python bench.py --impl reference --gpus N --steps K ...   # CPU arm: the reference's algorithm on the host cores
+  python bench.py ... --dump-outputs DIR                    # also write the last timed step's outputs as DIR/<name>.npy
 
 A step = one pass of the hot path (FMT -> 4-stage cascade: warp + group-correlation + visibility aggregation ->
 cost regularisation -> soft-argmax) over one batch of synthetic reference views; the workload is BASELINE.json
@@ -30,6 +31,33 @@ WORKLOADS = {
     "small": dict(name="plumbing: V=3, numdepth=48, 128x192", V=3, H=128, W=192, numdepth=48),
 }
 TMP = [5.0, 5.0, 5.0, 1.0]
+H100_HBM_GBS = 3350.0              # NVIDIA H100 SXM data sheet (700 W card)
+H100_FP16_DENSE_TFLOPS = 989.0     # same data sheet, dense FP16 tensor-core rate
+DUMP_SAMPLE = 1 << 18              # elements kept of a probability volume larger than this (fixed, seeded positions)
+
+
+def dump_outputs(path, outs):
+    """Writes what the hot path returned for the first reference view of the last timed step as float32 .npy files:
+    the final depth and confidence maps in full, per stage the depth and confidence maps, and a fixed, seeded sample of
+    every per-stage probability volume (DUMP_SAMPLE elements; their flat positions are stored next to them, float64).
+    About 45 MB for the DTU workload, under 64 MB for Tanks and Temples."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    for out in outs[:1]:
+        arrays = {"refined_depth": out["refined_depth"], "photometric_confidence": out["photometric_confidence"]}
+        for s in range(1, 5):
+            so = out[f"stage{s}"]
+            arrays[f"stage{s}_depth"] = so["depth"]
+            arrays[f"stage{s}_photometric_confidence"] = so["photometric_confidence"]
+            pv = so["prob_volume"].reshape(-1)
+            idx = np.random.default_rng(1000 + s).choice(pv.numel(), size=min(DUMP_SAMPLE, pv.numel()), replace=False)
+            idx.sort()
+            arrays[f"stage{s}_prob_volume_sample"] = pv[torch.from_numpy(idx).to(pv.device)]
+            arrays[f"stage{s}_prob_volume_sample_index"] = idx
+        for name, t in arrays.items():
+            v = t.detach().float().cpu().numpy() if hasattr(t, "detach") else np.asarray(t)
+            np.save(os.path.join(path, f"{name}.npy"), v.astype(np.float64 if v.dtype.kind in "iu" else np.float32))
 
 
 def algorithmic_bytes(V, H, W, feat_chs=(64, 32, 16, 8), ndepths=(32, 16, 8, 4), G=8):
@@ -42,7 +70,7 @@ def algorithmic_bytes(V, H, W, feat_chs=(64, 32, 16, 8), ndepths=(32, 16, 8, 4),
 
 
 class ClockSampler(threading.Thread):
-    """Samples nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks/throttle reasons during the timed region."""
 
     def __init__(self, gpu_index):
         super().__init__(daemon=True)
@@ -151,8 +179,8 @@ def cpu_reference_pass(wl, threads, seed=1234):
 
 
 def cpu_threads():
-    """Host threads of the CPU arm: measured on the 2 x 32-core GPU box, the ATen kernels peak at 32 threads (12.5 s per
-    depth map; 64: 14.6 s; all 128 hyper-threads: 170 s)."""
+    """Host threads of the CPU arm: the reference's ATen kernels stop scaling beyond about 32 threads and slow down with
+    hyper-threads, so at most 32 are used (tools/cpu_threads_probe.py measures it for a given host)."""
     return max(1, min(32, os.cpu_count() or 1))
 
 
@@ -187,7 +215,7 @@ def run_ours(a, wl, rank, world, local_rank):
     from mvsformerplusplus_b200 import _lib
 
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py: no CUDA device - the B200 hot path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise RuntimeError("bench.py: no CUDA device - the hot path has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     numa = bind_to_gpu_numa_node(local_rank) if world > 1 else None   # before any pinned allocation
@@ -223,17 +251,21 @@ def run_ours(a, wl, rank, world, local_rank):
     lane_bufs = [local_buf] + [torch.empty_like(local_buf) for _ in range(n_lanes - 1)]
     lane_gathered = [torch.cuda.Event() for _ in range(n_lanes)]
     step_no = [0]
+    last_outs = [None]   # what the last resident step returned, one output dict per reference view (--dump-outputs)
 
     def step_resident():
         k = step_no[0] % n_lanes
         step_no[0] += 1
         lane, buf = lanes[k], lane_bufs[k]
+        outs = []
         with torch.cuda.stream(lane):
             lane.wait_event(lane_gathered[k])           # the gather of this lane's previous step has read `buf`
             for b, (f, p, d) in enumerate(dev_inputs):
                 out = net.forward_features(f, p, d, TMP)
                 buf[b, 0].copy_(out["refined_depth"][0])
                 buf[b, 1].copy_(out["photometric_confidence"][0])
+                outs.append(out)
+        last_outs[0] = outs
         # the only collective on the path: gather of the depth / confidence maps in item order (SURVEY.md 8e), issued on the
         # main stream in step order on every rank (after the lane's kernels; the other lane keeps running)
         if world > 1:
@@ -288,10 +320,13 @@ def run_ours(a, wl, rank, world, local_rank):
     if sampler:
         sampler.start()
     _lib.launch_count(reset=True)
-    ms_step = timed(step_resident, a.steps, max(a.warmup, 3))
-    launches = _lib.launch_count(reset=True) // (a.steps + max(a.warmup, 3))
+    ms_step = timed(step_resident, a.steps, a.warmup)
+    launches = _lib.launch_count(reset=True) // max(1, a.steps + a.warmup)
     clocks = sampler.stop() if sampler else None
-    ms_e2e = timed(step_e2e, a.steps, max(a.warmup, 3))
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, last_outs[0])
+    last_outs[0] = None
+    ms_e2e = timed(step_e2e, a.steps, a.warmup)
     d2h = host_out.numel() * 4
 
     # ---- per-entry-point device time (CUDA events on the launching stream) for the roofline of the fused
@@ -308,49 +343,33 @@ def run_ours(a, wl, rank, world, local_rank):
         att_ms, att_n = _lib.ktimer_read("attention_tc")
         _lib.ktimer_enable(False)
         per_map = {k: v["ms"] / reps for k, v in summ.items()}
-        peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-        peaks = json.load(open(peaks_path)) if os.path.exists(peaks_path) else {}
-        # dominant kernel of the step: stage-1 softmax attention (tcgen05), one launch per transformer layer.
+        # dominant kernel of the step: stage-1 softmax attention (wgmma), one launch per transformer layer.
         # algorithmic FLOPs per launch = 2 GEMMs x 2 N^2 hd per head (the 3 split-precision products are overhead)
         n_tok = (net.ndepths[0] // 2) * (H // 8 // 4) * (W // 8 // 4)   # stage 1: D x H/8 x W/8, down_rate (2,4,4)
         att_flops = 4.0 * n_tok * n_tok * 16 * 4
         att_launch_ms = att_ms / max(att_n, 1)
-        tf_peak = peaks.get("bf16_tflops_sustained", 1480.0)
-        tf_which = ("measured (MEASURED_PEAKS.json bf16_tflops_sustained: the kernel runs inside a long step)"
-                    if peaks else "fallback (B200_PROFILING.md)")
+        tf_peak, tf_which = H100_FP16_DENSE_TFLOPS, "H100 SXM data sheet, dense FP16 (700 W card)"
         achieved_tf = att_flops / 1e12 / (att_launch_ms / 1e3) if att_launch_ms > 0 else 0.0
-        traffic = traffic_wc = None   # dram bytes of the same kernels from the committed ncu capture (profiles/)
-        tpath = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-        if os.path.exists(tpath) and wl is WORKLOADS["dtu"]:
-            tj = json.load(open(tpath))
-            traffic = tj.get("attention_fa_kernel", {}).get("dram_bytes_per_launch")
-            traffic_wc = tj.get("warp_corr_entropy_store + corr_aggregate (8 launches / depth map)", {}).get("dram_bytes_per_depth_map")
+        traffic = traffic_wc = None   # DRAM bytes are not measured (no hardware-counter profiler on the benchmark machines)
         line_extra["roofline"] = {"bound": "tensor", "kernel": "attention_fa_kernel (stage-1 transformer regulariser, 1 launch / layer)",
                                   "achieved": achieved_tf, "peak": tf_peak, "unit": "TFLOP/s", "frac": achieved_tf / tf_peak,
                                   "traffic": traffic, "peak_source": tf_which, "algorithmic_flops_per_launch": att_flops,
                                   "launch_ms": att_launch_ms, "launches_per_depth_map": att_n // reps,
                                   "share_of_step": att_ms / reps / ms_step if ms_step > 0 else None,
-                                  "note": "bound by the XU pipe (ncu: 83.7 % busy): 3.06e9 exp2 per launch at 16 / clk / SM = 0.66 ms, plus the "
-                                          "mbarrier handshake latency between the MMA and softmax warps (DESIGN.md 4); "
+                                  "note": "the softmax needs one exp2 per score (MUFU, 16 / clk / SM); "
                                           "Q/K/V are fp16 hi+lo (3 products for the scores), the probabilities fp16"}
         # the fused warp + group-correlation kernels are the HBM-roofline kernels of the path (8 launches / depth map)
         t_wc = sum(per_map.get(k, 0.0) for k in ("mvsf_warp_corr_entropy", "mvsf_warp_corr_aggregate",
                                                   "mvsf_warp_corr_entropy_store", "mvsf_corr_aggregate"))
         alg = algorithmic_bytes(wl["V"], H, W)
-        if peaks:
-            peak, which = peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)"
-        else:
-            peak, which = 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        peak, which = H100_HBM_GBS, "H100 SXM data sheet, 3.35 TB/s HBM3"
         achieved = sum(alg) / 1e9 / (t_wc / 1e3) if t_wc > 0 else 0.0
         line_extra["roofline_hbm"] = {"bound": "hbm", "kernel": "warp_corr_entropy_store + corr_aggregate (8 launches / depth map)",
                                       "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                                       "traffic": traffic_wc, "peak_source": which, "algorithmic_bytes_per_depth_map": sum(alg),
                                       "kernel_ms_per_depth_map": t_wc,
-                                      "note": "algorithmic bytes = features + hypotheses + volume; traffic = measured DRAM bytes of the pass-A / "
-                                              "pass-B launches of one depth map (profiles/r2_ncu_traffic.json; stage 4 pass A = selection kernel + "
-                                              "TMA pipeline kernel + the L1 kernel's skipped launch): the per-view group correlations spilled "
-                                              "between the two passes are implementation traffic.  The 4-corner fp32 gather is bound by the SM "
-                                              "load path (3.6 GB per stage and pass at 128 B/clk/SM): ceiling ~0.22 of the HBM roofline"}
+                                      "note": "algorithmic bytes = features + hypotheses + volume; the per-view group correlations "
+                                              "spilled between the two passes are implementation traffic and not counted"}
         line_extra["kernel_ms_per_depth_map"] = {k.replace("mvsf_", ""): round(v, 4) for k, v in sorted(per_map.items())}
 
     if rank == 0:
@@ -365,11 +384,11 @@ def run_ours(a, wl, rank, world, local_rank):
                               "oracle port calling the reference's ATen kernels F.grid_sample + SDPA)")}
         maps = B * world
         line = {"metric": "depth-maps/sec (hot path: FMT + 4-stage cascade)", "value": maps * 1000.0 / ms_step,
-                "unit": "depth-maps/s", "n_gpus": world, "steps": a.steps, "warmup": max(a.warmup, 3), "ms_per_step": ms_step,
+                "unit": "depth-maps/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms_step,
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
                 "config": {"workload": wl["name"], "ref_views_per_gpu_per_step": B, "parallelism": f"shard{world}",
                            "l2": "inputs_larger_than_l2 (531 MB feature pyramids per depth map)",
-                           "precision": "fp32-class parity mode: tcgen05 GEMMs / attention scores / 3-D and 2-D convolutions on fp16 hi+lo "
+                           "precision": "fp32-class parity mode: wgmma GEMMs / attention scores / 3-D and 2-D convolutions on fp16 hi+lo "
                                         "split operands (22-bit mantissa, fp32 accumulate), attention probabilities fp16, "
                                         "everything else fp32 SIMT",
                            "e2e_pipeline": "pinned host batch (allocated on the GPU's NUMA node) -> copy stream -> device slots; "
@@ -411,8 +430,7 @@ def run_dsweep(a):
     torch.manual_seed(0)
     sd = synth.randomize_state_dict(build_hotpath_params(default_args()).eval(), seed=7)
     wts = packing.pack_vis(sd, "fusions.3.vis.").to(dev)
-    peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak = json.load(open(peaks_path))["hbm_gbs"] if os.path.exists(peaks_path) else 6650.0
+    peak = H100_HBM_GBS
     rows = []
     for D in (48, 96, 192, 384):
         k = torch.arange(D, dtype=torch.float32, device=dev) / (D - 1)
@@ -432,7 +450,7 @@ def run_dsweep(a):
         _lib.check(L.mvsf_vis_cnn(P(ent), P(wts), P(vis), V - 1, H, W, st()), "vis_cnn")
         pass_b()
         torch.cuda.synchronize()
-        reps = max(1, a.steps // 3)
+        reps = max(1, a.steps)
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
         ta = tb = 0.0
         for _ in range(reps):
@@ -450,7 +468,7 @@ def run_dsweep(a):
             "config": {"workload": "dsweep: plane-sweep hypotheses uniform in inverse depth over 425..931 mm, two-gather plan "
                                    "(pass A entropy + pass B aggregation), inputs larger than L2 (283 MB of features)"},
             "roofline": {"bound": "hbm", "peak": peak, "unit": "GB/s", "achieved": best, "frac": best / peak, "traffic": None},
-            "sweep": rows, "gpu_launches": 2 * len(rows) * max(1, a.steps // 3)}
+            "sweep": rows, "gpu_launches": 2 * len(rows) * max(1, a.steps)}
     print(json.dumps(line), flush=True)
 
 
@@ -463,10 +481,10 @@ def main():
     ap.add_argument("--workload", default="dtu", choices=sorted(WORKLOADS) + ["dsweep"])
     ap.add_argument("--batch", type=int, default=1, help="reference views per GPU per step")
     ap.add_argument("--streams", type=int, default=1,
-                    help="compute streams per GPU: consecutive steps alternate between them.  EXPERIMENTAL above 1: two depth maps in "
-                         "flight measured +8.7 %% (79.8 maps/s) but the attention kernel deadlocks once in a few hundred launches when "
-                         "kernels of another stream run next to it (DESIGN.md 5); the bounded waits turn that into a CUDA error")
+                    help="compute streams per GPU: consecutive steps alternate between them (two depth maps in flight)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32)")
     a = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -477,9 +495,6 @@ def main():
         return
     wl = WORKLOADS[a.workload]
     if a.impl == "reference":
-        if a.steps > 3:
-            a.steps = 3  # each step is ~15-60 s of host work; keep the arm within minutes
-        a.warmup = min(a.warmup, 1)
         run_reference_arm(a, wl, rank, world)
         return
     run_ours(a, wl, rank, world, local_rank)

@@ -1,5 +1,5 @@
 /*
- * libmvsf_b200 - C ABI of the B200-native MVSFormer++ depth-inference hot path.
+ * libmvsf_b200 - C ABI of the CUDA-native (sm_90a) MVSFormer++ depth-inference hot path.
  *
  * The reference (maybeLx/MVSFormerPlusPlus) has no FFI layer: its seams are Python callables
  * (SURVEY.md §8b).  Each entry point below states the reference callable (file:line, relative to the
@@ -93,12 +93,12 @@ int mvsf_warp_corr_set_max_window_miss(int permille);
 int mvsf_warp_corr_last_selection(int* used_pipeline, int* miss_permille);
 
 /* ---- measurement hook: 1 = prefer the largest shared-memory carve-out for every kernel of the context (cudaDeviceSetCacheConfig),
- * 0 = driver default.  Used to test whether carve-out switches play a part in the two-stream deadlock (DESIGN.md 5). */
+ * 0 = driver default. */
 int mvsf_set_prefer_shared_carveout(int on);
 
 /* ---- which of the two cost-volume plans to run for a stage shape: 1 = two gathers (mvsf_warp_corr_entropy, mvsf_vis_cnn,
  * mvsf_warp_corr_aggregate; no intermediate buffer), 0 = spill plan (mvsf_warp_corr_entropy_store, mvsf_vis_cnn,
- * mvsf_corr_aggregate; needs a [(V-1)][D][H][W][8] fp32 buffer; the faster one on B200).  Both give the same volume. */
+ * mvsf_corr_aggregate; needs a [(V-1)][D][H][W][8] fp32 buffer).  Both give the same volume. */
 int mvsf_warp_corr_plan(int C, int G, int D, int H, int W, int V, size_t spill_budget_bytes);
 
 /* ---- W2+W3+W4 pass A: warp + group correlation summed over groups + softmax-entropy over D.
@@ -129,12 +129,12 @@ int mvsf_corr_aggregate(const float* corr, const float* vis, float* volume, int 
  *      :453-504 (kind 1: CostRegNet3D, stride (1,2,2), 1^3 prob + bias).  volume [D][H][W][C] -> logits [D][H][W].
  * wts: packed by packing.pack_costreg_unet (per layer [27][Cin][Cout] with BN scale folded, then bias[Cout]). */
 int mvsf_costreg_unet_workspace_bytes(int kind, int C, int D, int H, int W, size_t* bytes);
-/* install time: wts -> wts_tc, the fp16 hi/lo weight slabs of the tcgen05 implicit-GEMM convolutions (csrc/conv3d_tc.cu) */
+/* install time: wts -> wts_tc, the fp16 hi/lo weight slabs of the wgmma implicit-GEMM convolutions (csrc/conv3d_tc.cu) */
 int mvsf_costreg_unet_tc_bytes(size_t* bytes);
 int mvsf_costreg_unet_pack_tc(int kind, const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
 int mvsf_costreg_unet_forward(int kind, const float* volume, const float* wts, const void* wts_tc, float* logits,
                               void* workspace, size_t workspace_bytes, int C, int D, int H, int W, mvsf_stream_t stream);
-/* test seam: ONE 3x3x3 layer of the U-Nets on the tcgen05 implicit-GEMM path, fp32 in / out (module.py:367-504:
+/* test seam: ONE 3x3x3 layer of the U-Nets on the wgmma implicit-GEMM path, fp32 in / out (module.py:367-504:
  * Conv3d / strided Conv3d / ConvTranspose3d(output_padding = stride - 1) + folded BN + ReLU, optional skip added after the
  * ReLU).  mode 0: stride 1, 1: stride (sd,2,2), 2: transposed (sd,2,2).  in [ID][IH][IW][cin]; w32 = [27][cin][cout] then
  * bias[cout]; skip (or NULL) and out [OD][OH][OW][cout]; workspace >= 4*(nin + 2*nout) + 216*cin*max(cout,16) + 512 bytes. */
@@ -145,7 +145,7 @@ int mvsf_conv3d_tc_layer(int mode, int sd, const float* in, const float* w32, co
 /* ---- R1: models/module.py:602-646 PureTransformerCostReg (+ position_encoding.py:164-189 PositionEncoding3D).
  * volume [D][H][W][C] is modified in place by the PE add; pos [3][D][H][W] or NULL.
  * Fixed by the shipped config: down_rate (2,4,4), mid 64, heads 4, mlp 256.  softmax_scale = hd^-0.5*log_tal(N).
- * wts16 = mvsf_split_weights_f16(wts) (fp16 hi|lo parts for the tcgen05 GEMMs), n_wts = number of floats in wts. */
+ * wts16 = mvsf_split_weights_f16(wts) (fp16 hi|lo parts for the wgmma GEMMs), n_wts = number of floats in wts. */
 int mvsf_costreg_tr_workspace_bytes(int C, int D, int H, int W, size_t* bytes);
 int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, const void* wts16, size_t n_wts,
                             float* logits, void* workspace, size_t workspace_bytes, int C, int D, int H, int W,
@@ -159,13 +159,13 @@ int mvsf_split_weights_f16(const float* wts, void* out16, size_t n, mvsf_stream_
 int mvsf_attention_set_precision(int p_lo);
 
 /* softmax attention of R1 alone: models/dino/layers/attention.py:141-170 (FlashAttention2.forward after the qkv linear).
- * qkv [N][3][4][16] fp32 -> out [N][64]; workspace >= (N+128)*896 bytes.  tcgen05 tensor cores, 3-term split-fp16 operands,
- * fp32 accumulation in TMEM; |q*scale|, |k|, |v| must be < 65504. */
+ * qkv [N][3][4][16] fp32 -> out [N][64]; workspace >= (N+128)*896 bytes.  wgmma tensor cores, 3-term split-fp16 operands,
+ * fp32 accumulation in registers; |q*scale|, |k|, |v| must be < 65504. */
 int mvsf_attention_forward(const float* qkv, float* out, void* workspace, size_t workspace_bytes, int N,
                            float softmax_scale, mvsf_stream_t stream);
 
 /* token-wise linear layer alone (nn.Linear, e.g. models/module.py:520-522 FFN.linear1): C[M,N] = act(A[M,K] W[N,K]^T + bias)
- * on the tcgen05 tensor cores with fp16 hi/lo split operands (fp32-class accuracy).  N % 16 == 0, N <= 256, K % 64 == 0.
+ * on the wgmma tensor cores with fp16 hi/lo split operands (fp32-class accuracy).  N in {16, 64, 128, 192, 256}, K % 64 == 0.
  * workspace >= (M+N)*2K*2 + 256 bytes.  gelu != 0 applies the exact-erf GELU. */
 int mvsf_linear_tc_forward(const float* A, const float* W, const float* bias, float* C, void* workspace,
                            size_t workspace_bytes, int M, int N, int K, int gelu, mvsf_stream_t stream);

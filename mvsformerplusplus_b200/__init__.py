@@ -1,4 +1,4 @@
-"""B200-native depth-inference hot path of MVSFormer++ (FMT -> warp/group-correlation/visibility aggregation ->
+"""CUDA-native (H100, sm_90a) depth-inference hot path of MVSFormer++ (FMT -> warp/group-correlation/visibility aggregation ->
 cost regularisation -> soft-argmax, 4-stage cascade) behind the reference's Python seams.  See DESIGN.md."""
 from .config import default_args, load_args, validate_args  # noqa: F401
 

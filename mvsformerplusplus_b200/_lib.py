@@ -55,7 +55,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(f"{LIB_PATH} is missing: build it with `python -m mvsformerplusplus_b200.build` "
-                               "(the B200 hot path has no CPU/PyTorch fallback)")
+                               "(the hot path has no CPU/PyTorch fallback)")
         L = ctypes.CDLL(LIB_PATH)
         L.mvsf_last_error.restype = ctypes.c_char_p
         L.mvsf_last_error.argtypes = []

@@ -1,4 +1,4 @@
-"""Builds libmvsf_b200.so in-tree with nvcc for sm_100a (no torch headers involved: the library is pure CUDA
+"""Builds libmvsf_b200.so in-tree with nvcc for sm_90a (no torch headers involved: the library is pure CUDA
 runtime behind a C ABI).  Usage: python -m mvsformerplusplus_b200.build [--force] [--verbose]"""
 import hashlib
 import os
@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmvsf_b200.so")
 STAMP = os.path.join(HERE, ".libmvsf_b200.stamp")
 SOURCES = ["api.cu", "geometry.cu", "warp_corr.cu", "warp_tile.cu", "vis_cnn.cu", "costreg_unet.cu", "costreg_tr.cu", "fmt.cu", "linear_tc.cu", "conv3d_tc.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "--extended-lambda"] + os.environ.get("MVSF_EXTRA_NVCC_FLAGS", "").split()
 
 
@@ -53,7 +53,7 @@ def build(force=False, verbose=False):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed (see output above)")
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static", "-lrt", "-lpthread", "-ldl"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart_static", "-lrt", "-lpthread", "-ldl"]
     subprocess.check_call(cmd)
     with open(STAMP, "w") as f:
         f.write(dig)

@@ -51,7 +51,7 @@ def validate_args(args):
     if args.get("fusion_type", "cnn") != "cnn":
         raise NotImplementedError(f"Not implemented fusion type: {args.get('fusion_type')}.")
     if not args.get("inverse_depth", False):
-        raise NotImplementedError("B200 hot path implements the shipped inverse_depth=True scheduling only")
+        raise NotImplementedError("the hot path implements the shipped inverse_depth=True scheduling only")
     fm = args["FMT_config"]
     if fm.get("attention_type") != "Linear":
         raise NotImplementedError("Unkown attention type", fm.get("attention_type"))

@@ -32,7 +32,7 @@ int device_sm_count(int dev) {
   const int slot = dev & 63;
   int v = cache[slot].load(std::memory_order_relaxed);
   if (v <= 0) {
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     cache[slot].store(v, std::memory_order_relaxed);
   }
   return v;

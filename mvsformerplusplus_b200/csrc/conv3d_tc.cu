@@ -1,41 +1,46 @@
 // 3x3x3 convolutions of the U-Net cost regularisers (models/module.py:367-408 CostRegNet, :453-504 CostRegNet3D) as
-// implicit GEMMs on the 5th-generation tensor cores, fp32-class accuracy.
+// implicit GEMMs on the Hopper tensor cores (wgmma), fp32-class accuracy.
 //
 //   * activations live in HBM as two fp16 tensors (hi, lo; x ~= hi + lo carries 22 mantissa bits), NDHWC.  A tile is
 //     16 (h) x 8*NT (w) cells of one depth slice.  Per (input depth slice, group of KG channel octets) "unit" ONE thread
 //     issues TMA box loads (cp.async.bulk.tensor.5d over (c, w, h, d, hi|lo); the conv padding is TMA's out-of-bounds
 //     zero fill) that land the halo of the tile in shared memory as PLANES of voxel octets: plane[row][col] = 8 channels
-//     = 16 bytes.  Eight w-neighbours are then 128 contiguous bytes = one UMMA "core matrix" of the canonical no-swizzle
+//     = 16 bytes.  Eight w-neighbours are then 128 contiguous bytes = one "core matrix" of the canonical no-swizzle
 //     K-major layout, the h rows are the 8-row groups (SBO = row pitch) and hi / lo planes (or the two octets) are the
 //     two K-chunks of a K = 16 MMA (LBO = plane distance).  A filter tap (kh, kw) is nothing but a different descriptor
 //     start address: no im2col, no per-element address arithmetic anywhere;
-//   * KG = 1: per tap two tcgen05.mma.kind::f16 (M = 128 cells, N = Cout, K = 16)
+//   * an M-tile is 16 x 8 cells = 128 GEMM rows; its two m64 halves (h rows 0-7 / 8-15) belong to the two MMA warpgroups,
+//     which keep the fp32 accumulators in registers and run the epilogue themselves;
+//   * KG = 1: per tap two wgmma (M = 64 cells, N = Cout, K = 16)
 //         [x_hi | x_lo] x [w_hi ; w_hi]   and   [x_hi | x_lo] x [w_lo ; 0]       (x_lo*w_lo ~ 2^-22 is dropped)
 //     KG = 2 (16 channels per unit): K = 16 spans the two octets and three MMAs x_lo*w_hi, x_hi*w_lo, x_hi*w_hi are
-//     issued; fp32 accumulation in TMEM; the weight slabs come pre-arranged from conv3d_tc_pack and travel with the
-//     unit (one cp.async.bulk) through the same mbarrier ring (expect_tx / complete_tx);
+//     issued; the weight slabs come pre-arranged from conv3d_tc_pack and travel with the unit (one cp.async.bulk)
+//     through the same mbarrier ring (expect_tx / complete_tx);
 //   * stride-(SD,2,2) convolutions keep four parity planes (even/odd h x even/odd w, one strided tensor map each) so
 //     that every tap is again a dense plane access; transposed convolutions run in gather form over INPUT cells with
 //     four accumulators, one per output parity class (every (kh, kw) tap feeds exactly one class).  Taps that read the
-//     same input shift (dih, diw) are fused along N: the class accumulators sit in TMEM in the order [0, 1, 3, 2] so
-//     that the 4 / 2 / 2 / 1 classes fed by the shifts (0,0) / (0,1) / (1,0) / (1,1) are contiguous column ranges;
-//   * persistent, warp-specialised CTAs (one per SM, tiles strided by gridDim.x): warp 0 = TMA producer, warp 1 = MMA
-//     issuer, warps 2-9 = two epilogue warpgroups (one TMEM lane = one cell per thread: bias (folded BatchNorm), ReLU,
-//     skip add, fp16 hi|lo split or the fused 1x1x1 `prob` conv).  Rings: full[s]/empty[s] for the operand stages,
-//     accf[b]/acce[b] for the two TMEM accumulator buffers, so loads, MMAs and the epilogue of consecutive tiles overlap.
+//     same input shift (dih, diw) are fused along N: the class accumulators sit in the order [0, 1, 3, 2] so that the
+//     4 / 2 / 2 / 1 classes fed by the shifts (0,0) / (0,1) / (1,0) / (1,1) are contiguous column ranges;
+//   * persistent, warp-specialised CTAs (one per SM, tiles strided by gridDim.x): warpgroup 0 = TMA producer (one
+//     thread), warpgroups 1-2 = MMA + epilogue (bias (folded BatchNorm), ReLU, skip add, fp16 hi|lo split or the fused
+//     1x1x1 `prob` conv).  Ring: full[s] / empty[s]; each MMA warpgroup keeps one unit of MMAs in flight while it issues
+//     the next, so loads and MMAs of consecutive units overlap, and the producer runs ahead into the next tile while the
+//     epilogue of the current one runs.
 #include "conv3d_tc.cuh"
 
 #include <cuda.h>
 
+#include <type_traits>
+
 #include "linear_tc.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace mvsf {
 
-using namespace umma;
+using namespace gmma;
 
 namespace c3 {
-constexpr int NEPI = 256, THREADS = 64 + NEPI, MAX_STAGES = 8;   // warp 0: TMA, warp 1: MMA, warps 2-9: epilogue
+constexpr int THREADS = 384, MAX_STAGES = 8;   // warpgroup 0: TMA (one thread), warpgroups 1-2: MMA + epilogue
 template <int MODE, int NT>
 struct Geo {
   static constexpr int TW = 8 * NT, TH = 16;
@@ -52,18 +57,11 @@ __host__ __device__ inline uint32_t slab_bytes(int cout) { return (uint32_t)npad
 
 struct alignas(64) Maps { CUtensorMap m[4]; };   // CONV_S2: one map per (h, w) parity; otherwise m[0]
 
-__device__ __forceinline__ void expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
 // TMA tile load of a 5-D box (c, w, h, d, hi/lo); out-of-range coordinates (the conv padding) are filled with zeros
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, int c4, uint32_t bar) {
   asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
                ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
                : "memory");
-}
-__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 }  // namespace c3
 
@@ -89,97 +87,71 @@ __device__ __forceinline__ DepthTaps depth_taps(int od, int SD, int ID) {
   return t;
 }
 
-template <int MODE, int OUT>
-__device__ __forceinline__ void conv_epilogue_item(const ConvTcArgs& a, uint32_t tcol, int NPAD, bool valid, size_t vox) {
+// epilogue of one GEMM row (cell) of one accumulator: channels 8 b + 2 q, + 1 (q = lane % 4) of accumulator row half h.
+// Returns this thread's share of the fused 1x1x1 prob conv (OUT_PROB); the four threads of a quad hold one cell.
+template <int OUT, int NPAD>
+__device__ __forceinline__ float conv_epilogue_frag(const ConvTcArgs& a, const float* acc, int h, int q, bool valid, size_t vox) {
   const int COUT = a.COUT;
   float prob = 0.f;
-  for (int c16 = 0; c16 < NPAD / 16; ++c16) {
-    float v[16];
-    tmem_ld16(tcol + c16 * 16, v);
 #pragma unroll
-    for (int g = 0; g < 2; ++g) {
-      const int c0 = c16 * 16 + g * 8;
-      if (c0 >= COUT) continue;
-      float x[8];
-      const float4 b0 = ldg4(a.bias + c0), b1 = ldg4(a.bias + c0 + 4);
-      x[0] = fmaxf(v[g * 8 + 0] + b0.x, 0.f); x[1] = fmaxf(v[g * 8 + 1] + b0.y, 0.f);
-      x[2] = fmaxf(v[g * 8 + 2] + b0.z, 0.f); x[3] = fmaxf(v[g * 8 + 3] + b0.w, 0.f);
-      x[4] = fmaxf(v[g * 8 + 4] + b1.x, 0.f); x[5] = fmaxf(v[g * 8 + 5] + b1.y, 0.f);
-      x[6] = fmaxf(v[g * 8 + 6] + b1.z, 0.f); x[7] = fmaxf(v[g * 8 + 7] + b1.w, 0.f);
-      if (!valid) continue;
-      if (OUT == OUT_SPLIT) {
-        if (a.skip_hi) {
-          const uint4 sh = *reinterpret_cast<const uint4*>(a.skip_hi + vox * COUT + c0);
-          const uint4 sl = *reinterpret_cast<const uint4*>(a.skip_lo + vox * COUT + c0);
-          const __half2* h2 = reinterpret_cast<const __half2*>(&sh);
-          const __half2* l2 = reinterpret_cast<const __half2*>(&sl);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 fh = __half22float2(h2[e]), fl = __half22float2(l2[e]);
-            x[2 * e] += fh.x + fl.x;
-            x[2 * e + 1] += fh.y + fl.y;
-          }
-        }
-        split_store8(a.out_hi + vox * COUT + c0, a.out_lo + vox * COUT + c0, x);
-      } else {
-        const float4 s0 = ldg4(a.skip32 + vox * COUT + c0), s1 = ldg4(a.skip32 + vox * COUT + c0 + 4);
-        x[0] += s0.x; x[1] += s0.y; x[2] += s0.z; x[3] += s0.w;
-        x[4] += s1.x; x[5] += s1.y; x[6] += s1.z; x[7] += s1.w;
-        if (OUT == OUT_F32) {
-          float* op = a.out32 + vox * COUT + c0;
-          *reinterpret_cast<float4*>(op) = make_float4(x[0], x[1], x[2], x[3]);
-          *reinterpret_cast<float4*>(op + 4) = make_float4(x[4], x[5], x[6], x[7]);
-        } else {
-          if (c0 == 0) prob = __ldg(a.probw + COUT);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) prob = fmaf(x[e], __ldg(a.probw + c0 + e), prob);
-        }
+  for (int b = 0; b < NPAD / 8; ++b) {
+    const int c = 8 * b + 2 * q;
+    if (8 * b >= COUT) continue;
+    const float2 b2 = *reinterpret_cast<const float2*>(a.bias + c);
+    float x0 = fmaxf(acc[4 * b + 2 * h] + b2.x, 0.f), x1 = fmaxf(acc[4 * b + 2 * h + 1] + b2.y, 0.f);
+    if (!valid) continue;
+    if (OUT == OUT_SPLIT) {
+      if (a.skip_hi) {
+        const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(a.skip_hi + vox * COUT + c));
+        const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(a.skip_lo + vox * COUT + c));
+        x0 += fh.x + fl.x;
+        x1 += fh.y + fl.y;
       }
+      split_store2(a.out_hi + vox * COUT + c, a.out_lo + vox * COUT + c, x0, x1);
+    } else {
+      const float2 s2 = *reinterpret_cast<const float2*>(a.skip32 + vox * COUT + c);
+      x0 += s2.x; x1 += s2.y;
+      if (OUT == OUT_F32) *reinterpret_cast<float2*>(a.out32 + vox * COUT + c) = make_float2(x0, x1);
+      else prob = fmaf(x1, __ldg(a.probw + c + 1), x0 * __ldg(a.probw + c));
     }
   }
-  if (OUT == OUT_PROB && valid) a.out32[vox] = prob;
+  return prob;
 }
 
+template <int NREG>
+__device__ __forceinline__ void fence_acc(float (&acc)[NREG]) { fence_regs<NREG>(acc); }
+
 // Persistent kernel: CTA i works on tiles i, i + gridDim.x, ...; tile = (output depth slice, 16 x 8*NT cells).
-template <int MODE, int NT, int OUT>
+template <int MODE, int NT, int OUT, int NPAD>
 __global__ void __launch_bounds__(c3::THREADS, 1)
 conv3d_tc_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, int OD, int OH, int OW, int tiles_w,
                  int tiles_h, int ntiles) {
   using G = c3::Geo<MODE, NT>;
   constexpr int PC = G::PC, NSUB = G::NSUB;
   constexpr int NCLS = MODE == DECONV_S2 ? 4 : 1;
+  constexpr int ACC = NCLS * NPAD / 2;                            // accumulator registers per M-tile
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int CIN = a.CIN, COUT = a.COUT, SD = a.SD, ID = a.ID, IH = a.IH, IW = a.IW;
-  const int NPAD = c3::npad(COUT);
+  const int CIN = a.CIN, SD = a.SD, ID = a.ID, IH = a.IH, IW = a.IW;
   const int KG = a.KG;                                            // channel octets per unit
-  const uint32_t b_bytes = c3::slab_bytes(COUT);
+  const uint32_t b_bytes = c3::slab_bytes(NPAD);
   const uint32_t a_bytes = (uint32_t)KG * G::OCT_BYTES;
   const uint32_t stage_bytes = (a_bytes + b_bytes + 127u) / 128u * 128u;
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bars = sbase + NS * stage_bytes;                 // full[8] | empty[8] | accf[2] | acce[2] | tmem slot
-  const uint32_t bar_full = bars, bar_empty = bars + 64, bar_accf = bars + 128, bar_acce = bars + 144;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + NS * stage_bytes + 160);
+  const uint32_t bars = sbase + NS * stage_bytes;                 // full[8] | empty[8]
+  const uint32_t bar_full = bars, bar_empty = bars + 64;
   const int ngroups = (CIN >> 3) / KG;
-  const uint32_t acc_cols = (uint32_t)(NT * NCLS * NPAD);         // one accumulator buffer
 
-  uint32_t ncols = 32;
-  while (ncols < 2 * acc_cols) ncols <<= 1;
   if (tid == 0) {
-    for (int i = 0; i < c3::MAX_STAGES; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 1); }
-    mbar_init(bar_accf, 1); mbar_init(bar_accf + 8, 1);
-    mbar_init(bar_acce, c3::NEPI); mbar_init(bar_acce + 8, c3::NEPI);
+    for (int i = 0; i < c3::MAX_STAGES; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 2); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), ncols);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // --------------------------------------------------------------------------------------- TMA producer
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");   // registers go to the accumulators of the MMA warpgroups
+    if (tid == 0) {
       uint32_t g = 0;
       for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int tw = tile % tiles_w, th = (tile / tiles_w) % tiles_h, od = tile / (tiles_w * tiles_h);
@@ -190,7 +162,7 @@ conv3d_tc_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, in
             const int s = g % NS;
             mbar_wait(bar_empty + 8 * s, (uint32_t)(((g / NS) & 1) ^ 1));
             const uint32_t st = sbase + s * stage_bytes, full = bar_full + 8 * s;
-            c3::expect_tx(full, (uint32_t)(KG * NSUB) * 2u * G::SUB_BYTES + b_bytes);
+            expect_tx(full, (uint32_t)(KG * NSUB) * 2u * G::SUB_BYTES + b_bytes);
             for (int og = 0; og < KG; ++og) {
               const int c = (grp * KG + og) * 8;
 #pragma unroll
@@ -202,130 +174,124 @@ conv3d_tc_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, in
                 c3::tma_load_5d(st + (uint32_t)(og * NSUB + sub) * G::PAIR, &maps.m[sub], c, w0, h0, dt.id[ds], 0, full);
               }
             }
-            c3::bulk_load(st + a_bytes, a.wtc + (size_t)(dt.kd[ds] * ngroups + grp) * (b_bytes / 2), b_bytes, full);
+            bulk_load(st + a_bytes, a.wtc + (size_t)(dt.kd[ds] * ngroups + grp) * (b_bytes / 2), b_bytes, full);
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // --------------------------------------------------------------------------------------- MMA issue
-    {   // converged warp, one elected lane per tcgen05 instruction (see conv3d_col_kernel)
-      const uint32_t blk = (uint32_t)NPAD * 32u;   // one weight block: NPAD rows x 2 k-chunks
-      uint32_t g = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const int od = tile / (tiles_w * tiles_h);
-        const DepthTaps dt = depth_taps<MODE>(od, SD, ID);
-        const int U = dt.n * ngroups;
-        const int buf = it & 1;
-        mbar_wait(bar_acce + 8 * buf, (uint32_t)(((it >> 1) & 1) ^ 1));   // the epilogue has drained this accumulator buffer
-        tc_fence_after_sync();
-        const uint32_t tacc0 = tmem_base + (uint32_t)buf * acc_cols;
-        for (int u = 0; u < U; ++u, ++g) {
-          const int s = g % NS;
-          mbar_wait(bar_full + 8 * s, (uint32_t)((g / NS) & 1));
-          tc_fence_after_sync();
-          const uint32_t sA = sbase + s * stage_bytes, sB = sA + a_bytes;
-          // one fused tap group: A start offset, first weight block, number of blocks (N = nb * NPAD), accumulator column
-          auto issue = [&](uint32_t aoff, int bstart, int nb, int dcol, bool overwrite) {
-            const uint32_t n = (uint32_t)(nb * NPAD);
-            const uint32_t idesc = make_idesc_f16(128, (int)n);
-            const uint32_t t0 = sB + (uint32_t)bstart * 2u * blk, t1 = t0 + (uint32_t)nb * blk;
-            const uint64_t b0 = make_desc(t0, n * 16u, 128), b1 = make_desc(t1, n * 16u, 128);
-            // consecutive MMAs go to different accumulators (M-tiles): back-to-back MMAs on one accumulator serialise
-            if (KG == 1) {
-#pragma unroll
-              for (int t = 0; t < NT; ++t)                                                       // K = [hi | lo] of one octet
-                mma_f16_ss_elect(tacc0 + (uint32_t)(t * NCLS * NPAD + dcol), make_desc(sA + aoff + t * 128, G::SUB_BYTES, G::PITCH), b0,
-                           idesc, overwrite ? 0u : 1u);                                        // x [w_hi ; w_hi]
-#pragma unroll
-              for (int t = 0; t < NT; ++t)
-                mma_f16_ss_elect(tacc0 + (uint32_t)(t * NCLS * NPAD + dcol), make_desc(sA + aoff + t * 128, G::SUB_BYTES, G::PITCH), b1,
-                           idesc, 1u);                                                         // x [w_lo ; 0]
-            } else {
-#pragma unroll
-              for (int t = 0; t < NT; ++t)                                                       // K = two octets; lo planes
-                mma_f16_ss_elect(tacc0 + (uint32_t)(t * NCLS * NPAD + dcol),
-                           make_desc(sA + G::SUB_BYTES + aoff + t * 128, G::OCT_BYTES, G::PITCH), b0, idesc, overwrite ? 0u : 1u);  // x_lo * w_hi
-#pragma unroll
-              for (int t = 0; t < NT; ++t)
-                mma_f16_ss_elect(tacc0 + (uint32_t)(t * NCLS * NPAD + dcol), make_desc(sA + aoff + t * 128, G::OCT_BYTES, G::PITCH), b1,
-                           idesc, 1u);                                                         // x_hi * w_lo
-#pragma unroll
-              for (int t = 0; t < NT; ++t)
-                mma_f16_ss_elect(tacc0 + (uint32_t)(t * NCLS * NPAD + dcol), make_desc(sA + aoff + t * 128, G::OCT_BYTES, G::PITCH), b0,
-                           idesc, 1u);                                                         // x_hi * w_hi
-            }
-          };
-          if (MODE == DECONV_S2) {
-            // input shift (dih, diw) -> fused classes; weight blocks in conv3d_tc_pack's order
-            issue(0u, 0, 4, 0, u == 0);                                   // (0,0): taps (1,1) (1,2) (2,2) (2,1) -> classes 0 1 3 2
-            issue(16u, 4, 2, NPAD, false);                                // (0,1): taps (1,0) (2,0)             -> classes 1 3
-            issue((uint32_t)PC * 16u, 6, 2, 2 * NPAD, false);             // (1,0): taps (0,2) (0,1)             -> classes 3 2
-            issue((uint32_t)(PC + 1) * 16u, 8, 1, 2 * NPAD, false);       // (1,1): tap  (0,0)                   -> class 3
-          } else {
-#pragma unroll
-            for (int kh = 0; kh < 3; ++kh) {
-#pragma unroll
-              for (int kw = 0; kw < 3; ++kw) {
-                int sub = 0, rs = kh, cs = kw;
-                if (MODE == CONV_S2) {
-                  sub = (kh == 1 ? 0 : 2) + (kw == 1 ? 0 : 1);
-                  rs = kh == 2 ? 1 : 0; cs = kw == 2 ? 1 : 0;
-                }
-                issue((uint32_t)sub * G::PAIR + (uint32_t)(rs * PC + cs) * 16u, kh * 3 + kw, 1, 0, u == 0 && kh == 0 && kw == 0);
-              }
-            }
-          }
-          commit_elect(bar_empty + 8 * s);
-        }
-        commit_elect(bar_accf + 8 * buf);
-      }
-    }
-  } else {
-    // --------------------------------------------------------------------------------------- epilogue (2 warpgroups)
-    const int wg = (warp - 2) >> 2, quarter = warp & 3;   // a warp may only touch TMEM lanes 32 * (warp % 4) ...
-    const int m = quarter * 32 + lane;                    // TMEM lane = GEMM row = cell (h = m / 8, w = m % 8) of an M-tile
-    int it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int tw = tile % tiles_w, th = (tile / tiles_w) % tiles_h, od = tile / (tiles_w * tiles_h);
-      const int buf = it & 1;
-      mbar_wait(bar_accf + 8 * buf, (uint32_t)((it >> 1) & 1));
-      tc_fence_after_sync();
-      const uint32_t trow = tmem_base + (uint32_t)buf * acc_cols + ((uint32_t)(quarter * 32) << 16);
-      const int ch = th * 16 + (m >> 3);
-#pragma unroll 1
-      for (int item = wg; item < NT * NCLS; item += 2) {
-        const int t = item / NCLS, cls = item % NCLS;
-        const int cw = tw * G::TW + t * 8 + (m & 7);
-        int oh, ow;
-        bool valid;
-        if (MODE == DECONV_S2) { oh = 2 * ch + (cls >> 1); ow = 2 * cw + (cls & 1); valid = ch < IH && cw < IW; }
-        else { oh = ch; ow = cw; valid = ch < OH && cw < OW; }
-        const size_t vox = valid ? ((size_t)od * OH + oh) * OW + ow : 0;
-        const uint32_t tcol = trow + (uint32_t)((t * NCLS + (cls ^ (cls >> 1))) * NPAD);   // class order [0, 1, 3, 2]
-        conv_epilogue_item<MODE, OUT>(a, tcol, NPAD, valid, vox);
-      }
-      tc_fence_before_sync();
-      mbar_arrive(bar_acce + 8 * buf);
-    }
+    return;
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, ncols);
+  // ----------------------------------------------------------------------------------------- MMA + epilogue warpgroups
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int half = (warp >> 2) - 1, wq = warp & 3, q = lane & 3, t128 = tid & 127;
+  const uint32_t blk = (uint32_t)NPAD * 32u;   // one weight block: NPAD rows x 2 k-chunks
+  float acc[NT][ACC];
+  auto release = [&](uint32_t gb) { if (t128 == 0) mbar_arrive(bar_empty + 8 * (gb % NS)); };
+  uint32_t g = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int tw = tile % tiles_w, th = (tile / tiles_w) % tiles_h, od = tile / (tiles_w * tiles_h);
+    const DepthTaps dt = depth_taps<MODE>(od, SD, ID);
+    const int U = dt.n * ngroups;
+    int pend = -1;
+    for (int u = 0; u < U; ++u, ++g) {
+      const int s = g % NS;
+      mbar_wait(bar_full + 8 * s, (uint32_t)((g / NS) & 1));
+      const uint32_t sA = sbase + s * stage_bytes + (uint32_t)half * 8u * G::PITCH, sB = sbase + s * stage_bytes + a_bytes;
+      // one fused tap group: A start offset, first weight block, NB blocks (N = NB * NPAD), first accumulator column
+      auto issue = [&](auto nb_c, uint32_t aoff, int bstart, auto dcol_c, bool overwrite) {
+        constexpr int NB = decltype(nb_c)::value, DCOL = decltype(dcol_c)::value;
+        constexpr uint32_t n = (uint32_t)(NB * NPAD);
+        const uint32_t t0 = sB + (uint32_t)bstart * 2u * blk, t1 = t0 + (uint32_t)NB * blk;
+        const uint64_t b0 = make_desc(t0, n * 16u, 128), b1 = make_desc(t1, n * 16u, 128);
+        // consecutive MMAs go to different accumulators (M-tiles): back-to-back MMAs on one accumulator serialise
+        if (KG == 1) {
+#pragma unroll
+          for (int t = 0; t < NT; ++t)                                                       // K = [hi | lo] of one octet
+            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + aoff + t * 128, G::SUB_BYTES, G::PITCH), b0, overwrite ? 0u : 1u);  // x [w_hi ; w_hi]
+#pragma unroll
+          for (int t = 0; t < NT; ++t)
+            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + aoff + t * 128, G::SUB_BYTES, G::PITCH), b1, 1u);                 // x [w_lo ; 0]
+        } else {
+#pragma unroll
+          for (int t = 0; t < NT; ++t)                                                       // K = two octets; lo planes
+            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + G::SUB_BYTES + aoff + t * 128, G::OCT_BYTES, G::PITCH), b0, overwrite ? 0u : 1u);  // x_lo * w_hi
+#pragma unroll
+          for (int t = 0; t < NT; ++t)
+            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + aoff + t * 128, G::OCT_BYTES, G::PITCH), b1, 1u);                 // x_hi * w_lo
+#pragma unroll
+          for (int t = 0; t < NT; ++t)
+            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + aoff + t * 128, G::OCT_BYTES, G::PITCH), b0, 1u);                 // x_hi * w_hi
+        }
+      };
+      using I1 = std::integral_constant<int, 1>;
+      using I0 = std::integral_constant<int, 0>;
+      wg_fence();
+      if constexpr (MODE == DECONV_S2) {
+        // input shift (dih, diw) -> fused classes; weight blocks in conv3d_tc_pack's order
+        issue(std::integral_constant<int, 4>{}, 0u, 0, I0{}, u == 0);                                              // (0,0): taps (1,1) (1,2) (2,2) (2,1) -> classes 0 1 3 2
+        issue(std::integral_constant<int, 2>{}, 16u, 4, std::integral_constant<int, NPAD>{}, false);                // (0,1): taps (1,0) (2,0)             -> classes 1 3
+        issue(std::integral_constant<int, 2>{}, (uint32_t)PC * 16u, 6, std::integral_constant<int, 2 * NPAD>{}, false);        // (1,0): taps (0,2) (0,1) -> classes 3 2
+        issue(I1{}, (uint32_t)(PC + 1) * 16u, 8, std::integral_constant<int, 2 * NPAD>{}, false);                  // (1,1): tap  (0,0)                   -> class 3
+      } else {
+#pragma unroll
+        for (int kh = 0; kh < 3; ++kh) {
+#pragma unroll
+          for (int kw = 0; kw < 3; ++kw) {
+            int sub = 0, rs = kh, cs = kw;
+            if (MODE == CONV_S2) {
+              sub = (kh == 1 ? 0 : 2) + (kw == 1 ? 0 : 1);
+              rs = kh == 2 ? 1 : 0; cs = kw == 2 ? 1 : 0;
+            }
+            issue(I1{}, (uint32_t)sub * G::PAIR + (uint32_t)(rs * PC + cs) * 16u, kh * 3 + kw, I0{}, u == 0 && kh == 0 && kw == 0);
+          }
+        }
+      }
+      wg_commit();
+      if (pend >= 0) {
+        wg_wait<1>();
+        release((uint32_t)pend);
+      }
+      pend = (int)g;
+    }
+    wg_wait<0>();
+#pragma unroll
+    for (int t = 0; t < NT; ++t) fence_acc(acc[t]);
+    release((uint32_t)pend);
+    // ---- epilogue: GEMM row 64 half + 16 wq + lane / 4 + 8 h = cell (h = 8 half + 2 wq + h, w = lane / 4) of an M-tile
+#pragma unroll
+    for (int t = 0; t < NT; ++t)
+#pragma unroll
+      for (int cls = 0; cls < NCLS; ++cls)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int ch = th * 16 + 8 * half + 2 * wq + h;
+          const int cw = tw * G::TW + t * 8 + (lane >> 2);
+          int oh, ow;
+          bool valid;
+          if (MODE == DECONV_S2) { oh = 2 * ch + (cls >> 1); ow = 2 * cw + (cls & 1); valid = ch < IH && cw < IW; }
+          else { oh = ch; ow = cw; valid = ch < OH && cw < OW; }
+          const size_t vox = valid ? ((size_t)od * OH + oh) * OW + ow : 0;
+          float prob = conv_epilogue_frag<OUT, NPAD>(a, acc[t] + (cls ^ (cls >> 1)) * (NPAD / 2), h, q, valid, vox);   // class order [0, 1, 3, 2]
+          if (OUT == OUT_PROB) {
+            prob += __shfl_xor_sync(0xffffffffu, prob, 1);
+            prob += __shfl_xor_sync(0xffffffffu, prob, 2);
+            if (q == 0 && valid) a.out32[vox] = prob + __ldg(a.probw + a.COUT);
+          }
+        }
+  }
 }
 
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Depth-streaming variant for layers whose DEPTH stride is 1 (every 3x3x3 conv of CostRegNet3D, the stride-1 convs of
-// CostRegNet).  The MMAs above are bound by the shared-memory read of the A operand (4 KB per instruction whatever N is),
-// so instead of visiting an input slice three times - once per output slice it feeds - a work item is a COLUMN: a tile
-// x a run of output depth slices [d0, d1).  Input slice `id` is loaded ONCE and one MMA per tap multiplies it with
-// [W(kd=2) ; W(kd=1) ; W(kd=0)] (N = 3 * Cout), feeding the accumulators of the output slices id-1, id, id+1 at once.
-// The accumulators live in a ring of 4 TMEM slots per M-tile (slot = od % 4, consecutive slots are contiguous columns,
-// a window that wraps is issued as two MMAs); slice id-1 is complete once the MMAs of input slice id have retired and is
-// drained by the epilogue warps while the next input slice is multiplied.  3x fewer A-operand reads and TMA bytes.
-template <int MODE, int NT>
+// CostRegNet).  The MMAs above are bound by the shared-memory read of the A operand, so instead of visiting an input
+// slice three times - once per output slice it feeds - a work item is a COLUMN: a tile x a run of output depth slices
+// [d0, d1).  Input slice `id` is loaded ONCE and one MMA per tap multiplies it with [W(kd=2) ; W(kd=1) ; W(kd=0)]
+// (N = 3 * Cout), feeding the accumulators of the output slices id-1, id, id+1 at once.  The accumulators live in a ring
+// of 4 slots per M-tile (slot = od % 4, consecutive slots are contiguous registers, a window that wraps is issued as two
+// MMAs); slice id-1 is complete once the MMAs of input slice id have retired and goes through the epilogue before the
+// next input slice is multiplied.  3x fewer A-operand reads and TMA bytes.
+template <int MODE, int NT, int NPAD>
 __global__ void __launch_bounds__(c3::THREADS, 1)
 conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, int wres, int OH, int OW, int tiles_w,
                   int tiles_h, int DC, int nitems) {
@@ -333,8 +299,7 @@ conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, i
   constexpr int PC = G::PC, NSUB = G::NSUB;
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int CIN = a.CIN, COUT = a.COUT, D = a.ID;
-  const int NPAD = c3::npad(COUT);
+  const int CIN = a.CIN, D = a.ID;
   const int KG = a.KG;
   const int ngroups = (CIN >> 3) / KG;
   const uint32_t slab = (uint32_t)NPAD * 1728u;                   // 9 taps x 2 variants x (2 k-chunks x 3*NPAD rows x 16 B)
@@ -343,31 +308,24 @@ conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, i
   const uint32_t sbase = smem_u32(smem);
   const uint32_t wbase = sbase;                                   // resident weight slabs (wres)
   const uint32_t ring = sbase + (wres ? ((uint32_t)ngroups * slab + 127u) / 128u * 128u : 0u);
-  const uint32_t bars = ring + NS * stage_bytes;                  // full[8] | empty[8] | accf[4] | acce[4] | wbar | tmem slot
-  const uint32_t bar_full = bars, bar_empty = bars + 64, bar_accf = bars + 128, bar_acce = bars + 160, bar_w = bars + 192;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + (bars - sbase) + 200);
+  const uint32_t bars = ring + NS * stage_bytes;                  // full[8] | empty[8] | wbar
+  const uint32_t bar_full = bars, bar_empty = bars + 64, bar_w = bars + 128;
 
-  uint32_t ncols = 32;
-  while (ncols < (uint32_t)(4 * NT * NPAD)) ncols <<= 1;
   if (tid == 0) {
-    for (int i = 0; i < c3::MAX_STAGES; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 1); }
-    for (int i = 0; i < 4; ++i) { mbar_init(bar_accf + 8 * i, 1); mbar_init(bar_acce + 8 * i, c3::NEPI); }
+    for (int i = 0; i < c3::MAX_STAGES; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 2); }
     mbar_init(bar_w, 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), ncols);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   const int tiles_hw = tiles_w * tiles_h;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // --------------------------------------------------------------------------------------- TMA producer
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (tid == 0) {
       if (wres) {
-        c3::expect_tx(bar_w, (uint32_t)ngroups * slab);
-        for (int grp = 0; grp < ngroups; ++grp) c3::bulk_load(wbase + grp * slab, a.wtc + (size_t)grp * (slab / 2), slab, bar_w);
+        expect_tx(bar_w, (uint32_t)ngroups * slab);
+        for (int grp = 0; grp < ngroups; ++grp) bulk_load(wbase + grp * slab, a.wtc + (size_t)grp * (slab / 2), slab, bar_w);
       }
       uint32_t g = 0;
       for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
@@ -380,7 +338,7 @@ conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, i
             const int s = g % NS;
             mbar_wait(bar_empty + 8 * s, (uint32_t)(((g / NS) & 1) ^ 1));
             const uint32_t st = ring + s * stage_bytes, full = bar_full + 8 * s;
-            c3::expect_tx(full, (uint32_t)(KG * NSUB) * 2u * G::SUB_BYTES + (wres ? 0u : slab));
+            expect_tx(full, (uint32_t)(KG * NSUB) * 2u * G::SUB_BYTES + (wres ? 0u : slab));
             for (int og = 0; og < KG; ++og) {
               const int c = (grp * KG + og) * 8;
 #pragma unroll
@@ -391,117 +349,123 @@ conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, i
                 c3::tma_load_5d(st + (uint32_t)(og * NSUB + sub) * G::PAIR, &maps.m[sub], c, w0, h0, id, 0, full);
               }
             }
-            if (!wres) c3::bulk_load(st + a_bytes, a.wtc + (size_t)grp * (slab / 2), slab, full);
+            if (!wres) bulk_load(st + a_bytes, a.wtc + (size_t)grp * (slab / 2), slab, full);
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // --------------------------------------------------------------------------------------- MMA issue
-    // The whole warp runs this code converged (every value is warp-uniform and lives in uniform registers); one elected
-    // lane issues each tcgen05 instruction.  An `if (lane == 0)` version costs ~20 instructions per MMA (per-instruction
-    // divergence handling + register -> uniform register moves) and the issuing thread is the bottleneck of the kernel.
-    {
-      if (wres) mbar_wait(bar_w, 0u);
-      const uint32_t btile = (uint32_t)NPAD * 96u;    // one (tap, variant) weight tile: 2 k-chunks x 3*NPAD rows x 16 B
-      const uint32_t blbo = (uint32_t)NPAD * 48u;     // k-chunk stride inside a weight tile
-      uint32_t g = 0, pm = 0;                         // pm bit s: parity of the number of completed uses of slot s
-      for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
-        const int ck = item / tiles_hw;
-        const int d0 = ck * DC, d1 = min(D, d0 + DC);
-        const int first_id = max(d0 - 1, 0), last_id = min(d1, D - 1);
-        for (int id = first_id; id <= last_id; ++id) {
-          const int oa = max(id - 1, d0), ob = min(id + 1, d1 - 1);       // output slices fed by this input slice
-          const int fa = id == first_id ? oa : id + 1;                    // [fa, ob]: slices that receive their FIRST contribution
-          for (int od = fa; od <= ob; ++od) mbar_wait(bar_acce + 8 * (od & 3), ((pm >> (od & 3)) & 1u) ^ 1u);  // slot drained
-          tc_fence_after_sync();
-          for (int grp = 0; grp < ngroups; ++grp, ++g) {
-            const int s = g % NS;
-            mbar_wait(bar_full + 8 * s, (uint32_t)((g / NS) & 1));
-            tc_fence_after_sync();
-            const uint32_t sA = ring + s * stage_bytes;
-            const uint32_t sB = wres ? wbase + grp * slab : sA + a_bytes;
-            // MMAs of one (tap, variant) over the output slices [x, y]; a window that wraps around the 4-slot ring is split
-            auto mma_range = [&](int x, int y, bool overwrite, uint32_t astart, uint32_t albo, uint32_t tile) {
-              while (x <= y) {
-                const int sx = x & 3;
-                const int len = min(y - x + 1, 4 - sx);
-                const uint32_t n = (uint32_t)(len * NPAD);
-                const uint32_t idesc = make_idesc_f16(128, (int)n);
-                const uint64_t bd = make_desc(tile + (uint32_t)((x - id + 1) * NPAD) * 16u, blbo, 128);
+    return;
+  }
+  // ----------------------------------------------------------------------------------------- MMA + epilogue warpgroups
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int half = (warp >> 2) - 1, wq = warp & 3, q = lane & 3, t128 = tid & 127;
+  if (wres) mbar_wait(bar_w, 0u);
+  constexpr uint32_t btile = (uint32_t)NPAD * 96u;    // one (tap, variant) weight tile: 2 k-chunks x 3*NPAD rows x 16 B
+  constexpr uint32_t blbo = (uint32_t)NPAD * 48u;     // k-chunk stride inside a weight tile
+  float acc[NT][4 * NPAD / 2];                        // [M-tile][slot 0..3 x NPAD columns]
+  auto release = [&](uint32_t gb) { if (t128 == 0) mbar_arrive(bar_empty + 8 * (gb % NS)); };
+  auto epilogue = [&](int od, int th, int tw) {       // output slice od (slot od % 4) is complete
+    const int slot = od & 3;
 #pragma unroll
-                for (int t = 0; t < NT; ++t)
-                  mma_f16_ss_elect(tmem_base + (uint32_t)((t * 4 + sx) * NPAD), make_desc(astart + t * 128, albo, G::PITCH), bd, idesc,
-                                   overwrite ? 0u : 1u);
-                x += len;
-              }
-            };
+    for (int sl = 0; sl < 4; ++sl) {
+      if (sl != slot) continue;
 #pragma unroll
-            for (int kh = 0; kh < 3; ++kh) {
+      for (int t = 0; t < NT; ++t)
 #pragma unroll
-              for (int kw = 0; kw < 3; ++kw) {
-                int sub = 0, rs = kh, cs = kw;
-                if (MODE == CONV_S2) {
-                  sub = (kh == 1 ? 0 : 2) + (kw == 1 ? 0 : 1);
-                  rs = kh == 2 ? 1 : 0; cs = kw == 2 ? 1 : 0;
-                }
-                const uint32_t aoff = sA + (uint32_t)sub * G::PAIR + (uint32_t)(rs * PC + cs) * 16u;
-                const uint32_t t0 = sB + (uint32_t)(kh * 3 + kw) * 2u * btile, t1 = t0 + btile;   // w_hi tile, w_lo tile
-                const bool first = grp == 0 && kh == 0 && kw == 0;
-                // variant list: (A start, A k-chunk stride, weight tile)
-                const uint32_t va[3] = {KG == 1 ? aoff : aoff + G::SUB_BYTES, KG == 1 ? aoff : aoff, aoff};
-                const uint32_t vl = KG == 1 ? G::SUB_BYTES : G::OCT_BYTES;
-                const uint32_t vt[3] = {t0, t1, t0};
-                const int nv = KG == 1 ? 2 : 3;     // KG 1: x [w_hi;w_hi], x [w_lo;0]   KG 2: x_lo*w_hi, x_hi*w_lo, x_hi*w_hi
+        for (int h = 0; h < 2; ++h) {
+          const int ch = th * 16 + 8 * half + 2 * wq + h;
+          const int cw = tw * G::TW + t * 8 + (lane >> 2);
+          const bool valid = ch < OH && cw < OW;
+          const size_t vox = valid ? ((size_t)od * OH + ch) * OW + cw : 0;
+          conv_epilogue_frag<OUT_SPLIT, NPAD>(a, acc[t] + sl * (NPAD / 2), h, q, valid, vox);
+        }
+    }
+  };
+  uint32_t g = 0;
+  for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
+    const int tw = item % tiles_w, th = (item / tiles_w) % tiles_h, ck = item / tiles_hw;
+    const int d0 = ck * DC, d1 = min(D, d0 + DC);
+    const int first_id = max(d0 - 1, 0), last_id = min(d1, D - 1);
+    for (int id = first_id; id <= last_id; ++id) {
+      const int oa = max(id - 1, d0), ob = min(id + 1, d1 - 1);       // output slices fed by this input slice
+      const int fa = id == first_id ? oa : id + 1;                    // [fa, ob]: slices that receive their FIRST contribution
+      int pend = -1;
+      for (int grp = 0; grp < ngroups; ++grp, ++g) {
+        const int s = g % NS;
+        mbar_wait(bar_full + 8 * s, (uint32_t)((g / NS) & 1));
+        const uint32_t sA = ring + s * stage_bytes + (uint32_t)half * 8u * G::PITCH;
+        const uint32_t sB = wres ? wbase + grp * slab : ring + s * stage_bytes + a_bytes;
+        // MMAs of one (tap, variant) over the output slices [x, y]; a window that wraps around the 4-slot ring is split.
+        // Accumulator registers must be indexed statically: the (first slot, length) pair selects one unrolled case.
+        auto mma_range = [&](int x, int y, bool overwrite, uint32_t astart, uint32_t albo, uint32_t tile) {
+          while (x <= y) {
+            const int sx = x & 3;
+            const int len = min(y - x + 1, 4 - sx);
+            const uint64_t bd = make_desc(tile + (uint32_t)((x - id + 1) * NPAD) * 16u, blbo, 128);
+            const uint32_t accf = overwrite ? 0u : 1u;
 #pragma unroll
-                for (int v = 0; v < 3; ++v) {
-                  if (v >= nv) break;
-                  if (first && v == 0) {
-                    if (fa > oa) mma_range(oa, fa - 1, false, va[v], vl, vt[v]);
-                    if (fa <= ob) mma_range(fa, ob, true, va[v], vl, vt[v]);
-                  } else {
-                    mma_range(oa, ob, false, va[v], vl, vt[v]);
-                  }
+            for (int c0 = 0; c0 < 4; ++c0) {
+#pragma unroll
+              for (int ln = 1; ln <= 3; ++ln) {
+                if (c0 + ln > 4 || c0 != sx || ln != len) continue;
+#pragma unroll
+                for (int t = 0; t < NT; ++t) {
+                  const uint64_t ad = make_desc(astart + t * 128, albo, G::PITCH);
+                  float* d = acc[t] + c0 * (NPAD / 2);
+                  if (ln == 1) mma_ss<NPAD>(d, ad, bd, accf);
+                  else if (ln == 2) mma_ss<2 * NPAD>(d, ad, bd, accf);
+                  else mma_ss<3 * NPAD>(d, ad, bd, accf);
                 }
               }
             }
-            commit_elect(bar_empty + 8 * s);
+            x += len;
           }
-          if (id - 1 >= d0) { commit_elect(bar_accf + 8 * ((id - 1) & 3)); pm ^= 1u << ((id - 1) & 3); }
-          if (id == last_id && id <= d1 - 1) { commit_elect(bar_accf + 8 * (id & 3)); pm ^= 1u << (id & 3); }
+        };
+        wg_fence();
+#pragma unroll
+        for (int kh = 0; kh < 3; ++kh) {
+#pragma unroll
+          for (int kw = 0; kw < 3; ++kw) {
+            int sub = 0, rs = kh, cs = kw;
+            if (MODE == CONV_S2) {
+              sub = (kh == 1 ? 0 : 2) + (kw == 1 ? 0 : 1);
+              rs = kh == 2 ? 1 : 0; cs = kw == 2 ? 1 : 0;
+            }
+            const uint32_t aoff = sA + (uint32_t)sub * G::PAIR + (uint32_t)(rs * PC + cs) * 16u;
+            const uint32_t t0 = sB + (uint32_t)(kh * 3 + kw) * 2u * btile, t1 = t0 + btile;   // w_hi tile, w_lo tile
+            const bool first = grp == 0 && kh == 0 && kw == 0;
+            // variant list: (A start, A k-chunk stride, weight tile)
+            const uint32_t va[3] = {KG == 1 ? aoff : aoff + G::SUB_BYTES, KG == 1 ? aoff : aoff, aoff};
+            const uint32_t vl = KG == 1 ? G::SUB_BYTES : G::OCT_BYTES;
+            const uint32_t vt[3] = {t0, t1, t0};
+            const int nv = KG == 1 ? 2 : 3;     // KG 1: x [w_hi;w_hi], x [w_lo;0]   KG 2: x_lo*w_hi, x_hi*w_lo, x_hi*w_hi
+#pragma unroll
+            for (int v = 0; v < 3; ++v) {
+              if (v >= nv) break;
+              if (first && v == 0) {
+                if (fa > oa) mma_range(oa, fa - 1, false, va[v], vl, vt[v]);
+                if (fa <= ob) mma_range(fa, ob, true, va[v], vl, vt[v]);
+              } else {
+                mma_range(oa, ob, false, va[v], vl, vt[v]);
+              }
+            }
+          }
         }
-      }
-    }
-  } else {
-    // --------------------------------------------------------------------------------------- epilogue (2 warpgroups)
-    const int wg = (warp - 2) >> 2, quarter = warp & 3;
-    const int m = quarter * 32 + lane;
-    uint32_t pm = 0;
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
-      const int tw = item % tiles_w, th = (item / tiles_w) % tiles_h, ck = item / tiles_hw;
-      const int d0 = ck * DC, d1 = min(D, d0 + DC);
-      const int ch = th * 16 + (m >> 3);
-      for (int od = d0; od < d1; ++od) {
-        const int slot = od & 3;
-        mbar_wait(bar_accf + 8 * slot, (pm >> slot) & 1u);
-        pm ^= 1u << slot;
-        tc_fence_after_sync();
-        const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16);
-#pragma unroll 1
-        for (int t = wg; t < NT; t += 2) {
-          const int cw = tw * G::TW + t * 8 + (m & 7);
-          const bool valid = ch < OH && cw < OW;
-          const size_t vox = valid ? ((size_t)od * OH + ch) * OW + cw : 0;
-          conv_epilogue_item<MODE, OUT_SPLIT>(a, trow + (uint32_t)((t * 4 + slot) * NPAD), NPAD, valid, vox);
+        wg_commit();
+        if (pend >= 0) {
+          wg_wait<1>();
+          release((uint32_t)pend);
         }
-        tc_fence_before_sync();
-        mbar_arrive(bar_acce + 8 * slot);
+        pend = (int)g;
       }
+      wg_wait<0>();
+#pragma unroll
+      for (int t = 0; t < NT; ++t) fence_acc(acc[t]);
+      release((uint32_t)pend);
+      if (id - 1 >= d0) epilogue(id - 1, th, tw);
+      if (id == last_id && id <= d1 - 1) epilogue(id, th, tw);
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, ncols);
 }
 
 // ------------------------------------------------------------------------------------------------------- host
@@ -645,11 +609,11 @@ static int make_map(CUtensorMap* m, const __half* hi, const __half* lo, int C, i
   return MVSF_OK;
 }
 
-template <int MODE, int NT, int OUT>
+template <int MODE, int NT, int OUT, int NPAD>
 static int launch_one(const ConvTcArgs& a, int NS, size_t smem, int OD, int OH, int OW, int cells_h, int cells_w,
                       int num_sms, cudaStream_t s) {
   using G = c3::Geo<MODE, NT>;
-  auto kern = conv3d_tc_kernel<MODE, NT, OUT>;
+  auto kern = conv3d_tc_kernel<MODE, NT, OUT, NPAD>;
   static DeviceOnce once;
   const int dev = current_device();
   if (once.need(dev)) {
@@ -674,6 +638,18 @@ static int launch_one(const ConvTcArgs& a, int NS, size_t smem, int OD, int OH, 
   return MVSF_OK;
 }
 
+// accumulator registers per MMA thread: NT x NCLS x NPAD / 2 <= 128
+template <int MODE, int OUT, int NPAD>
+static int launch_nt(const ConvTcArgs& a, int nt, int NS, size_t smem, int OD, int OH, int OW, int cells_h, int cells_w,
+                     int num_sms, cudaStream_t s) {
+  constexpr int NCLS = MODE == DECONV_S2 ? 4 : 1;
+  if constexpr (4 * NCLS * NPAD <= 256)
+    if (nt == 4) return launch_one<MODE, 4, OUT, NPAD>(a, NS, smem, OD, OH, OW, cells_h, cells_w, num_sms, s);
+  if constexpr (2 * NCLS * NPAD <= 256)
+    if (nt == 2) return launch_one<MODE, 2, OUT, NPAD>(a, NS, smem, OD, OH, OW, cells_h, cells_w, num_sms, s);
+  return launch_one<MODE, 1, OUT, NPAD>(a, NS, smem, OD, OH, OW, cells_h, cells_w, num_sms, s);
+}
+
 template <int MODE, int OUT>
 static int launch_mode(const ConvTcArgs& a, cudaStream_t s) {
   int OD, OH, OW, cells_h, cells_w;
@@ -684,7 +660,8 @@ static int launch_mode(const ConvTcArgs& a, cudaStream_t s) {
   const int NPAD = c3::npad(a.COUT);
   const uint32_t b_bytes = c3::slab_bytes(a.COUT);
   const int ncls = MODE == DECONV_S2 ? 4 : 1;
-  // tile width: the widest tile (least halo) whose two accumulator buffers fit TMEM and that keeps the persistent CTAs busy
+  // tile width: the widest tile (least halo) whose accumulators fit the registers of the MMA warpgroups and that keeps
+  // the persistent CTAs busy
   int best_nt = 0;
   double best_eff = -1.0;
   const int nts[3] = {4, 2, 1};
@@ -694,7 +671,7 @@ static int launch_mode(const ConvTcArgs& a, cudaStream_t s) {
     const uint32_t oct = nt == 4 ? c3::Geo<MODE, 4>::OCT_BYTES : (nt == 2 ? c3::Geo<MODE, 2>::OCT_BYTES : c3::Geo<MODE, 1>::OCT_BYTES);
     const size_t stage = align_up((size_t)a.KG * oct + b_bytes, 128);
     stage_of[nt] = stage;
-    if (2 * nt * ncls * NPAD > 512 || 2 * stage + 256 > 227 * 1024) continue;
+    if (nt * ncls * NPAD > 256 || 2 * stage + 256 > 227 * 1024) continue;
     const long long ntiles = (long long)cdiv(cells_w, 8 * nt) * cdiv(cells_h, 16) * OD;
     const double eff = (double)ntiles / (double)(cdiv(ntiles, num_sms) * (long long)num_sms);
     if (eff >= 0.85) { best_nt = nt; break; }
@@ -705,18 +682,18 @@ static int launch_mode(const ConvTcArgs& a, cudaStream_t s) {
   int NS = (int)((227 * 1024 - 256) / stage);
   if (NS > c3::MAX_STAGES) NS = c3::MAX_STAGES;
   const size_t smem = NS * stage + 256;
-  switch (best_nt) {
-    case 4: return launch_one<MODE, 4, OUT>(a, NS, smem, OD, OH, OW, cells_h, cells_w, num_sms, s);
-    case 2: return launch_one<MODE, 2, OUT>(a, NS, smem, OD, OH, OW, cells_h, cells_w, num_sms, s);
-    default: return launch_one<MODE, 1, OUT>(a, NS, smem, OD, OH, OW, cells_h, cells_w, num_sms, s);
+  if constexpr (OUT == OUT_SPLIT) {
+    if (NPAD == 32) return launch_nt<MODE, OUT, 32>(a, best_nt, NS, smem, OD, OH, OW, cells_h, cells_w, num_sms, s);
+    if (NPAD == 64) return launch_nt<MODE, OUT, 64>(a, best_nt, NS, smem, OD, OH, OW, cells_h, cells_w, num_sms, s);
   }
+  return launch_nt<MODE, OUT, 16>(a, best_nt, NS, smem, OD, OH, OW, cells_h, cells_w, num_sms, s);
 }
 
 
-template <int MODE, int NT>
+template <int MODE, int NT, int NPAD>
 static int launch_col_one(const ConvTcArgs& a, int NS, int wres, size_t smem, int OH, int OW, int DC, int num_sms, cudaStream_t s) {
   using G = c3::Geo<MODE, NT>;
-  auto kern = conv3d_col_kernel<MODE, NT>;
+  auto kern = conv3d_col_kernel<MODE, NT, NPAD>;
   static DeviceOnce once;
   const int dev = current_device();
   if (once.need(dev)) {
@@ -758,7 +735,7 @@ static int launch_col(const ConvTcArgs& a, cudaStream_t s) {
   const int nts[3] = {4, 2, 1};
   for (int k = 0; k < 3; ++k) {
     const int nt = nts[k];
-    if (4 * nt * NPAD > 512) continue;
+    if (4 * nt * NPAD > 128) continue;                          // accumulator registers: 4 slots x NT x NPAD / 2 <= 64 (more spill)
     const uint32_t oct = nt == 4 ? c3::Geo<MODE, 4>::OCT_BYTES : (nt == 2 ? c3::Geo<MODE, 2>::OCT_BYTES : c3::Geo<MODE, 1>::OCT_BYTES);
     const size_t stage = align_up((size_t)a.KG * oct + (wres ? 0 : slab), 128);
     const size_t fixed = (wres ? wres_bytes : 0) + 256;
@@ -777,17 +754,17 @@ static int launch_col(const ConvTcArgs& a, cudaStream_t s) {
     }
   }
   MVSF_REQUIRE(best_nt > 0, "conv3d_col: no tile shape fits (CIN %d COUT %d)", a.CIN, a.COUT);
-  switch (best_nt) {
-    case 4: return launch_col_one<MODE, 4>(a, best_ns, wres, best_smem, OH, OW, best_dc, num_sms, s);
-    case 2: return launch_col_one<MODE, 2>(a, best_ns, wres, best_smem, OH, OW, best_dc, num_sms, s);
-    default: return launch_col_one<MODE, 1>(a, best_ns, wres, best_smem, OH, OW, best_dc, num_sms, s);
+  if (NPAD == 16) {
+    if (best_nt == 2) return launch_col_one<MODE, 2, 16>(a, best_ns, wres, best_smem, OH, OW, best_dc, num_sms, s);
+    return launch_col_one<MODE, 1, 16>(a, best_ns, wres, best_smem, OH, OW, best_dc, num_sms, s);
   }
+  return launch_col_one<MODE, 1, 32>(a, best_ns, wres, best_smem, OH, OW, best_dc, num_sms, s);
 }
 
 int launch_conv3d_tc(const ConvTcArgs& a, int mode, int out_mode, cudaStream_t s) {
   MVSF_REQUIRE(a.in_hi && a.in_lo && a.wtc && a.bias, "conv3d_tc: null pointer");
-  MVSF_REQUIRE(a.CIN % 8 == 0 && a.CIN >= 8 && a.CIN <= 64 && a.COUT % 8 == 0 && a.COUT >= 8 && a.COUT <= 64 &&
-                   (a.COUT == 8 || a.COUT % 16 == 0), "conv3d_tc: channels must be 8, 16, 32, 48 or 64");
+  MVSF_REQUIRE(a.CIN % 8 == 0 && a.CIN >= 8 && a.CIN <= 64 && (a.COUT == 8 || a.COUT == 16 || a.COUT == 32 || a.COUT == 64),
+               "conv3d_tc: input channels must be a multiple of 8 up to 64, output channels 8, 16, 32 or 64");
   MVSF_REQUIRE(a.SD == 1 || a.SD == 2, "conv3d_tc: depth stride must be 1 or 2");
   MVSF_REQUIRE(a.KG == conv3d_tc_kg(mode, a.CIN), "conv3d_tc: KG must be conv3d_tc_kg(mode, CIN) (it fixes the weight slab layout)");
   MVSF_REQUIRE(((uintptr_t)a.in_hi & 15) == 0 && ((uintptr_t)a.in_lo & 15) == 0 && ((uintptr_t)a.wtc & 15) == 0,

@@ -1,4 +1,4 @@
-// Host-side interface of the tcgen05 implicit-GEMM 3-D convolutions (conv3d_tc.cu) used by the U-Net regularisers.
+// Host-side interface of the wgmma implicit-GEMM 3-D convolutions (conv3d_tc.cu) used by the U-Net regularisers.
 #pragma once
 #include <cuda_fp16.h>
 

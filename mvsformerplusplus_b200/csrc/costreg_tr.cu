@@ -12,7 +12,7 @@
 
 #include "linear.cuh"
 #include "linear_tc.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace mvsf {
 
@@ -100,7 +100,7 @@ __device__ __forceinline__ float ex2f(float x) {
   return y;
 }
 
-#include "attention_fa.cuh"   // second-generation attention kernel (inside namespace mvsf)
+#include "attention_fa.cuh"   // attention kernel (inside namespace mvsf)
 
 // un-patchify epilogue: u [N][256] (n = vox*8+co) -> LayerNorm3D over the 8 channels of each voxel (eps 1e-6)
 // -> prob 1x1x1 (8 -> 1) + bias -> logits [D][H][W]
@@ -146,16 +146,16 @@ static int run_attention(const float* qkv, float* o, __half* o2, __half* tiled, 
   static DeviceOnce once;
   const int dev = current_device();
   if (once.need(dev)) {
-    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa6::SMEM));
-    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa6::SMEM));
+    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa::SMEM));
+    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa::SMEM));
     once.done(dev);
   }
   cudaEvent_t kt = ktimer_enabled() ? ktimer_begin("attention_tc", s) : nullptr;
-  const dim3 grid(cdiv(ntiles, 2), 4);
+  const dim3 grid(ntiles, 4);
   if (g_attention_plo)
-    attention_fa_kernel<true><<<grid, fa6::THREADS, fa6::SMEM, s>>>(tiled, o, o2, N, ntiles);
+    attention_fa_kernel<true><<<grid, fa::THREADS, fa::SMEM, s>>>(tiled, o, o2, N, ntiles);
   else
-    attention_fa_kernel<false><<<grid, fa6::THREADS, fa6::SMEM, s>>>(tiled, o, o2, N, ntiles);
+    attention_fa_kernel<false><<<grid, fa::THREADS, fa::SMEM, s>>>(tiled, o, o2, N, ntiles);
   if (kt) ktimer_end(kt, s);
   MVSF_LAUNCH_CHECK("attention_tc");
   return MVSF_OK;

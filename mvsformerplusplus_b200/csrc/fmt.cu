@@ -7,7 +7,7 @@
 // summaries of the two cross layers depend only on the reference view and are computed once.
 #include "linear.cuh"
 #include "linear_tc.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace mvsf {
 
@@ -158,7 +158,7 @@ linattn_apply_kernel(const float* __restrict__ q, int ldq, const float* __restri
   }
 }
 
-#include "fmt_smooth_tc.cuh"   // fused upsample + lateral add + 3x3 smooth conv on tcgen05
+#include "fmt_smooth_tc.cuh"   // fused upsample + lateral add + 3x3 smooth conv on wgmma
 
 struct FmtWs {
   __half *xn2, *att2, *hid2;   // fp16 hi|lo split activations: [M][128], [M][128], [M][512]

@@ -3,14 +3,15 @@
 //   phase 1 (SIMT)   pre = lateral (NCHW) + bilinear_up2(red) (NHWC, F.interpolate align_corners=False) on the 18 x 34 halo
 //                    of a 16 x 32 output tile, written as fp16 hi|lo voxel-octet planes in shared memory (zero outside the
 //                    image = the conv padding) - the upsampled + added tensor never goes to HBM
-//   phase 2 (tcgen05) 3x3 conv as implicit GEMM: four 16 x 8 M-tiles, a tap = a descriptor start address (conv3d_tc.cu);
+//   phase 2 (wgmma)  3x3 conv as implicit GEMM: four 16 x 8 M-tiles (two m64 halves each, two M-tiles per warpgroup, one
+//                    after the other), a tap = a descriptor start address (conv3d_tc.cu);
 //                    C = 8: one MMA per tap  [x_hi | x_lo] x [[w_hi;w_hi] | [w_lo;0]]  (N = 32);
 //                    C >= 16: per 16 channels  x_hi x [w_hi | w_lo] (N = 2C) and x_lo x w_hi (N = C) onto the first half
-//   phase 3          TMEM -> registers: add the two halves, fp32 NHWC store
+//   phase 3          accumulator registers: add the two halves, fp32 NHWC store
 #pragma once
 
 namespace sm2 {
-using namespace umma;
+using namespace gmma;
 constexpr int PR = 18, PC = 34;
 constexpr uint32_t PLANE = PR * PC * 16, PITCH = PC * 16;
 template <int C>
@@ -19,8 +20,7 @@ struct Cfg {
   static constexpr int NPAD = C < 16 ? 16 : C;           // rows of one weight part
   static constexpr int NG = C < 16 ? 1 : C / 16;         // K = 16 groups
   static constexpr uint32_t BT = 2 * 2 * NPAD * 16;      // one (tap, group) weight tile: 2 k-chunks x 2 NPAD rows x 16 B
-  static constexpr uint32_t OFF_PL = 0, OFF_BT = 2 * NO * PLANE, OFF_BAR = OFF_BT + 9 * NG * BT, SMEM = OFF_BAR + 32;
-  static constexpr uint32_t TCOLS = 4 * 2 * NPAD;        // accumulator columns (4 M-tiles x [first | second] part)
+  static constexpr uint32_t OFF_PL = 0, OFF_BT = 2 * NO * PLANE, SMEM = OFF_BT + 9 * NG * BT;
 };
 }  // namespace sm2
 
@@ -35,10 +35,6 @@ fmt_smooth_tc_kernel(const float* __restrict__ red, const float* __restrict__ la
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int H = 2 * h, W = 2 * w;
   const uint32_t sb = smem_u32(smem);
-  const uint32_t bar = sb + K::OFF_BAR;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + K::OFF_BAR + 16);
-  uint32_t ncols = 32;
-  while (ncols < K::TCOLS) ncols <<= 1;
 
   // ---- once per CTA: weight tiles.  wts = [tap][ci][co] fp32.  Tile (tap, g) = [2 k-chunks][2 NPAD rows][8 halves]:
   //      C >= 16: rows [0, NPAD) = w_hi, [NPAD, 2 NPAD) = w_lo, k-chunk kc = input channels 16 g + 8 kc + e
@@ -59,21 +55,10 @@ fmt_smooth_tc_kernel(const float* __restrict__ red, const float* __restrict__ la
     else v = part == 0 ? hi : lo;
     reinterpret_cast<__half*>(smem + K::OFF_BT)[i] = v;
   }
-  if (tid == 0) { mbar_init(bar, 1); fence_barrier_init(); }
-  if (warp == 0) tmem_alloc(sb + K::OFF_BAR + 16, ncols);
   fence_proxy_async();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t el = elect_one();
-  constexpr uint32_t a_hi = desc_hi(PITCH), b_hi = desc_hi(128);
-  const uint32_t idesc_full = make_idesc_f16(128, 2 * NPAD), idesc_half = make_idesc_f16(128, NPAD);
-  uint32_t phase = 0;
-
-  const int quarter = warp & 3, m = quarter * 32 + lane;
-  const int er = m >> 3, ec0 = (warp >> 2) * 16 + (m & 7);     // warps 0-3: M-tiles 0, 1; warps 4-7: M-tiles 2, 3
-  const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)((warp >> 2) * 2 * 2 * NPAD);
+  const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
+  float acc[2][NPAD];   // one M-tile: [m64 half][accumulator of N = 2 NPAD columns: first | second part]
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, v = tile / (tiles_x * tiles_y);
@@ -117,67 +102,59 @@ fmt_smooth_tc_kernel(const float* __restrict__ red, const float* __restrict__ la
       split_store8(p, p + PLANE / 2, pre);     // hi plane of octet o, then its lo plane (+ PLANE bytes)
     }
     fence_proxy_async();
-    tc_fence_before_sync();
     __syncthreads();
-    // ---- phase 2: MMAs (converged warp 0, elected lane)
-    if (warp == 0) {
-      tc_fence_after_sync();
+#pragma unroll 1
+    for (int k = 0; k < 2; ++k) {
+      const int ct = 2 * wg + k;
+      // ---- phase 2: MMAs of M-tile ct
+      wg_fence();
 #pragma unroll
       for (int kh = 0; kh < 3; ++kh) {
 #pragma unroll
         for (int kw = 0; kw < 3; ++kw) {
-          const uint32_t aoff = (uint32_t)(kh * PC + kw) * 16u;
+          const uint32_t aoff = (uint32_t)(kh * PC + kw) * 16u + (uint32_t)ct * 128u;
 #pragma unroll
           for (int g = 0; g < NG; ++g) {
-            const uint32_t wb = desc_lo(sb + K::OFF_BT + (uint32_t)((kh * 3 + kw) * NG + g) * K::BT, 2 * NPAD * 16);
-            const uint32_t acc = (kh | kw | g) ? 1u : 0u;
-            if (C < 16) {
-              const uint32_t ad = desc_lo(sb + K::OFF_PL + aoff, PLANE);                     // K = [hi | lo] planes of the octet
+            const uint64_t wb = make_desc(sb + K::OFF_BT + (uint32_t)((kh * 3 + kw) * NG + g) * K::BT, 2 * NPAD * 16, 128);
+            const uint32_t first = (kh | kw | g) ? 1u : 0u;
 #pragma unroll
-              for (int ct = 0; ct < 4; ++ct) mma_f16_ss_lh(el, tmem_base + ct * 2 * NPAD, ad + ct * 8, a_hi, wb, b_hi, idesc_full, acc);
-            } else {
-              // planes of group g: [hi o(2g) | lo o(2g) | hi o(2g+1) | lo o(2g+1)]: K chunks = the two hi (or lo) planes
-              const uint32_t ah = desc_lo(sb + K::OFF_PL + (uint32_t)(4 * g) * PLANE + aoff, 2 * PLANE), al = ah + (PLANE >> 4);
-#pragma unroll
-              for (int ct = 0; ct < 4; ++ct) mma_f16_ss_lh(el, tmem_base + ct * 2 * NPAD, ah + ct * 8, a_hi, wb, b_hi, idesc_full, acc);
-#pragma unroll
-              for (int ct = 0; ct < 4; ++ct) mma_f16_ss_lh(el, tmem_base + ct * 2 * NPAD, al + ct * 8, a_hi, wb, b_hi, idesc_half, 1u);
+            for (int hf = 0; hf < 2; ++hf) {
+              const uint32_t arow = aoff + (uint32_t)hf * 8u * PITCH;
+              if (C < 16) {   // K = [hi | lo] planes of the octet
+                mma_ss<2 * NPAD>(acc[hf], make_desc(sb + K::OFF_PL + arow, PLANE, PITCH), wb, first);
+              } else {
+                // planes of group g: [hi o(2g) | lo o(2g) | hi o(2g+1) | lo o(2g+1)]: K chunks = the two hi (or lo) planes
+                const uint32_t ah = sb + K::OFF_PL + (uint32_t)(4 * g) * PLANE + arow;
+                mma_ss<2 * NPAD>(acc[hf], make_desc(ah, 2 * PLANE, PITCH), wb, first);
+                mma_ss<NPAD>(acc[hf], make_desc(ah + PLANE, 2 * PLANE, PITCH), wb, 1u);
+              }
             }
           }
         }
       }
-      commit_el(el, bar);
-    }
-    // ---- phase 3: epilogue
-    mbar_wait(bar, phase);
-    phase ^= 1u;
-    tc_fence_after_sync();
+      wg_commit();
+      wg_wait<0>();
+      fence_regs<NPAD>(acc[0]);
+      fence_regs<NPAD>(acc[1]);
+      // ---- phase 3: epilogue (channels 8 b + 2 q, + 1 of rows 8 hf + 2 wq + h, column 8 ct + lane / 4)
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      const int y = y0 + er, x = x0 + ec0 + k * 8;
-      const bool valid = y < H && x < W;
-      float* op = out + (((size_t)v * H + (valid ? y : 0)) * W + (valid ? x : 0)) * C;
+      for (int hf = 0; hf < 2; ++hf)
 #pragma unroll
-      for (int c16 = 0; c16 < NPAD / 16; ++c16) {
-        float a[16], b[16];
-        tmem_ld16(trow + k * 2 * NPAD + c16 * 16, a);
-        tmem_ld16(trow + k * 2 * NPAD + NPAD + c16 * 16, b);
-        if (valid) {
+        for (int h = 0; h < 2; ++h) {
+          const int y = y0 + 8 * hf + 2 * wq + h, x = x0 + 8 * ct + (lane >> 2);
+          if (y >= H || x >= W) continue;
+          float* op = out + (((size_t)v * H + y) * W + x) * C;
 #pragma unroll
-          for (int q4 = 0; q4 < 4; ++q4) {
-            if (c16 * 16 + q4 * 4 < C)
-              *reinterpret_cast<float4*>(op + c16 * 16 + q4 * 4) =
-                  make_float4(a[q4 * 4] + b[q4 * 4], a[q4 * 4 + 1] + b[q4 * 4 + 1], a[q4 * 4 + 2] + b[q4 * 4 + 2], a[q4 * 4 + 3] + b[q4 * 4 + 3]);
+          for (int b = 0; b < NPAD / 8; ++b) {
+            if (8 * b >= C) continue;
+            const float o0 = acc[hf][4 * b + 2 * h] + acc[hf][4 * (b + NPAD / 8) + 2 * h];
+            const float o1 = acc[hf][4 * b + 2 * h + 1] + acc[hf][4 * (b + NPAD / 8) + 2 * h + 1];
+            *reinterpret_cast<float2*>(op + 8 * b + 2 * q) = make_float2(o0, o1);
           }
         }
-      }
     }
-    tc_fence_before_sync();
-    __syncthreads();   // planes and accumulators are free again
+    __syncthreads();   // planes are free again
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, ncols);
 }
 
 template <int C>
@@ -190,12 +167,7 @@ static int launch_fmt_smooth_tc(const float* red, const float* lat, const float*
   const int num_sms = device_sm_count(dev);
   if (once.need(dev)) {
     MVSF_CUDA_OK(cudaFuncSetAttribute(fmt_smooth_tc_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K::SMEM));
-    // resident CTAs per SM: registers (<= 80 x 256 threads -> 3), shared memory, tensor memory (512 columns per SM)
-    uint32_t ncols = 32;
-    while (ncols < K::TCOLS) ncols <<= 1;
-    per_sm = 3;
-    if (per_sm > (int)(512 / ncols)) per_sm = 512 / ncols;
-    if (per_sm > (int)((220 * 1024) / K::SMEM)) per_sm = (int)((220 * 1024) / K::SMEM);
+    MVSF_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fmt_smooth_tc_kernel<C>, 256, K::SMEM));
     if (per_sm < 1) per_sm = 1;
     once.done(dev);
   }

@@ -390,7 +390,8 @@ int mvsf_position3d(const float* kinv_ref, const float* depth, const float* dept
   if (mode == 1 || mode == 2 || mode == 3) {
     size_t total = (size_t)D * H * W;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    const int cap = device_sm_count(current_device()) * 8;
+    if (blocks > cap) blocks = cap;
     pos3d_minmax_kernel<<<blocks, 256, 0, s>>>(kinv_ref, depth, reinterpret_cast<unsigned*>(stats), D, H, W);
     MVSF_LAUNCH_CHECK("pos3d_minmax");
   }

@@ -1,21 +1,22 @@
-// Token-wise linear layers on the 5th-generation tensor cores:  C[M,N] = epi(A[M,K] * W[N,K]^T), fp32-class accuracy.
-//   * operands are split into fp16 hi + lo parts (hi+lo carries 22 mantissa bits); three tcgen05.mma.kind::f16 products
-//     per K-step (lo*hi, hi*lo, hi*hi) accumulate in fp32 in TMEM - a single-pass fp16/bf16/tf32 GEMM would move the
+// Token-wise linear layers on the Hopper tensor cores:  C[M,N] = epi(A[M,K] * W[N,K]^T), fp32-class accuracy.
+//   * operands are split into fp16 hi + lo parts (hi+lo carries 22 mantissa bits); three wgmma.m64nNk16 products per
+//     K-step (lo*hi, hi*lo, hi*hi) accumulate in fp32 registers - a single-pass fp16/bf16/tf32 GEMM would move the
 //     depth probabilities by ~1e-3 (SURVEY.md 7.3), the split stays at ~1e-6 relative;
-//   * tile = 128 rows x all N columns (N <= 256): the accumulator is 128 TMEM lanes x N columns; persistent CTAs (one per
-//     SM) keep the weights resident in shared memory and stream A in K-blocks of 64 through a 3-stage cp.async ring in the
-//     canonical no-swizzle K-major layout (umma.cuh); one thread issues the MMAs, tcgen05.commit -> mbarrier releases a
-//     stage; accumulators are double-buffered in TMEM so epilogue and MMA overlap;
-//   * epilogue: each of the 128 threads owns one accumulator row (tcgen05.ld 32x32b), so bias / GELU / ELU+1 / residual /
-//     LayerNorm need no cross-thread traffic; optionally also emits the fp16 hi|lo split of the result for the next GEMM.
+//   * tile = 128 rows x all N columns (N <= 256); persistent CTAs (one per SM) keep the weights resident in shared memory
+//     and stream A in K-blocks of 64 through a 4-stage cp.async ring in the canonical no-swizzle K-major layout
+//     (wgmma.cuh); mbarriers full[s] / empty[s] hand the stages between the producer warpgroup and the two MMA warpgroups;
+//   * each MMA warpgroup owns 64 rows of the tile and runs its epilogue from the accumulator registers: bias / GELU /
+//     ELU+1 / residual element-wise, LayerNorm with the row reduced over the four threads that share it; optionally also
+//     emits the fp16 hi|lo split of the result for the next GEMM.  While the MMA warpgroups run an epilogue the producer
+//     is already filling the ring with the next tile's K-blocks.
 // Used by the stage-1 transformer regulariser (module.py:507-646) and FMT (FMT.py, block.py:336-346).
 #include "linear_tc.cuh"
 
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace mvsf {
 
-using namespace umma;
+using namespace gmma;
 
 constexpr int TC_BM = 128, TC_BK = 64;
 
@@ -39,222 +40,129 @@ __global__ void split_f16_kernel(const float* __restrict__ x, int ldx, __half* _
   pl[0] = __halves2half2(lo[0], lo[1]); pl[1] = __halves2half2(lo[2], lo[3]);
 }
 
-__device__ __forceinline__ void store_split16(__half* c2row, int N, int col, const float (&v)[16]) {
-  __align__(16) __half hi[16], lo[16];
-#pragma unroll
-  for (int e = 0; e < 16; ++e) {
-    hi[e] = __float2half_rn(v[e]);
-    lo[e] = __float2half_rn(v[e] - __half2float(hi[e]));
-  }
-  uint4* dh = reinterpret_cast<uint4*>(c2row + col);
-  uint4* dl = reinterpret_cast<uint4*>(c2row + N + col);
-  dh[0] = reinterpret_cast<uint4*>(hi)[0]; dh[1] = reinterpret_cast<uint4*>(hi)[1];
-  dl[0] = reinterpret_cast<uint4*>(lo)[0]; dl[1] = reinterpret_cast<uint4*>(lo)[1];
-}
-
-// Persistent, warp-specialised kernel.  256 threads:
-//   warps 0-3  producers: cp.async-fill the A ring (one K-block of 128 rows, hi+lo, per stage); thread 0 issues the MMAs
-//   warps 4-7 / 8-11  epilogue warpgroups for even / odd tiles: TMEM -> registers -> global, one accumulator row per thread
-// The weight tiles of all K-blocks stay resident in shared memory for the CTA's lifetime; accumulators are double
-// buffered in TMEM (2 x N columns) so the epilogue of tile i overlaps the loads and MMAs of tile i+1.
-// mbarriers: empty[s] (MMAs that read stage s finished -> refill), acc_full[b] / acc_empty[b] (accumulator hand-over).
-// Two epilogue groups: even / odd tiles (= the two TMEM buffers).  Element-wise epilogues (bias / GELU / ELU+1 / residual)
-// use 8 warps per group - two warps per TMEM lane quarter, each taking half of the N columns: those epilogues are bound by
-// instruction issue (erf, fp16 hi|lo split: ~30 instructions per element), and 16 epilogue warps keep all four schedulers
-// busy; the LayerNorm epilogues need a whole row per thread (and ~130-170 registers), they keep 4 warps per group.
-constexpr int TC_NPROD = 128;
-template <int EPI> struct TcCfg {
-  static constexpr bool LN = (EPI == LIN_RES_LN || EPI == LIN_LN);
-  static constexpr int WPG = LN ? 4 : 8;          // epilogue warps per group
-  static constexpr int NEPI = 2 * WPG * 32;
-  static constexpr int THREADS = TC_NPROD + NEPI;
-};
-
-template <int EPI>
-__device__ __forceinline__ void tc_epilogue_tile(const TcLinArgs& a, uint32_t tacc, int m0, int warp4, int lane, int c_begin, int c_end) {
-  const int N = a.N;
-  const int row = warp4 * 32 + lane;
-  const int m = m0 + row;
-  const bool mvalid = m < a.M;
-  const uint32_t trow = tacc + ((uint32_t)(warp4 * 32) << 16);
-  const float* resrow = (EPI == LIN_RES || EPI == LIN_RES_LN) ? a.res + (size_t)(mvalid ? m : 0) * a.ldres : nullptr;
-  float* crow = a.C ? a.C + (size_t)(mvalid ? m : 0) * a.ldc : nullptr;
-  __half* c2row = a.C2 ? a.C2 + (size_t)(mvalid ? m : 0) * a.ldc2 : nullptr;
-  if (EPI == LIN_RES_LN || EPI == LIN_LN) {  // N == 64: the whole row lives in this thread's registers
-    float x[64];
-    float s = 0.f;
-    uint32_t raw[4][16];                 // the whole accumulator row in flight, one wait
-#pragma unroll
-    for (int c = 0; c < 4; ++c) tmem_ld16_nowait(trow + c * 16, raw[c]);
-    tmem_ld_wait();
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {   // 128-bit loads of bias / gamma / this row's residual
-        const int col = c * 16 + q * 4;
-        const float4 b4 = a.bias ? ldg4(a.bias + col) : make_float4(0.f, 0.f, 0.f, 0.f);
-        float t[4] = {__uint_as_float(raw[c][q * 4]) + b4.x, __uint_as_float(raw[c][q * 4 + 1]) + b4.y,
-                      __uint_as_float(raw[c][q * 4 + 2]) + b4.z, __uint_as_float(raw[c][q * 4 + 3]) + b4.w};
-        if (EPI == LIN_RES_LN) {
-          const float4 g4 = ldg4(a.gamma + col);
-          const float4 r4 = mvalid ? *reinterpret_cast<const float4*>(resrow + col) : make_float4(0.f, 0.f, 0.f, 0.f);
-          t[0] = r4.x + g4.x * t[0]; t[1] = r4.y + g4.y * t[1]; t[2] = r4.z + g4.z * t[2]; t[3] = r4.w + g4.w * t[3];
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { x[col + j] = t[j]; s += t[j]; }
-      }
-    }
-    if (a.Cpre && mvalid) {
-      float* prow = a.Cpre + (size_t)m * a.ldcpre;
-#pragma unroll
-      for (int e = 0; e < 16; ++e) *reinterpret_cast<float4*>(prow + e * 4) = make_float4(x[e * 4], x[e * 4 + 1], x[e * 4 + 2], x[e * 4 + 3]);
-    }
-    const float mean = s * (1.0f / 64.0f);
-    float q = 0.f;
-#pragma unroll
-    for (int e = 0; e < 64; ++e) { float d = x[e] - mean; q = fmaf(d, d, q); }
-    const float sd = sqrtf(q * (1.0f / 64.0f) + a.ln_eps);
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      float o[16];
-#pragma unroll
-      for (int e = 0; e < 16; ++e) {
-        const int col = c * 16 + e;
-        o[e] = __fdiv_rn(x[col] - mean, sd) * __ldg(a.ln_w + col) + __ldg(a.ln_b + col);
-      }
-      if (mvalid) {
-        if (crow) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            *reinterpret_cast<float4*>(crow + c * 16 + e * 4) = make_float4(o[e * 4], o[e * 4 + 1], o[e * 4 + 2], o[e * 4 + 3]);
-        }
-        if (c2row) store_split16(c2row, N, c * 16, o);
-      }
-    }
-  } else {
-    // software pipeline over the 16-column chunks: the tensor-memory load of chunk c+1 is in flight while chunk c is
-    // processed (a tcgen05.ld + wait costs a few hundred cycles; issued back to back they dominated the epilogue).
-    // Two named register buffers, chunks handled in pairs (a dynamically indexed buffer would live in local memory).
-    auto process = [&](int c, const uint32_t (&raw)[16]) {
-      float v[16], bs[16], rs[16], gm[16];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {   // 128-bit loads of the per-column vectors and of this row's residual
-        const float4 b4 = a.bias ? ldg4(a.bias + c * 16 + q * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-        bs[q * 4] = b4.x; bs[q * 4 + 1] = b4.y; bs[q * 4 + 2] = b4.z; bs[q * 4 + 3] = b4.w;
-        if (EPI == LIN_RES) {
-          const float4 g4 = ldg4(a.gamma + c * 16 + q * 4);
-          gm[q * 4] = g4.x; gm[q * 4 + 1] = g4.y; gm[q * 4 + 2] = g4.z; gm[q * 4 + 3] = g4.w;
-          const float4 r4 = mvalid ? *reinterpret_cast<const float4*>(resrow + c * 16 + q * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-          rs[q * 4] = r4.x; rs[q * 4 + 1] = r4.y; rs[q * 4 + 2] = r4.z; rs[q * 4 + 3] = r4.w;
-        }
-      }
-#pragma unroll
-      for (int e = 0; e < 16; ++e) {
-        const int col = c * 16 + e;
-        float t = __uint_as_float(raw[e]) + bs[e];
-        if (EPI == LIN_GELU) t = gelu_erf_lean(t);
-        if (EPI == LIN_ELU1) t = (col < a.elu_cols) ? ((t > 0.f ? t : expm1f(t)) + 1.0f) : t;
-        if (EPI == LIN_RES) t = rs[e] + gm[e] * t;
-        v[e] = t;
-      }
-      if (mvalid) {
-        if (crow) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            *reinterpret_cast<float4*>(crow + c * 16 + e * 4) = make_float4(v[e * 4], v[e * 4 + 1], v[e * 4 + 2], v[e * 4 + 3]);
-        }
-        if (c2row) store_split16(c2row, N, c * 16, v);
-      }
-    };
-    uint32_t rawA[16], rawB[16];
-    if (c_begin < c_end) tmem_ld16_nowait(trow + c_begin * 16, rawA);
-    for (int c = c_begin; c < c_end; c += 2) {
-      tmem_ld_wait();
-      if (c + 1 < c_end) tmem_ld16_nowait(trow + (c + 1) * 16, rawB);
-      process(c, rawA);
-      if (c + 1 < c_end) {
-        tmem_ld_wait();
-        if (c + 2 < c_end) tmem_ld16_nowait(trow + (c + 2) * 16, rawA);
-        process(c + 1, rawB);
-      }
-    }
-  }
-}
-
+// 384 threads: warpgroup 0 = producers (cp.async fills of the A ring), warpgroups 1 and 2 = MMA + epilogue of rows
+// [0, 64) and [64, 128) of every tile.  The weight tiles of all K-blocks stay resident in shared memory for the CTA's
+// lifetime.  Each MMA warpgroup keeps one K-block of MMAs in flight while it issues the next, and releases a ring stage
+// as soon as the MMAs that read it have retired.
+constexpr int TC_NPROD = 128, TC_THREADS = 384;
 constexpr int TC_RING = 4;   // A-tile stages; two fills stay in flight behind the block whose MMAs are being issued
 
-template <int EPI>
-__global__ void __launch_bounds__(TcCfg<EPI>::THREADS, 1)
+template <int N, int EPI>
+__device__ __forceinline__ void tc_epilogue(const TcLinArgs& a, const float (&acc)[N / 2], int row0, int lane) {
+  const int q = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = row0 + 8 * h;
+    const bool mvalid = m < a.M;
+    const float* resrow = (EPI == LIN_RES || EPI == LIN_RES_LN) ? a.res + (size_t)(mvalid ? m : 0) * a.ldres : nullptr;
+    float* crow = a.C ? a.C + (size_t)(mvalid ? m : 0) * a.ldc : nullptr;
+    __half* c2row = a.C2 ? a.C2 + (size_t)(mvalid ? m : 0) * a.ldc2 : nullptr;
+    if constexpr (EPI == LIN_RES_LN || EPI == LIN_LN) {   // N == 64: a row is spread over the 4 threads of a quad
+      float x[16];
+      float s = 0.f;
+#pragma unroll
+      for (int b = 0; b < 8; ++b) {
+        const int col = 8 * b + 2 * q;
+        const float2 b2 = a.bias ? *reinterpret_cast<const float2*>(a.bias + col) : make_float2(0.f, 0.f);
+        float t0 = acc[4 * b + 2 * h] + b2.x, t1 = acc[4 * b + 2 * h + 1] + b2.y;
+        if (EPI == LIN_RES_LN) {
+          const float2 g2 = *reinterpret_cast<const float2*>(a.gamma + col);
+          const float2 r2 = mvalid ? *reinterpret_cast<const float2*>(resrow + col) : make_float2(0.f, 0.f);
+          t0 = r2.x + g2.x * t0; t1 = r2.y + g2.y * t1;
+        }
+        x[2 * b] = t0; x[2 * b + 1] = t1;
+        s += t0 + t1;
+      }
+      if (a.Cpre && mvalid) {
+        float* prow = a.Cpre + (size_t)m * a.ldcpre;
+#pragma unroll
+        for (int b = 0; b < 8; ++b) *reinterpret_cast<float2*>(prow + 8 * b + 2 * q) = make_float2(x[2 * b], x[2 * b + 1]);
+      }
+      s += __shfl_xor_sync(0xffffffffu, s, 1);
+      s += __shfl_xor_sync(0xffffffffu, s, 2);
+      const float mean = s * (1.0f / 64.0f);
+      float v = 0.f;
+#pragma unroll
+      for (int e = 0; e < 16; ++e) { const float d = x[e] - mean; v = fmaf(d, d, v); }
+      v += __shfl_xor_sync(0xffffffffu, v, 1);
+      v += __shfl_xor_sync(0xffffffffu, v, 2);
+      const float sd = sqrtf(v * (1.0f / 64.0f) + a.ln_eps);
+      if (mvalid) {
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+          const int col = 8 * b + 2 * q;
+          const float o0 = __fdiv_rn(x[2 * b] - mean, sd) * __ldg(a.ln_w + col) + __ldg(a.ln_b + col);
+          const float o1 = __fdiv_rn(x[2 * b + 1] - mean, sd) * __ldg(a.ln_w + col + 1) + __ldg(a.ln_b + col + 1);
+          if (crow) *reinterpret_cast<float2*>(crow + col) = make_float2(o0, o1);
+          if (c2row) split_store2(c2row + col, c2row + N + col, o0, o1);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int b = 0; b < N / 8; ++b) {
+        const int col = 8 * b + 2 * q;
+        const float2 b2 = a.bias ? *reinterpret_cast<const float2*>(a.bias + col) : make_float2(0.f, 0.f);
+        float t[2] = {acc[4 * b + 2 * h] + b2.x, acc[4 * b + 2 * h + 1] + b2.y};
+        if (EPI == LIN_RES) {
+          const float2 g2 = *reinterpret_cast<const float2*>(a.gamma + col);
+          const float2 r2 = mvalid ? *reinterpret_cast<const float2*>(resrow + col) : make_float2(0.f, 0.f);
+          t[0] = r2.x + g2.x * t[0]; t[1] = r2.y + g2.y * t[1];
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          if (EPI == LIN_GELU) t[e] = gelu_erf_lean(t[e]);
+          if (EPI == LIN_ELU1) t[e] = (col + e < a.elu_cols) ? ((t[e] > 0.f ? t[e] : expm1f(t[e])) + 1.0f) : t[e];
+        }
+        if (mvalid) {
+          if (crow) *reinterpret_cast<float2*>(crow + col) = make_float2(t[0], t[1]);
+          if (c2row) split_store2(c2row + col, c2row + N + col, t[0], t[1]);
+        }
+      }
+    }
+  }
+}
+
+template <int N, int EPI>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 linear_tc_kernel(TcLinArgs a) {
-  constexpr int WPG = TcCfg<EPI>::WPG, NTHREADS = TcCfg<EPI>::THREADS;
   extern __shared__ __align__(128) unsigned char smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int N = a.N, K = a.K;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const int K = a.K;
   const int nkb = K / TC_BK;
-  const uint32_t a_bytes = tile_bytes(TC_BM), b_bytes = tile_bytes(N);
+  constexpr uint32_t a_bytes = tile_bytes(TC_BM), b_bytes = tile_bytes(N);
   const uint32_t sbase = smem_u32(smem);
   const uint32_t sB = sbase;                                   // [nkb][hi tile | lo tile]
   const uint32_t sA = sB + nkb * 2 * b_bytes;                  // ring [TC_RING][hi tile | lo tile]
-  const uint32_t bars = sA + TC_RING * 2 * a_bytes;            // empty[3] | acc_full[2] | acc_empty[2]  (8 B each)
-  const uint32_t bar_empty = bars, bar_accf = bars + 8 * TC_RING, bar_acce = bar_accf + 16;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + (sA - sbase) + TC_RING * 2 * a_bytes + 64);
+  const uint32_t bar_full = sA + TC_RING * 2 * a_bytes, bar_empty = bar_full + 8 * TC_RING;
 
-  uint32_t ncols = 32;
-  while (ncols < (uint32_t)(2 * N)) ncols <<= 1;
   if (tid == 0) {
-    for (int i = 0; i < TC_RING; ++i) mbar_init(bar_empty + 8 * i, 1);
-    mbar_init(bar_accf + 0, 1); mbar_init(bar_accf + 8, 1);
-    mbar_init(bar_acce + 0, WPG * 32); mbar_init(bar_acce + 8, WPG * 32);
+    for (int i = 0; i < TC_RING; ++i) { mbar_init(bar_full + 8 * i, TC_NPROD); mbar_init(bar_empty + 8 * i, 2); }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), ncols);
   // resident weights: all K-blocks, hi and lo
   for (int kb = 0; kb < nkb; ++kb) {
-    fill_tile<NTHREADS>(sB + (2 * kb) * b_bytes, a.Bh + kb * TC_BK, a.ldb, N, N, tid);
-    fill_tile<NTHREADS>(sB + (2 * kb + 1) * b_bytes, a.Bl + kb * TC_BK, a.ldb, N, N, tid);
+    fill_tile<TC_THREADS>(sB + (2 * kb) * b_bytes, a.Bh + kb * TC_BK, a.ldb, N, N, tid);
+    fill_tile<TC_THREADS>(sB + (2 * kb + 1) * b_bytes, a.Bl + kb * TC_BK, a.ldb, N, N, tid);
   }
   cp_async_commit_group();
   cp_async_wait_group<0>();
   fence_proxy_async();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int ntiles = (a.M + TC_BM - 1) / TC_BM;
-  const uint32_t idesc = make_idesc_f16(TC_BM, N);
-  const uint32_t lbo_a = tile_lbo(TC_BM), lbo_b = tile_lbo(N);
+  const int my_tiles = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  constexpr uint32_t lbo_a = tile_lbo(TC_BM), lbo_b = tile_lbo(N);
 
-  if (warp < 4) {
-    // ------------------------------------------------------------------ producers + MMA issue (thread 0)
+  if (wg == 0) {
+    // ------------------------------------------------------------------ producers
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");   // registers go to the accumulators of the MMA warpgroups
     // Blocks g = 0, 1, ... enumerate the (tile, kb) pairs of this CTA in order; block g uses ring stage g % TC_RING.  The
-    // copies of blocks g, g-1 are still in flight while the MMAs of block g-2 are issued (two cp.async groups of prefetch:
-    // with one group the L2 / HBM latency of every 32 KB block was exposed - ncu: long-scoreboard stalls 25 per issue,
-    // issue slots 11 % busy on the K = 256 layers).
-    const int my_tiles = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+    // copies of blocks g, g-1 are still in flight when block g-2 is handed to the MMA warpgroups (two cp.async groups of
+    // prefetch keep the L2 / HBM latency of the 32 KB blocks hidden).
     const int nblk = my_tiles * nkb;
-    auto issue_block = [&](int gb) {   // MMAs of block gb (its copies have landed and are visible to the async proxy)
-      if (tid == 0) {
-        const int t_it = gb / nkb, kb = gb - t_it * nkb, st = gb % TC_RING;
-        const int buf = t_it & 1;
-        if (kb == 0) mbar_wait(bar_acce + 8 * buf, (uint32_t)(((t_it >> 1) & 1) ^ 1));   // epilogue drained this accumulator
-        tc_fence_after_sync();
-        const uint32_t sa = sA + st * 2 * a_bytes;
-        const uint32_t sb = sB + kb * 2 * b_bytes;
-        const uint32_t tacc = tmem_base + (uint32_t)(buf * N);
-#pragma unroll
-        for (int i = 0; i < TC_BK / 16; ++i) {
-          const uint64_t ah = make_desc(sa + 2 * i * lbo_a, lbo_a, 128);
-          const uint64_t al = make_desc(sa + a_bytes + 2 * i * lbo_a, lbo_a, 128);
-          const uint64_t bh = make_desc(sb + 2 * i * lbo_b, lbo_b, 128);
-          const uint64_t bl = make_desc(sb + b_bytes + 2 * i * lbo_b, lbo_b, 128);
-          mma_f16_ss(tacc, al, bh, idesc, (kb > 0 || i > 0) ? 1u : 0u);
-          mma_f16_ss(tacc, ah, bl, idesc, 1u);
-          mma_f16_ss(tacc, ah, bh, idesc, 1u);
-        }
-        commit(bar_empty + 8 * st);
-        if (kb == nkb - 1) commit(bar_accf + 8 * buf);
-      }
+    auto publish = [&](int gb) {   // this thread's copies of block gb have landed: make them visible to the async proxy
+      fence_proxy_async();
+      mbar_arrive(bar_full + 8 * (gb % TC_RING));
     };
     int g = 0;
     for (int t_it = 0; t_it < my_tiles; ++t_it) {
@@ -268,57 +176,101 @@ linear_tc_kernel(TcLinArgs a) {
         fill_tile<TC_NPROD>(s0 + a_bytes, a.Al + (size_t)m0 * a.lda + kb * TC_BK, a.lda, TC_BM, valid_rows, tid);
         cp_async_commit_group();
         if (g >= 2) {
-          cp_async_wait_group<2>();       // block g-2's copies (of this thread) have landed
-          fence_proxy_async();
-          named_bar_sync(1, TC_NPROD);    // ... and everybody else's
-          issue_block(g - 2);
+          cp_async_wait_group<2>();
+          publish(g - 2);
         }
       }
     }
     if (nblk >= 2) {
       cp_async_wait_group<1>();
-      fence_proxy_async();
-      named_bar_sync(1, TC_NPROD);
-      issue_block(nblk - 2);
+      publish(nblk - 2);
     }
     if (nblk >= 1) {
       cp_async_wait_group<0>();
-      fence_proxy_async();
-      named_bar_sync(1, TC_NPROD);
-      issue_block(nblk - 1);
+      publish(nblk - 1);
     }
   } else {
-    // ------------------------------------------------------------------ epilogue warps
-    const int warp4 = warp & 3;         // the TMEM lane quarter this warp may access
-    const int ew = warp - 4;
-    const int grp = ew / WPG;           // epilogue group 0 drains buffer 0 (even tiles), group 1 buffer 1 (odd tiles)
-    const int part = (ew % WPG) >> 2;   // which share of the columns (element-wise epilogues: 2 warps per lane quarter)
-    const int nchunks = N / 16;
-    const int c_begin = (WPG == 8) ? (part ? (nchunks + 1) / 2 : 0) : 0;
-    const int c_end = (WPG == 8) ? (part ? nchunks : (nchunks + 1) / 2) : nchunks;
-    int tile_it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tile_it) {
-      const int buf = tile_it & 1;
-      if (buf != grp) continue;
-      mbar_wait(bar_accf + 8 * buf, (uint32_t)((tile_it >> 1) & 1));
-      tc_fence_after_sync();
-      tc_epilogue_tile<EPI>(a, tmem_base + (uint32_t)(buf * N), tile * TC_BM, warp4, lane, c_begin, c_end);
-      tc_fence_before_sync();
-      mbar_arrive(bar_acce + 8 * buf);
+    // ------------------------------------------------------------------ MMA + epilogue warpgroups
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int half = wg - 1;                     // rows [64 half, 64 half + 64) of every tile
+    const int t128 = tid & 127, lane = tid & 31;
+    const int row_in_tile = 64 * half + 16 * (t128 >> 5) + (lane >> 2);
+    float acc[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    auto release = [&](int gb) { if (t128 == 0) mbar_arrive(bar_empty + 8 * (gb % TC_RING)); };
+    int g = 0;
+    for (int t_it = 0; t_it < my_tiles; ++t_it) {
+      const int m0 = ((int)blockIdx.x + t_it * (int)gridDim.x) * TC_BM;
+      int pend = -1;
+      for (int kb = 0; kb < nkb; ++kb, ++g) {
+        const int st = g % TC_RING;
+        mbar_wait(bar_full + 8 * st, (uint32_t)((g / TC_RING) & 1));
+        const uint32_t sa = sA + st * 2 * a_bytes + (uint32_t)half * 1024u;   // 8 row groups of 128 B
+        const uint32_t sb = sB + kb * 2 * b_bytes;
+        wg_fence();
+#pragma unroll
+        for (int i = 0; i < TC_BK / 16; ++i) {
+          const uint64_t ah = make_desc(sa + 2 * i * lbo_a, lbo_a, 128);
+          const uint64_t al = make_desc(sa + a_bytes + 2 * i * lbo_a, lbo_a, 128);
+          const uint64_t bh = make_desc(sb + 2 * i * lbo_b, lbo_b, 128);
+          const uint64_t bl = make_desc(sb + b_bytes + 2 * i * lbo_b, lbo_b, 128);
+          mma_ss<N>(acc, al, bh, (kb > 0 || i > 0) ? 1u : 0u);
+          mma_ss<N>(acc, ah, bl, 1u);
+          mma_ss<N>(acc, ah, bh, 1u);
+        }
+        wg_commit();
+        if (pend >= 0) {
+          wg_wait<1>();
+          release(pend);
+        }
+        pend = g;
+      }
+      wg_wait<0>();
+      fence_regs<N / 2>(acc);
+      release(pend);
+      tc_epilogue<N, EPI>(a, acc, m0 + row_in_tile, lane);
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, ncols);
 }
 
 static size_t tc_smem_bytes(int N, int K) {
   return (size_t)(K / TC_BK) * 2 * tile_bytes(N) + (size_t)TC_RING * 2 * tile_bytes(TC_BM) + 128;
 }
 
+template <int N, int EPI>
+static int launch_tc(const TcLinArgs& a, size_t smem, int grid, cudaStream_t s) {
+  static DeviceOnce once;
+  const int dev = current_device();
+  if (once.need(dev)) {
+    MVSF_CUDA_OK(cudaFuncSetAttribute(linear_tc_kernel<N, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    once.done(dev);
+  }
+  linear_tc_kernel<N, EPI><<<grid, TC_THREADS, smem, s>>>(a);
+  MVSF_LAUNCH_CHECK("linear_tc");
+  return MVSF_OK;
+}
+
+template <int N>
+static int launch_tc_n(const TcLinArgs& a, int epi, size_t smem, int grid, cudaStream_t s) {
+  switch (epi) {
+    case LIN_BIAS: return launch_tc<N, LIN_BIAS>(a, smem, grid, s);
+    case LIN_GELU: return launch_tc<N, LIN_GELU>(a, smem, grid, s);
+    case LIN_ELU1: return launch_tc<N, LIN_ELU1>(a, smem, grid, s);
+    case LIN_RES: return launch_tc<N, LIN_RES>(a, smem, grid, s);
+    default: break;
+  }
+  if constexpr (N == 64) {
+    if (epi == LIN_RES_LN) return launch_tc<64, LIN_RES_LN>(a, smem, grid, s);
+    if (epi == LIN_LN) return launch_tc<64, LIN_LN>(a, smem, grid, s);
+  }
+  return fail(MVSF_ERR_INVALID, "linear_tc: unknown epilogue %d", epi);
+}
+
 int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s) {
   MVSF_REQUIRE(a.Ah && a.Al && a.Bh && a.Bl && (a.C || a.C2) && a.M > 0, "linear_tc: bad arguments");
-  MVSF_REQUIRE(a.N % 16 == 0 && a.N >= 16 && a.N <= 256 && a.K % TC_BK == 0 && a.K >= TC_BK, "linear_tc: need N %% 16 == 0, 16 <= N <= 256, K %% 64 == 0");
+  MVSF_REQUIRE((a.N == 16 || a.N == 64 || a.N == 128 || a.N == 192 || a.N == 256) && a.K % TC_BK == 0 && a.K >= TC_BK,
+               "linear_tc: need N in {16, 64, 128, 192, 256}, K %% 64 == 0");
   MVSF_REQUIRE((a.lda % 8) == 0 && (a.ldb % 8) == 0 && ((uintptr_t)a.Ah & 15) == 0 && ((uintptr_t)a.Al & 15) == 0 &&
                    ((uintptr_t)a.Bh & 15) == 0 && ((uintptr_t)a.Bl & 15) == 0, "linear_tc: operands must be 16-byte aligned");
   if (a.C) MVSF_REQUIRE((a.ldc % 4) == 0 && ((uintptr_t)a.C & 15) == 0, "linear_tc: C must be 16-byte aligned");
@@ -332,32 +284,16 @@ int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s) {
                            "linear_tc: Cpre needs a LayerNorm epilogue and 16-byte alignment");
   const size_t smem = tc_smem_bytes(a.N, a.K);
   MVSF_REQUIRE(smem <= 227 * 1024, "linear_tc: N*K too large for resident weights (%zu bytes of shared memory)", smem);
-  static DeviceOnce once;
-  const int dev = current_device();
-  const int num_sms = device_sm_count(dev);
-  if (once.need(dev)) {
-    const int maxs = 227 * 1024;
-    MVSF_CUDA_OK(cudaFuncSetAttribute(linear_tc_kernel<LIN_BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxs));
-    MVSF_CUDA_OK(cudaFuncSetAttribute(linear_tc_kernel<LIN_GELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxs));
-    MVSF_CUDA_OK(cudaFuncSetAttribute(linear_tc_kernel<LIN_ELU1>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxs));
-    MVSF_CUDA_OK(cudaFuncSetAttribute(linear_tc_kernel<LIN_RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxs));
-    MVSF_CUDA_OK(cudaFuncSetAttribute(linear_tc_kernel<LIN_RES_LN>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxs));
-    MVSF_CUDA_OK(cudaFuncSetAttribute(linear_tc_kernel<LIN_LN>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxs));
-    once.done(dev);
-  }
+  const int num_sms = device_sm_count(current_device());
   const int ntiles = cdiv(a.M, TC_BM);
-  dim3 grid(ntiles < num_sms ? ntiles : num_sms);  // persistent: one CTA per SM, tiles strided by gridDim.x
-  switch (epi) {
-    case LIN_BIAS: linear_tc_kernel<LIN_BIAS><<<grid, TcCfg<LIN_BIAS>::THREADS, smem, s>>>(a); break;
-    case LIN_GELU: linear_tc_kernel<LIN_GELU><<<grid, TcCfg<LIN_GELU>::THREADS, smem, s>>>(a); break;
-    case LIN_ELU1: linear_tc_kernel<LIN_ELU1><<<grid, TcCfg<LIN_ELU1>::THREADS, smem, s>>>(a); break;
-    case LIN_RES: linear_tc_kernel<LIN_RES><<<grid, TcCfg<LIN_RES>::THREADS, smem, s>>>(a); break;
-    case LIN_RES_LN: linear_tc_kernel<LIN_RES_LN><<<grid, TcCfg<LIN_RES_LN>::THREADS, smem, s>>>(a); break;
-    case LIN_LN: linear_tc_kernel<LIN_LN><<<grid, TcCfg<LIN_LN>::THREADS, smem, s>>>(a); break;
-    default: return fail(MVSF_ERR_INVALID, "linear_tc: unknown epilogue %d", epi);
+  const int grid = ntiles < num_sms ? ntiles : num_sms;  // persistent: one CTA per SM, tiles strided by gridDim.x
+  switch (a.N) {
+    case 16: return launch_tc_n<16>(a, epi, smem, grid, s);
+    case 64: return launch_tc_n<64>(a, epi, smem, grid, s);
+    case 128: return launch_tc_n<128>(a, epi, smem, grid, s);
+    case 192: return launch_tc_n<192>(a, epi, smem, grid, s);
+    default: return launch_tc_n<256>(a, epi, smem, grid, s);
   }
-  MVSF_LAUNCH_CHECK("linear_tc");
-  return MVSF_OK;
 }
 
 __global__ void split_blob_f16_kernel(const float* __restrict__ x, __half* __restrict__ hi, __half* __restrict__ lo, size_t n) {

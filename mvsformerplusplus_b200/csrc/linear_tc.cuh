@@ -1,4 +1,4 @@
-// Host-side interface of the tcgen05 linear layers (linear_tc.cu).
+// Host-side interface of the wgmma linear layers (linear_tc.cu).
 #pragma once
 #include <cuda_fp16.h>
 

@@ -5,23 +5,24 @@
 //   layer 1 (1 -> 16, 144 FMA / pixel)  SIMT over the 18 x 34 halo region; the result is stored as fp16 hi|lo VOXEL-OCTET
 //                                       PLANES in shared memory (plane[row][col] = 8 channels = 16 B), the layout in
 //                                       which a 3x3 tap is just another UMMA descriptor start address (see conv3d_tc.cu)
-//   layer 2 (16 -> 16) and 3 (16 -> 8)  implicit GEMMs on tcgen05: M-tile = 16 rows x 8 columns of pixels, N = 16, K = 16
-//                                       channels; per tap two MMAs: x_hi x [w_hi | w_lo] (N = 32, both products side by
-//                                       side) and x_lo x w_hi (N = 16, accumulated onto the first), fp32 accumulators in
-//                                       TMEM (a small-N tcgen05.mma costs ~50 clk whatever N is: fewer, wider MMAs); the layer-2 epilogue (bias, ReLU, zero outside the
-//                                       image = layer 3's padding) writes the planes of layer 3's input
-//   layer 4 + sigmoid                   in the layer-3 epilogue (one TMEM lane = one pixel per thread)
+//   layer 2 (16 -> 16) and 3 (16 -> 8)  implicit GEMMs on wgmma: M-tile = 16 rows x 8 columns of pixels (two m64 halves of
+//                                       8 rows), N = 16, K = 16 channels; per tap two MMAs: x_hi x [w_hi | w_lo] (N = 32,
+//                                       both products side by side) and x_lo x w_hi (N = 16, accumulated onto the first
+//                                       16 columns), fp32 accumulators in registers; each warpgroup owns two M-tiles; the
+//                                       layer-2 epilogue (bias, ReLU, zero outside the image = layer 3's padding) writes
+//                                       the planes of layer 3's input
+//   layer 4 + sigmoid                   in the layer-3 epilogue (the 8 channels of a pixel sit in the 4 threads of a quad)
 // The 16 x 32 region of layer 2 and the 14 x 30 tile of layer 3 are both covered by four 16 x 8 M-tiles; rows / columns of
 // an M-tile that fall outside the useful region read the zero border of the plane buffers and are discarded.
 // Two CTAs per SM (101 KB of shared memory each) overlap one CTA's SIMT phases with the other's MMAs.
 // The fp32 SIMT version this replaces ran at 48 % of the FMA peak (1.9 ms per DTU depth map).
 #include "common.cuh"
 #include "linear_tc.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace mvsf {
 
-using namespace umma;
+using namespace gmma;
 
 __device__ __forceinline__ void store_half8(__half* dst, const float (&v)[8]) {
   __align__(16) __half h[8];
@@ -42,7 +43,7 @@ constexpr int OFF_W2 = 160, OFF_B2 = 160 + 2304, OFF_W3 = OFF_B2 + 16,
 // shared memory (bytes): planes a1 [hi o0 | hi o1 | lo o0 | lo o1], planes a2, weight tiles, input, small params, barrier
 constexpr uint32_t OFF_A1 = 0, OFF_A2 = 4 * PLANE, OFF_B2T = 8 * PLANE, BT_LAYER = 9 * 1024,      // [tap][2 kc][32 rows: w_hi | w_lo][8]
                    OFF_B3T = OFF_B2T + BT_LAYER, OFF_IN = OFF_B3T + BT_LAYER, OFF_PAR = OFF_IN + IN_R * IN_C * 4,
-                   OFF_BAR = OFF_PAR + 1024, SMEM = OFF_BAR + 32;
+                   SMEM = OFF_PAR + 1024;
 // small parameter block (floats): w1[144] b1[16] b2[16] b3[8] w4[8] b4[1]
 constexpr int P_W1 = 0, P_B1 = 144, P_B2 = 160, P_B3 = 176, P_W4 = 184, P_B4 = 192;
 }  // namespace vc
@@ -62,9 +63,6 @@ vis_cnn_kernel(const float* __restrict__ entropy, const float* __restrict__ wts,
   const uint32_t sb = smem_u32(smem);
   float* in_s = reinterpret_cast<float*>(smem + OFF_IN);
   float* par = reinterpret_cast<float*>(smem + OFF_PAR);
-  const uint32_t bar = sb + OFF_BAR;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + OFF_BAR + 16);
-
   // ---- once per CTA: parameters, fp16 hi|lo weight tiles in the canonical K-major B layout, zero border of a2
   for (int i = tid; i < 160; i += 256) par[i] = __ldg(wts + i);                      // w1, b1
   if (tid < 16) par[P_B2 + tid] = __ldg(wts + OFF_B2 + tid);
@@ -82,44 +80,43 @@ vis_cnn_kernel(const float* __restrict__ entropy, const float* __restrict__ wts,
     t[kc * 256 + (16 + n) * 8 + e] = lo;
   }
   for (int i = tid; i < (int)(4 * PLANE / 16); i += 256) reinterpret_cast<uint4*>(smem + OFF_A2)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) { mbar_init(bar, 1); fence_barrier_init(); }
-  if (warp == 0) tmem_alloc(sb + OFF_BAR + 16, 256);
   fence_proxy_async();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t el = elect_one();
-  constexpr uint32_t a_hi = desc_hi(PITCH), b_hi = desc_hi(128);
-  const uint32_t idesc16 = make_idesc_f16(128, 16), idesc32 = make_idesc_f16(128, 32);
-  uint32_t phase = 0;
+  const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
+  float acc[2][2][16];   // [M-tile 2 wg + k][m64 half][accumulator]
 
-  // MMAs of one 3x3 layer over the four M-tiles: planes at `pl`, weight tiles at `bt`, accumulators at TMEM column `col`
-  auto issue_layer = [&](uint32_t pl, uint32_t bt, uint32_t col) {
+  // MMAs of one 3x3 layer over this warpgroup's two M-tiles: planes at `pl`, weight tiles at `bt`
+  // accumulator columns: [0, 16) = x_hi w_hi + x_lo w_hi, [16, 32) = x_hi w_lo
+  auto issue_layer = [&](uint32_t pl, uint32_t bt) {
+    wg_fence();
 #pragma unroll
     for (int kh = 0; kh < 3; ++kh) {
 #pragma unroll
       for (int kw = 0; kw < 3; ++kw) {
         const uint32_t aoff = (uint32_t)(kh * PC + kw) * 16u;
-        const uint32_t ah = desc_lo(pl + aoff, PLANE), al = desc_lo(pl + 2 * PLANE + aoff, PLANE);   // K = two octets
-        const uint32_t wb = desc_lo(bt + (kh * 3 + kw) * 1024, 512);
-        const uint32_t acc = (kh | kw) ? 1u : 0u;
-        // accumulator columns of M-tile ct: [32 ct, +16) = x_hi w_hi + x_lo w_hi, [32 ct + 16, +16) = x_hi w_lo
+        const uint64_t wb = make_desc(bt + (kh * 3 + kw) * 1024, 512, 128);
+        const uint32_t first = (kh | kw) ? 1u : 0u;
 #pragma unroll
-        for (int ct = 0; ct < 4; ++ct) mma_f16_ss_lh(el, tmem_base + col + ct * 32, ah + ct * 8, a_hi, wb, b_hi, idesc32, acc);
+        for (int k = 0; k < 2; ++k)
+#pragma unroll
+          for (int hf = 0; hf < 2; ++hf)
+            mma_ss<32>(acc[k][hf], make_desc(pl + aoff + (2 * wg + k) * 128 + hf * 8 * PITCH, PLANE, PITCH), wb, first);
         if (XLO) {
 #pragma unroll
-          for (int ct = 0; ct < 4; ++ct) mma_f16_ss_lh(el, tmem_base + col + ct * 32, al + ct * 8, a_hi, wb, b_hi, idesc16, 1u);
+          for (int k = 0; k < 2; ++k)
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf)
+              mma_ss<16>(acc[k][hf], make_desc(pl + 2 * PLANE + aoff + (2 * wg + k) * 128 + hf * 8 * PITCH, PLANE, PITCH), wb, 1u);
         }
       }
     }
-    commit_el(el, bar);
+    wg_commit();
+    wg_wait<0>();
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) fence_regs<16>(acc[k][hf]);
   };
-
-  // epilogue geometry: warp w reads TMEM lanes 32 (w % 4) ..., warps 0-3 take M-tiles 0 and 1, warps 4-7 M-tiles 2 and 3
-  const int quarter = warp & 3, m = quarter * 32 + lane;
-  const int er = m >> 3, ec0 = (warp >> 2) * 16 + (m & 7);     // row and first column (second M-tile: + 8)
-  const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)((warp >> 2) * 64);
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, n = tile / (tiles_x * tiles_y);
@@ -164,66 +161,58 @@ vis_cnn_kernel(const float* __restrict__ entropy, const float* __restrict__ wts,
       }
     }
     fence_proxy_async();
-    tc_fence_before_sync();
     __syncthreads();
-    if (warp == 0) { tc_fence_after_sync(); issue_layer(sb + OFF_A1, sb + OFF_B2T, 0u); }
+    issue_layer(sb + OFF_A1, sb + OFF_B2T);
     // ---- layer-2 epilogue: bias, ReLU, zero outside the image -> planes a2 (16 x 32 region anchored at row 0, column 0)
-    mbar_wait(bar, phase);
-    phase ^= 1u;
-    tc_fence_after_sync();
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      float v[16], v2[16];
-      tmem_ld16(trow + k * 32, v);
-      tmem_ld16(trow + k * 32 + 16, v2);
+    for (int k = 0; k < 2; ++k)
 #pragma unroll
-      for (int oc = 0; oc < 16; ++oc) v[oc] += v2[oc];
-      const int c = ec0 + k * 8;
-      const int gy = y0 - 1 + er, gx = x0 - 1 + c;
-      const bool inside = gy >= 0 && gy < H && gx >= 0 && gx < W;
+      for (int hf = 0; hf < 2; ++hf)
 #pragma unroll
-      for (int oc = 0; oc < 16; ++oc) v[oc] = inside ? fmaxf(v[oc] + par[P_B2 + oc], 0.0f) : 0.0f;
-      __half* p = reinterpret_cast<__half*>(smem + OFF_A2 + (uint32_t)(er * PC + c) * 16u);
-      const float (&lo8)[8] = reinterpret_cast<const float (&)[8]>(v[0]);
-      const float (&hi8)[8] = reinterpret_cast<const float (&)[8]>(v[8]);
-      if (XLO) {
-        split_store8(p, p + PLANE, lo8);
-        split_store8(p + PLANE / 2, p + PLANE / 2 + PLANE, hi8);
-      } else {
-        store_half8(p, lo8);
-        store_half8(p + PLANE / 2, hi8);
-      }
-    }
+        for (int h = 0; h < 2; ++h) {
+          const int er = 8 * hf + 2 * wq + h, c = 16 * wg + 8 * k + (lane >> 2);
+          const int gy = y0 - 1 + er, gx = x0 - 1 + c;
+          const bool inside = gy >= 0 && gy < H && gx >= 0 && gx < W;
+          __half* p = reinterpret_cast<__half*>(smem + OFF_A2 + (uint32_t)(er * PC + c) * 16u) + 2 * q;
+#pragma unroll
+          for (int b = 0; b < 2; ++b) {   // channel octet b: channels 8 b + 2 q, + 1
+            float v[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float x = acc[k][hf][4 * b + 2 * h + e] + acc[k][hf][4 * (b + 2) + 2 * h + e];
+              v[e] = inside ? fmaxf(x + par[P_B2 + 8 * b + 2 * q + e], 0.0f) : 0.0f;
+            }
+            // p is a __half*: + PLANE / 2 elements = + PLANE bytes.  Planes: [hi o0 | hi o1 | lo o0 | lo o1]
+            if (XLO) split_store2(p + b * (PLANE / 2), p + b * (PLANE / 2) + PLANE, v[0], v[1]);
+            else *reinterpret_cast<__half2*>(p + b * (PLANE / 2)) = __floats2half2_rn(v[0], v[1]);
+          }
+        }
     fence_proxy_async();
-    tc_fence_before_sync();
     __syncthreads();
-    if (warp == 0) { tc_fence_after_sync(); issue_layer(sb + OFF_A2, sb + OFF_B3T, 128u); }
-    // ---- layer-3 epilogue: bias, ReLU, 1x1 conv, sigmoid
-    mbar_wait(bar, phase);
-    phase ^= 1u;
-    tc_fence_after_sync();
+    issue_layer(sb + OFF_A2, sb + OFF_B3T);
+    // ---- layer-3 epilogue: bias, ReLU, 1x1 conv, sigmoid (channels 2 q, 2 q + 1 here, the quad adds the rest)
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      float v[16], v2[16];
-      tmem_ld16(trow + 128 + k * 32, v);
-      tmem_ld16(trow + 128 + k * 32 + 16, v2);
+    for (int k = 0; k < 2; ++k)
 #pragma unroll
-      for (int oc = 0; oc < 8; ++oc) v[oc] += v2[oc];
-      const int ox = ec0 + k * 8;
-      const int gy = y0 + er, gx = x0 + ox;
-      if (er < TH && ox < TW && gy < H && gx < W) {
-        float s = par[P_B4];
+      for (int hf = 0; hf < 2; ++hf)
 #pragma unroll
-        for (int oc = 0; oc < 8; ++oc) s = fmaf(fmaxf(v[oc] + par[P_B3 + oc], 0.f), par[P_W4 + oc], s);
-        vis[((size_t)n * H + gy) * W + gx] = __fdiv_rn(1.0f, 1.0f + expf(-s));
-      }
-    }
-    tc_fence_before_sync();
-    __syncthreads();   // a1, the input tile and the TMEM columns are free again
+        for (int h = 0; h < 2; ++h) {
+          float s = 0.f;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int oc = 2 * q + e;
+            const float x = acc[k][hf][2 * h + e] + acc[k][hf][8 + 2 * h + e];
+            s = fmaf(fmaxf(x + par[P_B3 + oc], 0.f), par[P_W4 + oc], s);
+          }
+          s += __shfl_xor_sync(0xffffffffu, s, 1);
+          s += __shfl_xor_sync(0xffffffffu, s, 2);
+          const int er = 8 * hf + 2 * wq + h, ox = 16 * wg + 8 * k + (lane >> 2);
+          const int gy = y0 + er, gx = x0 + ox;
+          if (q == 0 && er < TH && ox < TW && gy < H && gx < W)
+            vis[((size_t)n * H + gy) * W + gx] = __fdiv_rn(1.0f, 1.0f + expf(-(s + par[P_B4])));
+        }
+    __syncthreads();   // a1, a2 and the input tile are free again
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 256);
 }
 
 }  // namespace mvsf

@@ -447,9 +447,9 @@ static int warp_corr_entropy_impl(const float* feat, const float* homs, const fl
                                   int C, int G, int D, int H, int W, mvsf_stream_t stream);
 
 /* 1: run the cost volume as two gathers (mvsf_warp_corr_entropy + mvsf_warp_corr_aggregate, no intermediate buffer);
- * 0: spill plan (mvsf_warp_corr_entropy_store + mvsf_corr_aggregate, needs 4*(V-1)*G*D*H*W bytes).  Measured on B200 the
- * spill plan is the faster one at every stage of the shipped cascade (the gather is bound by the SM's load path, the
- * streaming pass by HBM), so the recommendation only depends on the buffer size the caller is willing to spend. */
+ * 0: spill plan (mvsf_warp_corr_entropy_store + mvsf_corr_aggregate, needs 4*(V-1)*G*D*H*W bytes).  The spill
+ * plan gathers once and streams the stored correlations (the gather is bound by the SM's load path, the streaming pass by
+ * HBM), so the recommendation only depends on the buffer size the caller is willing to spend. */
 int mvsf_warp_corr_plan(int C, int G, int D, int H, int W, int V, size_t spill_budget_bytes) {
   if (G != 8 || !(C == 8 || C == 16 || C == 32 || C == 64)) return 1;   // the spill kernels exist for G == 8 only
   const size_t spill = (size_t)4 * (size_t)(V > 1 ? V - 1 : 1) * G * D * H * W;

@@ -17,13 +17,8 @@
 //     round delivers depends on the tap's x/y parity; that is folded into per-tap swaps of the two x / y weights and
 //     base addresses (lane-constant predicates), so the 8 rounds themselves are straight-line code;
 //   * taps outside the staged window (depth outliers) fall back to global loads for that lane only.
-// Measured on B200 (DTU stage 4, 28.3 M taps per pass; DESIGN.md "warp + correlation" has the full table): pass A 0.37 ms,
-// pass B 0.42 ms - faster than the L1-gather kernels doing the same two gathers (0.43 / 0.50 ms), 28 % faster on the
-// plane-sweep microbenchmark, but slower than warp_corr.cu's spill plan (gather once, stream the stored correlations:
-// 0.51 + 0.19 ms), which therefore stays the default of the cascade; these kernels serve the two-gather plan (plane sweeps,
-// spill buffers over budget).  A variant that staged the window rows with cp.async.bulk (2-4 KB requests, odd row pitch)
-// instead of the tensor box measured slower (0.58 / 0.69 ms); with D = 4..8 taps per lane and window the per-window
-// skeleton (coordinates, bounding box, CTA barrier, staging latency) costs more than the conflict-free gather itself.
+// warp_corr.cu's spill plan (gather once, stream the stored correlations) is the default of the cascade; these kernels
+// serve the two-gather plan (plane sweeps, spill buffers over budget).
 #include <cuda.h>
 #include <float.h>
 #include <limits.h>
@@ -93,12 +88,9 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
   return v;
 }
-// acc (4 channels) += w * t, as two packed fp32x2 FMAs (FFMA2: one issue slot per two FMAs)
+// acc (4 channels) += w * t
 __device__ __forceinline__ void fma4(float4& acc, float w, const float4& t) {
-  const float2 ww = make_float2(w, w);
-  float2 lo = __ffma2_rn(make_float2(t.x, t.y), ww, make_float2(acc.x, acc.y));
-  float2 hi = __ffma2_rn(make_float2(t.z, t.w), ww, make_float2(acc.z, acc.w));
-  acc = make_float4(lo.x, lo.y, hi.x, hi.y);
+  acc = make_float4(fmaf(t.x, w, acc.x), fmaf(t.y, w, acc.y), fmaf(t.z, w, acc.z), fmaf(t.w, w, acc.w));
 }
 __device__ __forceinline__ float dot4(const float4& a, const float4& b) { return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.y, b.y, a.x * b.x))); }
 

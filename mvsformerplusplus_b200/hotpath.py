@@ -1,4 +1,4 @@
-"""Host side of the B200 hot path: Python/PyTorch mirrors of the reference seams (SURVEY.md §8b) that
+"""Host side of the CUDA hot path: Python/PyTorch mirrors of the reference seams (SURVEY.md §8b) that
 enqueue libmvsf_b200 kernels.  PyTorch is used for device memory, streams and module/state-dict plumbing only.
 
   StageNet.forward(features, proj_matrices, depth_values, tmp, position3d=None)   <- models/cost_volume.py:51-133
@@ -37,7 +37,7 @@ def _f32c(t):
 
 def _require_cuda(t, what):
     if not t.is_cuda:
-        raise RuntimeError(f"{what}: expected a CUDA tensor (the B200 hot path has no CPU fallback)")
+        raise RuntimeError(f"{what}: expected a CUDA tensor (the hot path has no CPU fallback)")
 
 
 def to_nhwc(x):
@@ -62,7 +62,7 @@ def to_nchw(x_nhwc):
 
 
 def split_weights_f16(flat):
-    """fp32 weight blob on the device -> fp16 [hi | lo] blob for the tcgen05 GEMMs (install time, once)."""
+    """fp32 weight blob on the device -> fp16 [hi | lo] blob for the wgmma GEMMs (install time, once)."""
     L = _lib.lib()
     n = flat.numel()
     assert n % 8 == 0
@@ -72,7 +72,7 @@ def split_weights_f16(flat):
 
 
 def pack_unet_tc(kind, flat):
-    """fp32 U-Net weight blob (packing.pack_costreg_unet) on the device -> fp16 hi/lo weight slabs of the tcgen05
+    """fp32 U-Net weight blob (packing.pack_costreg_unet) on the device -> fp16 hi/lo weight slabs of the wgmma
     implicit-GEMM convolutions (install time, once)."""
     L = _lib.lib()
     need = ctypes.c_size_t(0)
@@ -248,7 +248,7 @@ class StageNet(_PackedMixin, nn.Module):
     @torch.no_grad()
     def forward(self, features, proj_matrices, depth_values, tmp, position3d=None, keep_intermediates=False):
         if self.training:
-            raise NotImplementedError("B200 hot path implements the eval-mode forward (test.py); call .eval()")
+            raise NotImplementedError("the hot path implements the eval-mode forward (test.py); call .eval()")
         if self.depth_type != "ce":
             raise NotImplementedError("depth_type must be 'ce'")
         _require_cuda(features, "StageNet.forward(features)")

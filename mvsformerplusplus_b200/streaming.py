@@ -2,12 +2,9 @@
 device slots while the previous batches are still being computed, so the PCIe transfer of the FPN pyramids (531 MB per
 DTU reference view) overlaps the kernels instead of preceding them.
 
-EXPERIMENTAL, off by default: with `lanes` > 1 consecutive batches run on alternating compute streams (reference views are
-independent, SURVEY.md 8e): two depth maps in flight fill the SMs that the latency-bound kernels of one map (token linears,
-FMT, U-Net layers) leave idle - measured +8.7 % depth maps / s on B200 at the DTU size (tools/two_stream_probe.py),
-bit-identical results - BUT the stage-1 attention kernel deadlocks about once in several hundred launches when kernels of
-another stream run next to it (every warp parked on an mbarrier whose tcgen05.commit never arrives; GPU core dump analysis
-in DESIGN.md 5, still unresolved), which the bounded waits turn into a sticky CUDA error.  Do not enable it in production.
+Off by default: with `lanes` > 1 consecutive batches run on alternating compute streams (reference views are
+independent, SURVEY.md 8e), so that two depth maps in flight can fill the SMs that the latency-bound kernels of one map
+(token linears, FMT, U-Net layers) leave idle.
 
 The reference's test loop uploads synchronously (`sample_cuda = tocuda(sample)` then `model.forward(...)`,
 test.py / base trainer); this is the drop-in equivalent for a caller that already holds the feature pyramids on the

@@ -113,11 +113,13 @@ def test_validate_args_rejects_hard_coded_transformer_options():
 
 def test_reference_arm_reproduces_golden_fixture():
     """bench.py --impl reference runs the reference's own modules through oracle/ref_hotpath.py (from oracle/_ref, the
-    build-time copy, or /root/reference): it must reproduce the committed reference-executed fixture bit for bit."""
+    build-time copy): it must reproduce the committed reference-executed fixture to fp32 rounding.  Bit equality only
+    holds on the CPU that made the fixture: the reference's fp32 convolutions and GEMMs round differently on hosts with
+    another SIMD width (measured: 2e-7 relative on the depth map)."""
     from oracle import ref_hotpath as RH
     if RH.reference_root() is None:
-        pytest.skip("no reference sources (oracle/_ref not built and /root/reference absent)")
-    from tests.common import TMP, build_case, load_golden
+        pytest.skip("no reference sources (oracle/_ref is made by build() only where the reference is available)")
+    from tests.common import TMP, build_case, load_golden, max_abs, rel_linf
     gold, meta = load_golden("hotpath_v4_64x96")
     args, params, sd, feats, proj, dv = build_case(meta)
     R = RH.import_reference()
@@ -125,23 +127,26 @@ def test_reference_arm_reproduces_golden_fixture():
     model = RH.RefHotPath(R, args).eval()
     model.load_state_dict(sd, strict=True)
     out = RH.reference_hotpath(R, model, args, feats, proj, dv, TMP, capture=False)
-    assert torch.equal(out["refined_depth"][0], gold["refined_depth"])
-    assert torch.equal(out["photometric_confidence"][0], gold["photometric_confidence"])
+    assert rel_linf(out["refined_depth"][0], gold["refined_depth"]) < 1e-5
+    assert max_abs(out["photometric_confidence"][0], gold["photometric_confidence"]) < 1e-5
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/models"), reason="reference repository only exists in the build container")
 def test_install_on_reference_constructed_model_keeps_the_checkpoint_contract():
     """test.py:209-220 on the real thing: init_model -> DINOv2MVSNet(arch.args); install() swaps FMT_module / fusions for
     this package's modules; every state-dict key and value of the model is unchanged, so a reference checkpoint loads with
     strict=True before or after install()."""
     import json
     import sys
-    sys.path.insert(0, "/root/reference")
+    from oracle import ref_hotpath as RH
+    root = RH.reference_root()
+    if root is None or not os.path.isfile(os.path.join(root, "config", "mvsformer++.json")):
+        pytest.skip("no reference sources (oracle/_ref is made by build() only where the reference is available)")
+    sys.path.insert(0, root)
     import models.dino.layers.attention as A
     A.FLASH_AVAILABLE = False
     from models.networks.DINOv2_mvsformer_model import DINOv2MVSNet
     from mvsformerplusplus_b200 import hotpath
-    cfg = json.load(open("/root/reference/config/mvsformer++.json"))["arch"]["args"]
+    cfg = json.load(open(os.path.join(root, "config", "mvsformer++.json")))["arch"]["args"]
     torch.manual_seed(0)
     model = DINOv2MVSNet(cfg).eval()
     synth.randomize_state_dict(model.FMT_module, seed=3)

@@ -1,4 +1,4 @@
-"""Runs a few hot-path forwards at a named workload for ncu / timing breakdowns.
+"""Runs a few hot-path forwards at a named workload for timing breakdowns.
   python tools/profile_forward.py [--workload dtu] [--iters 2] [--breakdown]"""
 import argparse
 import json
