@@ -3,31 +3,37 @@
 //
 // One CTA works on one 128-query tile of one head (head dim 16).
 //   warp 8        bulk-copy producer: K / V^T tiles (pre-tiled by qkv_tile_kernel into the canonical K-major layouts, 4 KB
-//                 and 12 KB) through two mbarrier rings of NKV stages
+//                 and 10 KB) through two mbarrier rings of NKV stages
 //   warps 0-7     two warpgroups of 64 query rows each.  Per 128-key tile: S = Q_lo K_hi + Q_hi K_lo + Q_hi K_hi (three
 //                 m64n128k16 MMAs, fp32 scores in registers), online softmax (a row lives in the 4 threads of a quad), P
 //                 rounded to fp16 IN REGISTERS and used directly as the A operand of the P*V MMAs against
-//                 [V_lo | V_hi | 1] (N = 48): the ones row of V makes the tensor core produce the softmax normaliser of the
-//                 tile as well.  The tile's partial products are added (round to nearest) while folding the tile into
-//                 the running output.  The two warpgroups of a CTA (and the CTAs of an SM) interleave their softmax and
-//                 MMA phases on the SM's schedulers.
+//                 [V_lo | V_hi | 1 | 0] (N = 40): the ones row of V makes the tensor core produce the softmax normaliser of
+//                 the tile as well.  The tile's partial products are added (round to nearest) while folding the tile into
+//                 the running output.
+// Schedule (after FlashAttention-3): each warpgroup issues the scores of tile j+1 and P*V of tile j back to back; the
+// softmax of tile j+1 runs once the scores are complete (wgmma.wait_group 1) while P*V of tile j is still in flight, and
+// tile j is folded into the output after it.  Measured on an H100 SXM at 700 W (N = 27 648): 1.51-1.55 ms per launch
+// against 1.72-1.73 ms for a loop that waits for each product before its softmax.  Variants measured slower on the same
+// kind of card and dropped: a named-barrier ping-pong that alternates the two warpgroups' MMA issue (+4 %), and
+// computing 1/8 or 1/4 of the exponentials with a polynomial on the FMA pipe as FlashAttention-4 does
+// (+3 % and +9 % on top of the ping-pong loop).
 #pragma once
 
 namespace fa {
 using namespace gmma;
 constexpr int NCONS = 256, THREADS = NCONS + 32, NKV = 3;
 constexpr uint32_t TILE = 4096;                 // one canonical 128 x 16 (Q, K) fp16 tile
-constexpr uint32_t LBO_QK = 2048, LBO_V = 768;  // k-chunk strides: Q/K 128 rows; V^T 48 rows = V_lo dims | V_hi dims | ones row + 15 zero rows
-constexpr uint32_t V_TILE = 16 * LBO_V;         // 12 KB
+constexpr uint32_t LBO_QK = 2048, LBO_V = 640;  // k-chunk strides: Q/K 128 rows; V^T 40 rows = V_lo dims | V_hi dims | ones row + 7 zero rows
+constexpr uint32_t V_TILE = 16 * LBO_V;         // 10 KB
 // Q (hi, lo) | K ring (hi, lo) | V ring | barriers
 constexpr uint32_t OFF_Q = 0, OFF_K = 2 * TILE, OFF_V = OFF_K + NKV * 2 * TILE, OFF_BAR = OFF_V + NKV * V_TILE;
 constexpr uint32_t SMEM = OFF_BAR + 8 + 32 * NKV;
 }  // namespace fa
 
 // tiled layout: planes Qh, Ql, Kh, Kl of 4 heads x ntiles x 2048 halves (tile = [2 k-chunks][128 rows][8]) and one V plane
-// of 4 heads x ntiles x 6144 halves: V^T tile = [16 k-chunks of 8 keys][48 rows][8 keys] with rows 0-15 = dims of V_lo,
-// 16-31 = dims of V_hi, row 32 = ones (its product with P is the softmax normaliser of the tile), rows 33-47 = zero.
-// P_hi multiplies all 48 rows (N = 48), P_lo rows 16-47 (N = 32: V_hi and the ones row).  Rows / keys >= N of Q, K, V are zero.
+// of 4 heads x ntiles x 5120 halves: V^T tile = [16 k-chunks of 8 keys][40 rows][8 keys] with rows 0-15 = dims of V_lo,
+// 16-31 = dims of V_hi, row 32 = ones (its product with P is the softmax normaliser of the tile), rows 33-39 = zero.
+// P_hi multiplies all 40 rows (N = 40), P_lo rows 16-39 (N = 24: V_hi and the ones row).  Rows / keys >= N of Q, K, V are zero.
 __global__ void qkv_tile_kernel(const float* __restrict__ qkv, __half* __restrict__ tiled, int N, int ntiles, float qscale) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;   // (token, which, head, octet of 8 dims)
   const int total = ntiles * 128 * 3 * 4 * 2;
@@ -53,25 +59,100 @@ __global__ void qkv_tile_kernel(const float* __restrict__ qkv, __half* __restric
     __half* pl = ph + plane;
     split_store8(ph + oct * 1024 + r * 8, pl + oct * 1024 + r * 8, v);
   } else {
-    __half* pv = tiled + (size_t)4 * plane + ((size_t)h * ntiles + tile) * 6144;
+    __half* pv = tiled + (size_t)4 * plane + ((size_t)h * ntiles + tile) * 5120;
     const int kc = r >> 3, e = r & 7;
 #pragma unroll
     for (int d = 0; d < 8; ++d) {
       __half hi, lo;
       split_f16(v[d], hi, lo);
-      pv[kc * 384 + (oct * 8 + d) * 8 + e] = lo;
-      pv[kc * 384 + (16 + oct * 8 + d) * 8 + e] = hi;
+      pv[kc * 320 + (oct * 8 + d) * 8 + e] = lo;
+      pv[kc * 320 + (16 + oct * 8 + d) * 8 + e] = hi;
     }
     if (oct == 0) {
-      pv[kc * 384 + 32 * 8 + e] = __float2half_rn(1.0f);
-#pragma unroll
-      for (int z = 33; z < 40; ++z) pv[kc * 384 + z * 8 + e] = __float2half_rn(0.f);
+      pv[kc * 320 + 32 * 8 + e] = __float2half_rn(1.0f);
     } else {
 #pragma unroll
-      for (int z = 40; z < 48; ++z) pv[kc * 384 + z * 8 + e] = __float2half_rn(0.f);
+      for (int z = 33; z < 40; ++z) pv[kc * 320 + z * 8 + e] = __float2half_rn(0.f);
     }
   }
 }
+
+namespace fa {
+using namespace gmma;
+// S = Q_lo K_hi + Q_hi K_lo + Q_hi K_hi of the K tile at kt (issued and committed, not waited for)
+__device__ __forceinline__ void issue_scores(float (&S)[64], uint64_t q_hi, uint64_t q_lo, uint32_t kt) {
+  const uint64_t k_hi = make_desc(kt, LBO_QK, 128), k_lo = make_desc(kt + TILE, LBO_QK, 128);
+  mma_ss<128>(S, q_lo, k_hi, 0u);
+  mma_ss<128>(S, q_hi, k_lo, 1u);
+  mma_ss<128>(S, q_hi, k_hi, 1u);
+  wg_commit();
+}
+// O columns: [P V_lo (16) | P V_hi (16) | sum of P (1) | 0 (7)];  P_lo multiplies [V_hi | 1 | 0] onto columns 16..39
+template <bool PLO>
+__device__ __forceinline__ void issue_pv(float (&O)[20], const uint32_t (&ph)[8][4], const uint32_t (&pl)[8][4], uint32_t vt) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    mma_rs_n40(O, ph[i], make_desc(vt + 2 * i * LBO_V, LBO_V, 128), i > 0 ? 1u : 0u);
+    if (PLO) mma_rs_n24(O + 8, pl[i], make_desc(vt + 2 * i * LBO_V + 256, LBO_V, 128), 1u);
+  }
+  wg_commit();
+}
+// online softmax of score tile j, in place: S becomes 2^(S - m + 14) for the updated running maxima m of the thread's two
+// rows, corr = 2^(m_old - m)
+__device__ __forceinline__ void softmax_tile(float (&S)[64], float (&m)[2], float (&corr)[2], int j, int N, int q) {
+  if (j * 128 + 128 > N) {                 // last, partial tile only: keys >= N never win the max and get P = 0
+#pragma unroll
+    for (int i = 0; i < 64; ++i)
+      if (j * 128 + 8 * (i >> 2) + 2 * q + (i & 1) >= N) S[i] = -1e30f;
+  }
+  float mb[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float pmax = -1e30f;
+#pragma unroll
+    for (int b = 0; b < 16; ++b) pmax = fmaxf(pmax, fmaxf(S[4 * b + 2 * h], S[4 * b + 2 * h + 1]));
+    pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 1));
+    pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 2));
+    const float mx = fmaxf(m[h], pmax);
+    corr[h] = ex2f(m[h] - mx);
+    m[h] = mx;
+    // P is stored as fp16 (hi + lo): scale it by 2^14 (largest element 16384 < 65504) so that probabilities down to 4e-12
+    // survive - without the bias every p < 3e-8 underflows to zero, a SYSTEMATIC loss of up to N * 3e-8 in the
+    // normaliser for peaked rows.  The factor cancels in O / l.
+    mb[h] = mx - 14.0f;
+  }
+#pragma unroll
+  for (int i = 0; i < 64; ++i) S[i] = ex2f(S[i] - mb[(i >> 1) & 1]);
+}
+// P as the A operand of the P*V MMAs: k-step i (keys 16 i .. 16 i + 15) = registers 8 i .. 8 i + 7 of S
+template <bool PLO>
+__device__ __forceinline__ void pack_p(const float (&S)[64], uint32_t (&ph)[8][4], uint32_t (&pl)[8][4]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const float p0 = S[8 * i + 2 * r], p1 = S[8 * i + 2 * r + 1];
+      const __half2 hh = __floats2half2_rn(p0, p1);
+      ph[i][r] = *reinterpret_cast<const uint32_t*>(&hh);
+      if (PLO) {
+        const float2 hf = __half22float2(hh);
+        pl[i][r] = pack_half2(p0 - hf.x, p1 - hf.y);
+      }
+    }
+}
+// running output and normaliser of the thread's two rows <- tile (O, corr)
+__device__ __forceinline__ void fold_tile(float (&o)[2][4], float (&l)[2], const float (&O)[20], const float (&corr)[2], int lane) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int b = 0; b < 2; ++b)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) o[h][2 * b + e] = fmaf(o[h][2 * b + e], corr[h], O[4 * b + 2 * h + e] + O[4 * (b + 2) + 2 * h + e]);
+    const float lt = __shfl_sync(0xffffffffu, O[16 + 2 * h], lane & ~3);   // column 32 sits in the quad's first thread
+    l[h] = fmaf(l[h], corr[h], lt);
+  }
+}
+}  // namespace fa
 
 // PLO = true : P = P_hi + P_lo (22 mantissa bits), three partial products P_hi V_lo + P_hi V_hi + P_lo V_hi  (round-1 kernel)
 // PLO = false: P = P_hi only (fp16, 11 bits; the SAME rounded P feeds the numerator and the normaliser, so the rounding is an
@@ -93,7 +174,8 @@ attention_fa_kernel(const __half* __restrict__ tiled, float* __restrict__ out, _
                  bar_ve = bar_vf + 8 * NKV;
   if (tid == 0) {
     mbar_init(bar_q, 1);
-    // a K / V stage is free once both warpgroups' products that read it are complete
+    // a K / V stage is free once both warpgroups' products that read it are complete (K and V are released at different
+    // points of the loop, each by one thread per warpgroup)
     for (int i = 0; i < NKV; ++i) { mbar_init(bar_kf + 8 * i, 1); mbar_init(bar_ke + 8 * i, 2); mbar_init(bar_vf + 8 * i, 1); mbar_init(bar_ve + 8 * i, 2); }
     fence_barrier_init();
   }
@@ -114,7 +196,7 @@ attention_fa_kernel(const __half* __restrict__ tiled, float* __restrict__ out, _
         bulk_load(sb + OFF_K + (2 * s + 1) * TILE, base + 3 * plane + (size_t)t * 2048, TILE, bar_kf + 8 * s);
         mbar_wait(bar_ve + 8 * s, par);
         expect_tx(bar_vf + 8 * s, V_TILE);
-        bulk_load(sb + OFF_V + s * V_TILE, tiled + 4 * plane + ((size_t)head * ntiles + t) * 6144, V_TILE, bar_vf + 8 * s);
+        bulk_load(sb + OFF_V + s * V_TILE, tiled + 4 * plane + ((size_t)head * ntiles + t) * (V_TILE / 2), V_TILE, bar_vf + 8 * s);
       }
     }
     return;
@@ -123,7 +205,7 @@ attention_fa_kernel(const __half* __restrict__ tiled, float* __restrict__ out, _
   // thread (warpgroup wg, warp wq of it, lane): query rows 64 wg + 16 wq + lane / 4 + 8 h (h = 0, 1); score columns
   // 8 b + 2 (lane % 4) + e of accumulator register 4 b + 2 h + e
   const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
-  const int t128 = tid & 127;
+  const bool leader = (tid & 127) == 0;
   const uint64_t q_hi = make_desc(sb + OFF_Q + wg * 1024, LBO_QK, 128), q_lo = make_desc(sb + OFF_Q + TILE + wg * 1024, LBO_QK, 128);
   float o[2][4];   // per row: head dims 2q, 2q + 1, 8 + 2q, 9 + 2q
   float m[2] = {-1e30f, -1e30f}, l[2] = {0.f, 0.f};
@@ -131,80 +213,52 @@ attention_fa_kernel(const __half* __restrict__ tiled, float* __restrict__ out, _
   for (int h = 0; h < 2; ++h)
 #pragma unroll
     for (int d = 0; d < 4; ++d) o[h][d] = 0.f;
+  float S[64], O[20], corr[2];
+  uint32_t ph[8][4], pl[8][4];
   mbar_wait(bar_q, 0u);
-  for (int j = 0; j < ntiles; ++j) {
-    const int s = j % NKV;
-    const uint32_t par = (uint32_t)((j / NKV) & 1);
-    mbar_wait(bar_kf + 8 * s, par);
-    float S[64];
-    const uint32_t kt = sb + OFF_K + (2 * s) * TILE;
-    const uint64_t k_hi = make_desc(kt, LBO_QK, 128), k_lo = make_desc(kt + TILE, LBO_QK, 128);
+  mbar_wait(bar_kf, 0u);
+  wg_fence();
+  issue_scores(S, q_hi, q_lo, sb + OFF_K);     // scores of tile 0
+  wg_wait<0>();
+  fence_regs<64>(S);
+  if (leader) mbar_arrive(bar_ke);
+  softmax_tile(S, m, corr, 0, N, q);
+  pack_p<PLO>(S, ph, pl);
+  if (ntiles > 1) {                            // operands of iteration 0
+    mbar_wait(bar_kf + 8, 0u);
+    mbar_wait(bar_vf, 0u);
+  }
+  // iteration j: scores of tile j + 1 and P*V of tile j; the softmax of tile j + 1 overlaps P*V of tile j
+  for (int j = 0; j + 1 < ntiles; ++j) {
+    const int s = j % NKV, s1 = (j + 1) % NKV, s2 = (j + 2) % NKV;
     wg_fence();
-    mma_ss<128>(S, q_lo, k_hi, 0u);
-    mma_ss<128>(S, q_hi, k_lo, 1u);
-    mma_ss<128>(S, q_hi, k_hi, 1u);
-    wg_commit();
-    wg_wait<0>();
+    issue_scores(S, q_hi, q_lo, sb + OFF_K + (2 * s1) * TILE);
+    issue_pv<PLO>(O, ph, pl, sb + OFF_V + s * V_TILE);
+    wg_wait<1>();                              // the scores (the older group) are complete, P*V may still run
     fence_regs<64>(S);
-    if (t128 == 0) mbar_arrive(bar_ke + 8 * s);
-    if (j * 128 + 128 > N) {                 // last, partial tile only: keys >= N never win the max and get P = 0
-#pragma unroll
-      for (int i = 0; i < 64; ++i)
-        if (j * 128 + 8 * (i >> 2) + 2 * q + (i & 1) >= N) S[i] = -1e30f;
-    }
-    float corr[2], mb[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float pmax = -1e30f;
-#pragma unroll
-      for (int b = 0; b < 16; ++b) pmax = fmaxf(pmax, fmaxf(S[4 * b + 2 * h], S[4 * b + 2 * h + 1]));
-      pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 1));
-      pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 2));
-      const float mx = fmaxf(m[h], pmax);
-      corr[h] = ex2f(m[h] - mx);
-      m[h] = mx;
-      // P is stored as fp16 (hi + lo): scale it by 2^14 (largest element 16384 < 65504) so that probabilities down to 4e-12
-      // survive - without the bias every p < 3e-8 underflows to zero, a SYSTEMATIC loss of up to N * 3e-8 in the
-      // normaliser for peaked rows.  The factor cancels in O / l.
-      mb[h] = mx - 14.0f;
-    }
-    // P as the A operand of the P*V MMAs: k-step i (keys 16 i .. 16 i + 15) = registers 8 i .. 8 i + 7 of S
-    uint32_t ph[8][4], pl[8][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const float p0 = ex2f(S[8 * i + 2 * r] - mb[r & 1]), p1 = ex2f(S[8 * i + 2 * r + 1] - mb[r & 1]);
-        const __half2 hh = __floats2half2_rn(p0, p1);
-        ph[i][r] = *reinterpret_cast<const uint32_t*>(&hh);
-        if (PLO) {
-          const float2 hf = __half22float2(hh);
-          pl[i][r] = pack_half2(p0 - hf.x, p1 - hf.y);
-        }
-      }
-    mbar_wait(bar_vf + 8 * s, par);
-    // O columns: [P V_lo (16) | P V_hi (16) | sum of P (1) | 0 (15)];  P_lo multiplies [V_hi | 1] onto columns 16..47
-    float O[24];
-    const uint32_t vt = sb + OFF_V + s * V_TILE;
-    wg_fence();
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      mma_rs_n48(O, ph[i], make_desc(vt + 2 * i * LBO_V, LBO_V, 128), i > 0 ? 1u : 0u);
-      if (PLO) mma_rs_n32(O + 8, pl[i], make_desc(vt + 2 * i * LBO_V + 256, LBO_V, 128), 1u);
-    }
-    wg_commit();
+    if (leader) mbar_arrive(bar_ke + 8 * s1);
+    float corr1[2];
+    softmax_tile(S, m, corr1, j + 1, N, q);
+    // operands of the next iteration.  Waiting for them here, between the softmax and the wait for P*V, also keeps ptxas
+    // from hoisting that wait above the softmax: it does not move it across the polling loop.
+    if (j + 2 < ntiles) mbar_wait(bar_kf + 8 * s2, (uint32_t)(((j + 2) / NKV) & 1));
+    mbar_wait(bar_vf + 8 * s1, (uint32_t)(((j + 1) / NKV) & 1));
     wg_wait<0>();
-    fence_regs<24>(O);
-    if (t128 == 0) mbar_arrive(bar_ve + 8 * s);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-#pragma unroll
-      for (int b = 0; b < 2; ++b)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) o[h][2 * b + e] = fmaf(o[h][2 * b + e], corr[h], O[4 * b + 2 * h + e] + O[4 * (b + 2) + 2 * h + e]);
-      const float lt = __shfl_sync(0xffffffffu, O[16 + 2 * h], lane & ~3);   // column 32 sits in the quad's first thread
-      l[h] = fmaf(l[h], corr[h], lt);
-    }
+    fence_regs<20>(O);
+    if (leader) mbar_arrive(bar_ve + 8 * s);
+    fold_tile(o, l, O, corr, lane);
+    pack_p<PLO>(S, ph, pl);
+    corr[0] = corr1[0];
+    corr[1] = corr1[1];
+  }
+  {                                            // P*V of the last tile
+    const int j = ntiles - 1, s = j % NKV;
+    mbar_wait(bar_vf + 8 * s, (uint32_t)((j / NKV) & 1));
+    wg_fence();
+    issue_pv<PLO>(O, ph, pl, sb + OFF_V + s * V_TILE);
+    wg_wait<0>();
+    fence_regs<20>(O);
+    fold_tile(o, l, O, corr, lane);
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
