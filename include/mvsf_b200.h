@@ -187,6 +187,28 @@ int mvsf_fmt_forward(const float* f1, const float* f2, const float* f3, const fl
                      const float* wts, const void* wts16, size_t n_wts, float* o1, float* o2, float* o3, float* o4,
                      void* workspace, size_t workspace_bytes, int V, int H1, int W1, mvsf_stream_t stream);
 
+/* ---- P1: models/module.py:208-239 FPNEncoder.forward (feat_chs [8,16,32,64], norm_type 'BN', eval; every layer
+ *      Conv2d(bias=False) -> BatchNorm folded -> LeakyReLU(0.1), module.py:61-80).
+ * x [N][3][H][W] (H, W positive multiples of 8) -> c01 [N][H][W][8], c11 [N][H/2][W/2][16], c21 [N][H/4][W/4][32],
+ * c31 [N][H/8][W/8][64] (NHWC).  wts: packing.pack_fpn_encoder (per layer w [KS*KS][CI][CO] with BN scale folded, then
+ * the folded shift [CO], layers conv00, conv01, downsample1, conv10, conv11, downsample2, conv20, conv21, downsample3,
+ * conv30, conv31); wts_tc = mvsf_fpn_pack_tc(0, wts).  Bad shapes: -1, nothing launched. */
+int mvsf_fpn_encoder_workspace_bytes(int N, int H, int W, size_t* bytes);
+int mvsf_fpn_encoder_forward(const float* x, const float* wts, const void* wts_tc, float* c01, float* c11, float* c21,
+                             float* c31, void* workspace, size_t workspace_bytes, int N, int H, int W, mvsf_stream_t stream);
+/* ---- P2: models/module.py:242-270 FPNDecoder.forward (F.interpolate bilinear, align_corners=True; BN folded).
+ * c01..c31 as the encoder writes them (NHWC, full-resolution H x W) -> o0 [N][64][H/8][W/8], o1 [N][32][H/4][W/4],
+ * o2 [N][16][H/2][W/2], o3 [N][8][H][W] (NCHW: the layout mvsf_fmt_forward reads, DINOv2_mvsformer_model.py:95-98).
+ * wts: packing.pack_fpn_decoder (out0 [64 ci][64 co] + shift[64]; per level k: inner_k [CL][64] + bias[64], then out_k
+ * [9][64][C_k] + shift[C_k]); wts_tc = mvsf_fpn_pack_tc(1, wts).  The full-resolution intra feature never reaches HBM. */
+int mvsf_fpn_decoder_workspace_bytes(int N, int H, int W, size_t* bytes);
+int mvsf_fpn_decoder_forward(const float* c01, const float* c11, const float* c21, const float* c31, const float* wts,
+                             const void* wts_tc, float* o0, float* o1, float* o2, float* o3, void* workspace,
+                             size_t workspace_bytes, int N, int H, int W, mvsf_stream_t stream);
+/* install time: fp32 blob -> fp16 hi/lo weight tiles of the wgmma convolutions (csrc/fpn.cu); part 0 encoder, 1 decoder */
+int mvsf_fpn_tc_bytes(int part, size_t* bytes);
+int mvsf_fpn_pack_tc(int part, const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -47,6 +47,12 @@ SIGNATURES = {
     "mvsf_conf_accumulate": ([P, I, I, P, I, I, F, I, P], I),
     "mvsf_fmt_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
     "mvsf_fmt_forward": ([P] * 7 + [Z] + [P] * 5 + [Z, I, I, I, P], I),
+    "mvsf_fpn_encoder_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
+    "mvsf_fpn_encoder_forward": ([P] * 8 + [Z, I, I, I, P], I),
+    "mvsf_fpn_decoder_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
+    "mvsf_fpn_decoder_forward": ([P] * 11 + [Z, I, I, I, P], I),
+    "mvsf_fpn_tc_bytes": ([I, ctypes.POINTER(Z)], I),
+    "mvsf_fpn_pack_tc": ([I, P, P, Z, P], I),
 }
 
 

@@ -1,0 +1,488 @@
+// FPN feature pyramid: models/module.py:208-239 FPNEncoder and :242-270 FPNDecoder (eval, feat_chs [8,16,32,64], BN folded).
+// Every 3x3 / 5x5 convolution is one launch of fpn_conv_kernel, an implicit GEMM on wgmma in the scheme of vis_cnn.cu and
+// fmt_smooth_tc.cuh:
+//   phase 1 (SIMT)   a "source" writes the input of the layer for one output tile plus its halo as fp16 hi|lo voxel-octet
+//                    PLANES in shared memory (plane[row][col] = 8 channels = 16 B; zero outside the image = the padding), so
+//                    a tap is a descriptor start address.  Strided layers use S x S PARITY planes (conv3d_tc.cu): plane
+//                    (py, px) holds input rows S i + py, columns S j + px, and tap (kh, kw) of output (r, c) is row
+//                    r + kh / S, column c + kw / S of parity plane (kh % S, kw % S).
+//   phase 2 (wgmma)  M = 8 x 8 output pixels per m64 block, N = NS output channels of the CTA's N block.  Per 16 input
+//                    channels: x_hi x [w_hi | w_lo] (N = 2 NS) and x_lo x w_hi (N = NS, onto the first half); 8 input
+//                    channels: one MMA [x_hi | x_lo] x [[w_hi; w_hi] | [w_lo; 0]].  fp32 accumulators in registers.
+//   phase 3          folded bias (+ BN) and LeakyReLU(0.1) -> NHWC fp32 (encoder), or Swish -> NCHW fp32 (decoder).
+// Sources: an NHWC fp32 tensor (encoder layers), conv00 computed in SIMT from the [N][3][H][W] image (fused conv00 + conv01:
+// conv00's output never reaches HBM), and the decoder's intra_k = up2(intra_{k-1}) + inner_k(lateral_k) (align_corners=True
+// bilinear + 1x1 conv with bias; the tile interior of intra_1 / intra_2 is also stored for the next level, the
+// full-resolution intra_3 is not).  out0 (1x1 at 1/8 resolution) is a small SIMT kernel.
+#include "common.cuh"
+#include "linear_tc.cuh"
+#include "wgmma.cuh"
+
+namespace mvsf {
+namespace fpn {
+using namespace gmma;
+
+// one layer: CI -> CO channels, KS x KS kernel, stride S, output tile TR rows x 32 columns, NS output channels per CTA
+template <int CI_, int CO_, int KS_, int S_, int TR_, int NS_>
+struct Conv {
+  static constexpr int CI = CI_, CO = CO_, KS = KS_, S = S_, TR = TR_, NS = NS_;
+  static constexpr int PAD = (KS - 1) / 2, HALO = (KS - 1) / S;
+  static constexpr int PR = TR + HALO, PC = 32 + HALO;          // plane rows / columns
+  static constexpr int NO = CI / 8, NP = S * S, NG = CI < 16 ? 1 : CI / 16, NB = CO / NS;
+  static constexpr uint32_t PLANE = PR * PC * 16, PITCH = PC * 16;
+  static constexpr uint32_t BT = 64 * NS;                      // (tap, group) weight tile: [2 k-chunks][2 NS rows][8 halves]
+  static constexpr uint32_t WBYTES = KS * KS * NG * BT;        // weight tiles of one N block
+  static constexpr uint32_t OFF_W = NP * NO * 2 * PLANE, SMEM = OFF_W + WBYTES;
+  static_assert(CI % 8 == 0 && (CI == 8 || CI % 16 == 0) && CO % NS == 0 && TR % 8 == 0, "fpn conv shape");
+  static_assert(NS == 8 || NS == 16 || NS == 32, "fpn conv N block");
+  // plane of parity `par`, channel octet o, part hl (0 hi, 1 lo): groups of 16 channels are [hi o | lo o | hi o+1 | lo o+1]
+  __device__ static constexpr uint32_t plane(int par, int o, int hl) { return (uint32_t)((par * NO + o) * 2 + hl) * PLANE; }
+};
+
+// ---- sources (phase 1).  fill() is called by all 256 threads; the planes it writes are read after a fence + barrier.
+// input NHWC fp32 [N][IH][IW][CI]
+template <class L>
+struct NhwcSrc {
+  const float* in;
+  int IH, IW;
+  static constexpr uint32_t EXTRA = 0;
+  __device__ void fill(unsigned char* smem, int n, int y0, int x0, int tid) const {
+    constexpr int NPIX = L::PR * L::PC;
+    for (int i = tid; i < L::NP * NPIX * L::NO; i += 256) {
+      const int o = i % L::NO, rest = i / L::NO;
+      const int pix = rest % NPIX, par = rest / NPIX;
+      const int r = pix / L::PC, c = pix - r * L::PC;
+      const int iy = L::S * (y0 + r) - L::PAD + par / L::S, ix = L::S * (x0 + c) - L::PAD + par % L::S;
+      float v[8];
+      if (iy >= 0 && iy < IH && ix >= 0 && ix < IW) {
+        const float* p = in + (((size_t)n * IH + iy) * IW + ix) * L::CI + o * 8;
+        const float4 a = ldg4(p), b = ldg4(p + 4);
+        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+      } else {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) v[e] = 0.f;
+      }
+      __half* h = reinterpret_cast<__half*>(smem + L::plane(par, o, 0) + (uint32_t)pix * 16u);
+      split_store8(h, h + L::PLANE / 2, v);   // lo plane = + PLANE bytes
+    }
+  }
+};
+
+// conv00 (3 -> 8, 7x7, pad 3, folded BN, LeakyReLU) in SIMT from the image x [N][3][H][W]; w = [49 taps][3 ci][8 co], b[8]
+template <class L>
+struct Conv00Src {
+  const float* x;
+  const float* w;
+  int H, W;
+  static constexpr int IR = L::PR + 6, IC = L::PC + 6, NW = 49 * 3 * 8 + 8;
+  static constexpr uint32_t EXTRA = (3 * IR * IC + NW) * 4;
+  static_assert(L::CI == 8 && L::S == 1, "conv00 feeds an 8-channel stride-1 layer");
+  __device__ void fill(unsigned char* smem, int n, int y0, int x0, int tid) const {
+    float* in_s = reinterpret_cast<float*>(smem + L::SMEM);
+    float* ws = in_s + 3 * IR * IC;
+    for (int i = tid; i < NW; i += 256) ws[i] = __ldg(w + i);
+    const float* xn = x + (size_t)n * 3 * H * W;
+    for (int i = tid; i < 3 * IR * IC; i += 256) {
+      const int ch = i / (IR * IC), rem = i - ch * (IR * IC);
+      const int r = rem / IC, c = rem - r * IC;
+      const int gy = y0 - L::PAD - 3 + r, gx = x0 - L::PAD - 3 + c;
+      in_s[i] = (gy >= 0 && gy < H && gx >= 0 && gx < W) ? __ldg(xn + ((size_t)ch * H + gy) * W + gx) : 0.f;
+    }
+    __syncthreads();
+    for (int pix = tid; pix < L::PR * L::PC; pix += 256) {
+      const int r = pix / L::PC, c = pix - r * L::PC;
+      const int gy = y0 - L::PAD + r, gx = x0 - L::PAD + c;
+      float acc[8];
+#pragma unroll
+      for (int oc = 0; oc < 8; ++oc) acc[oc] = ws[NW - 8 + oc];
+      for (int ch = 0; ch < 3; ++ch)
+#pragma unroll
+        for (int ky = 0; ky < 7; ++ky)
+#pragma unroll
+          for (int kx = 0; kx < 7; ++kx) {
+            const float v = in_s[(ch * IR + r + ky) * IC + c + kx];
+            const float* wp = ws + ((ky * 7 + kx) * 3 + ch) * 8;
+#pragma unroll
+            for (int oc = 0; oc < 8; ++oc) acc[oc] = fmaf(v, wp[oc], acc[oc]);
+          }
+      const bool inside = gy >= 0 && gy < H && gx >= 0 && gx < W;
+#pragma unroll
+      for (int oc = 0; oc < 8; ++oc) acc[oc] = inside ? (acc[oc] > 0.f ? acc[oc] : 0.1f * acc[oc]) : 0.f;
+      __half* h = reinterpret_cast<__half*>(smem + L::plane(0, 0, 0) + (uint32_t)pix * 16u);
+      split_store8(h, h + L::PLANE / 2, acc);
+    }
+  }
+};
+
+// intra = F.interpolate(prev, scale_factor=2, bilinear, align_corners=True) + inner(lat):  prev [N][h][w][64],
+// lat [N][2h][2w][CL], w = inner [CL ci][64 co] then b[64]; intra_out (or NULL) receives the tile interior, NHWC fp32
+template <class L, int CL>
+struct IntraSrc {
+  const float* prev;
+  const float* lat;
+  const float* w;
+  float* intra_out;
+  int h, wd;
+  static constexpr uint32_t EXTRA = (CL * 64 + 64) * 4;
+  static_assert(L::CI == 64 && L::S == 1 && L::KS == 3, "decoder level: 3x3 conv of the 64-channel intra feature");
+  __device__ void fill(unsigned char* smem, int n, int y0, int x0, int tid) const {
+    float* ws = reinterpret_cast<float*>(smem + L::SMEM);
+    for (int i = tid; i < CL * 64 + 64; i += 256) ws[i] = __ldg(w + i);
+    __syncthreads();
+    const int H = 2 * h, W = 2 * wd;
+    // ATen area_pixel_compute_scale / source_index, align_corners=True: src = dst * (in - 1) / (out - 1)
+    const float scy = (float)(h - 1) / (float)(H - 1), scx = (float)(wd - 1) / (float)(W - 1);
+    const float* pv = prev + (size_t)n * h * wd * 64;
+    for (int i = tid; i < L::PR * L::PC * 8; i += 256) {
+      const int o = i & 7, pix = i >> 3;
+      const int r = pix / L::PC, c = pix - r * L::PC;
+      const int y = y0 - 1 + r, x = x0 - 1 + c;
+      float v[8];
+      if (y >= 0 && y < H && x >= 0 && x < W) {
+        const float sy = scy * (float)y, sx = scx * (float)x;
+        const int ya = (int)sy, yb = ya + (ya < h - 1 ? 1 : 0), xa = (int)sx, xb = xa + (xa < wd - 1 ? 1 : 0);
+        const float ly1 = sy - (float)ya, ly0 = 1.f - ly1, lx1 = sx - (float)xa, lx0 = 1.f - lx1;
+        const float* p00 = pv + ((size_t)ya * wd + xa) * 64 + o * 8;
+        const float* p01 = pv + ((size_t)ya * wd + xb) * 64 + o * 8;
+        const float* p10 = pv + ((size_t)yb * wd + xa) * 64 + o * 8;
+        const float* p11 = pv + ((size_t)yb * wd + xb) * 64 + o * 8;
+#pragma unroll
+        for (int q4 = 0; q4 < 2; ++q4) {
+          const float4 v00 = ldg4(p00 + q4 * 4), v01 = ldg4(p01 + q4 * 4), v10 = ldg4(p10 + q4 * 4), v11 = ldg4(p11 + q4 * 4);
+          const float a00[4] = {v00.x, v00.y, v00.z, v00.w}, a01[4] = {v01.x, v01.y, v01.z, v01.w};
+          const float a10[4] = {v10.x, v10.y, v10.z, v10.w}, a11[4] = {v11.x, v11.y, v11.z, v11.w};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float up = ly0 * (lx0 * a00[e] + lx1 * a01[e]) + ly1 * (lx0 * a10[e] + lx1 * a11[e]);
+            v[q4 * 4 + e] = up + ws[CL * 64 + o * 8 + q4 * 4 + e];
+          }
+        }
+        const float* lp = lat + (((size_t)n * H + y) * W + x) * CL;
+#pragma unroll 4
+        for (int ci = 0; ci < CL; ++ci) {
+          const float l = __ldg(lp + ci);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) v[e] = fmaf(l, ws[ci * 64 + o * 8 + e], v[e]);
+        }
+        if (intra_out != nullptr && r >= 1 && r <= L::TR && c >= 1 && c <= 32) {
+          float* op = intra_out + (((size_t)n * H + y) * W + x) * 64 + o * 8;
+          *reinterpret_cast<float4*>(op) = make_float4(v[0], v[1], v[2], v[3]);
+          *reinterpret_cast<float4*>(op + 4) = make_float4(v[4], v[5], v[6], v[7]);
+        }
+      } else {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) v[e] = 0.f;
+      }
+      __half* hp = reinterpret_cast<__half*>(smem + L::plane(0, o, 0) + (uint32_t)pix * 16u);
+      split_store8(hp, hp + L::PLANE / 2, v);
+    }
+  }
+};
+
+// ---- destinations (phase 3): two consecutive channels ch, ch + 1 of one output pixel, bias already added
+template <int CO>
+struct NhwcLeaky {   // encoder: LeakyReLU(0.1), [N][OH][OW][CO]
+  float* out;
+  __device__ void store(int n, int OH, int OW, int y, int x, int ch, float a, float b) const {
+    a = a > 0.f ? a : 0.1f * a;
+    b = b > 0.f ? b : 0.1f * b;
+    *reinterpret_cast<float2*>(out + (((size_t)n * OH + y) * OW + x) * CO + ch) = make_float2(a, b);
+  }
+};
+__device__ __forceinline__ float swish(float v) { return v / (1.0f + expf(-v)); }
+template <int CO>
+struct NchwSwish {   // decoder: Swish, [N][CO][OH][OW]
+  float* out;
+  __device__ void store(int n, int OH, int OW, int y, int x, int ch, float a, float b) const {
+    float* p = out + (((size_t)n * CO + ch) * OH + y) * OW + x;
+    p[0] = swish(a);
+    p[(size_t)OH * OW] = swish(b);
+  }
+};
+
+template <class L, class Src, class Dst>
+__global__ void __launch_bounds__(256)
+fpn_conv_kernel(const Src src, const Dst dst, const __half* __restrict__ wtc, const float* __restrict__ bias, int OH, int OW,
+                int tiles_x, int tiles_y, int ntiles) {
+  constexpr int NS = L::NS, KS = L::KS, S = L::S, NG = L::NG;
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int nb = blockIdx.y;
+  const uint32_t sb = smem_u32(smem);
+  // ---- once per CTA: the weight tiles of N block nb (packed at install time by mvsf_fpn_pack_tc)
+  {
+    const uint4* wsrc = reinterpret_cast<const uint4*>(wtc) + (size_t)nb * (L::WBYTES / 16);
+    uint4* wdst = reinterpret_cast<uint4*>(smem + L::OFF_W);
+    for (int i = tid; i < (int)(L::WBYTES / 16); i += 256) wdst[i] = __ldg(wsrc + i);
+  }
+  const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
+  float acc[2][NS];   // the m64 blocks of column groups 2 wg and 2 wg + 1: N = 2 NS accumulator columns [first | second]
+
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, n = tile / (tiles_x * tiles_y);
+    const int x0 = tx * 32, y0 = ty * L::TR;
+    src.fill(smem, n, y0, x0, tid);
+    fence_proxy_async();
+    __syncthreads();
+#pragma unroll 1
+    for (int rg = 0; rg < L::TR / 8; ++rg) {
+      wg_fence();
+#pragma unroll
+      for (int kh = 0; kh < KS; ++kh) {
+#pragma unroll
+        for (int kw = 0; kw < KS; ++kw) {
+          const int par = (kh % S) * S + (kw % S);
+          const uint32_t aoff = (uint32_t)((8 * rg + kh / S) * L::PC + kw / S) * 16u;
+#pragma unroll
+          for (int g = 0; g < NG; ++g) {
+            const uint64_t wb = make_desc(sb + L::OFF_W + (uint32_t)((kh * KS + kw) * NG + g) * L::BT, 2 * NS * 16, 128);
+            const uint32_t first = (kh | kw | g) ? 1u : 0u;
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+              const uint32_t arow = sb + aoff + (uint32_t)(2 * wg + k) * 128u;
+              if constexpr (L::CI == 8) {   // K = [hi | lo] planes of the single octet
+                mma_ss<2 * NS>(acc[k], make_desc(arow + L::plane(par, 0, 0), L::PLANE, L::PITCH), wb, first);
+              } else {                      // K chunks = the hi (or lo) planes of octets 2 g and 2 g + 1
+                const uint32_t ah = arow + L::plane(par, 2 * g, 0);
+                mma_ss<2 * NS>(acc[k], make_desc(ah, 2 * L::PLANE, L::PITCH), wb, first);
+                mma_ss<NS>(acc[k], make_desc(ah + L::PLANE, 2 * L::PLANE, L::PITCH), wb, 1u);
+              }
+            }
+          }
+        }
+      }
+      wg_commit();
+      wg_wait<0>();
+      fence_regs<NS>(acc[0]);
+      fence_regs<NS>(acc[1]);
+      // ---- epilogue: accumulator i of this thread = row 16 wq + lane / 4 + 8 h of the m64 block (pixel row 2 wq + h,
+      //      column lane / 4), column 8 b + 2 q + e (+ NS for the x_hi w_lo half)
+#pragma unroll
+      for (int k = 0; k < 2; ++k)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int y = y0 + 8 * rg + 2 * wq + h, x = x0 + 8 * (2 * wg + k) + (lane >> 2);
+          if (y >= OH || x >= OW) continue;
+#pragma unroll
+          for (int b = 0; b < NS / 8; ++b) {
+            const int ch = nb * NS + 8 * b + 2 * q;
+            const float o0 = acc[k][4 * b + 2 * h] + acc[k][4 * b + 2 * h + NS / 2] + __ldg(bias + ch);
+            const float o1 = acc[k][4 * b + 2 * h + 1] + acc[k][4 * b + 2 * h + 1 + NS / 2] + __ldg(bias + ch + 1);
+            dst.store(n, OH, OW, y, x, ch, o0, o1);
+          }
+        }
+    }
+    __syncthreads();   // planes are free again
+  }
+}
+
+// out0 = Swish(BN(conv1x1(conv31) + b)):  c31 [N][h][w][64] -> out [N][64][h][w];  w = [64 ci][64 co] then b[64]
+__global__ void __launch_bounds__(128) fpn_out0_kernel(const float* __restrict__ c31, const float* __restrict__ w,
+                                                        float* __restrict__ out, int HW, int npix) {
+  __shared__ float ws[64 * 64 + 64];
+  for (int i = threadIdx.x; i < 64 * 64 + 64; i += 128) ws[i] = __ldg(w + i);
+  __syncthreads();
+  const int p = blockIdx.x * 128 + threadIdx.x;
+  if (p >= npix) return;
+  const int n = p / HW, px = p - n * HW;
+  float xv[64];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const float4 t = ldg4(c31 + (size_t)p * 64 + 4 * i);
+    xv[4 * i] = t.x; xv[4 * i + 1] = t.y; xv[4 * i + 2] = t.z; xv[4 * i + 3] = t.w;
+  }
+#pragma unroll 4
+  for (int co = 0; co < 64; ++co) {
+    float s = ws[64 * 64 + co];
+#pragma unroll
+    for (int ci = 0; ci < 64; ++ci) s = fmaf(xv[ci], ws[ci * 64 + co], s);
+    out[((size_t)n * 64 + co) * HW + px] = swish(s);
+  }
+}
+
+// install time: fp32 [KS*KS taps][CI][CO] -> the weight tiles of fpn_conv_kernel, [N block][tap][group][2 kc][2 NS rows][8]
+__global__ void fpn_pack_kernel(const float* __restrict__ w, __half* __restrict__ out, int CI, int CO, int KK, int NS) {
+  const int NG = CI < 16 ? 1 : CI / 16;
+  const long long total = (long long)KK * NG * 64 * CO / 2;   // halves
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int e = (int)(i & 7);
+    long long rest = i >> 3;
+    const int row = (int)(rest % (2 * NS)); rest /= 2 * NS;
+    const int kc = (int)(rest & 1); rest >>= 1;
+    const int g = (int)(rest % NG); rest /= NG;
+    const int tap = (int)(rest % KK), nb = (int)(rest / KK);
+    const int part = row / NS, co = nb * NS + row % NS;
+    const int ci = CI == 8 ? e : g * 16 + kc * 8 + e;
+    const float wv = w[((size_t)tap * CI + ci) * CO + co];
+    const __half hi = __float2half_rn(wv), lo = __float2half_rn(wv - __half2float(hi));
+    __half v;
+    if (CI == 8) v = part == 0 ? hi : (kc == 0 ? lo : __float2half_rn(0.f));
+    else v = part == 0 ? hi : lo;
+    out[i] = v;
+  }
+}
+
+// ---- layer table.  fp32 blobs (packing.pack_fpn_encoder / pack_fpn_decoder): per layer w [KS*KS][CI][CO] then b[CO]
+struct LayerDesc { int ci, co, ks, ns; };
+constexpr LayerDesc kEnc[11] = {{3, 8, 7, 0},    {8, 8, 5, 8},    {8, 16, 5, 16},  {16, 16, 3, 16},
+                                {16, 16, 3, 16}, {16, 32, 5, 32}, {32, 32, 3, 32}, {32, 32, 3, 32},
+                                {32, 64, 3, 32}, {64, 64, 3, 32}, {64, 64, 3, 32}};
+// decoder blob: out0 [64][64] b[64]; then per level k = 1..3: inner_k [CL][64] b[64], out_k [9][64][C_k] b[C_k]
+constexpr LayerDesc kDec[3] = {{64, 32, 3, 32}, {64, 16, 3, 16}, {64, 8, 3, 8}};
+constexpr int kLat[3] = {32, 16, 8};
+
+template <int I> using EncL = Conv<kEnc[I].ci, kEnc[I].co, kEnc[I].ks, (I == 2 || I == 5 || I == 8) ? 2 : 1,
+                                   (I >= 8) ? 8 : 16, kEnc[I].ns>;
+template <int K> using DecL = Conv<64, kDec[K].co, 3, 1, K == 0 ? 8 : 16, kDec[K].ns>;
+
+constexpr size_t layer_floats(const LayerDesc& d) { return (size_t)d.ks * d.ks * d.ci * d.co + d.co; }
+constexpr size_t layer_tc_bytes(const LayerDesc& d) { return (size_t)d.ks * d.ks * (d.ci < 16 ? 1 : d.ci / 16) * 64 * d.co; }
+static size_t enc_off(int i) { size_t o = 0; for (int j = 0; j < i; ++j) o += layer_floats(kEnc[j]); return o; }
+static size_t enc_tc_off(int i) { size_t o = 0; for (int j = 1; j < i; ++j) o += layer_tc_bytes(kEnc[j]); return o; }
+static size_t dec_inner_off(int k) {   // float offset of inner_{k+1}
+  size_t o = 64 * 64 + 64;
+  for (int j = 0; j < k; ++j) o += (size_t)kLat[j] * 64 + 64 + layer_floats(kDec[j]);
+  return o;
+}
+static size_t dec_tc_off(int k) { size_t o = 0; for (int j = 0; j < k; ++j) o += layer_tc_bytes(kDec[j]); return o; }
+static size_t enc_tc_total() { return enc_tc_off(11); }
+static size_t dec_tc_total() { return dec_tc_off(3); }
+
+template <class L, class Src, class Dst>
+static int launch_conv(const Src& src, const Dst& dst, const void* wtc, const float* bias, int N, int OH, int OW,
+                       cudaStream_t s) {
+  constexpr uint32_t smem = L::SMEM + Src::EXTRA;
+  static_assert(smem <= 227 * 1024, "fpn conv: shared memory");
+  auto kern = fpn_conv_kernel<L, Src, Dst>;
+  static DeviceOnce once;
+  static int per_sm = 1;
+  const int dev = current_device();
+  if (once.need(dev)) {
+    MVSF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MVSF_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem));
+    if (per_sm < 1) per_sm = 1;
+    once.done(dev);
+  }
+  const int tiles_x = cdiv(OW, 32), tiles_y = cdiv(OH, L::TR);
+  const long long ntiles = (long long)tiles_x * tiles_y * N;
+  MVSF_REQUIRE(ntiles < (1ll << 30), "fpn: image too large");
+  long long cap = (long long)per_sm * device_sm_count(dev) / L::NB;
+  if (cap < 1) cap = 1;
+  dim3 grid((unsigned)(ntiles < cap ? ntiles : cap), L::NB);
+  kern<<<grid, 256, smem, s>>>(src, dst, reinterpret_cast<const __half*>(wtc), bias, OH, OW, tiles_x, tiles_y, (int)ntiles);
+  MVSF_LAUNCH_CHECK("fpn_conv");
+  return MVSF_OK;
+}
+
+// encoder layer I (>= 2) reading an NHWC map of the previous layer's size
+template <int I>
+static int enc_layer(const float* in, float* out, const float* wts, const unsigned char* wtc, int N, int IH, int IW,
+                     cudaStream_t s) {
+  using L = EncL<I>;
+  const int OH = IH / L::S, OW = IW / L::S;
+  return launch_conv<L>(NhwcSrc<L>{in, IH, IW}, NhwcLeaky<L::CO>{out}, wtc + enc_tc_off(I),
+                        wts + enc_off(I) + (size_t)L::KS * L::KS * L::CI * L::CO, N, OH, OW, s);
+}
+
+template <int K>
+static int dec_level(const float* prev, const float* lat, const float* wts, const unsigned char* wtc, float* intra_out,
+                     float* out, int N, int h, int w, cudaStream_t s) {
+  using L = DecL<K>;
+  const size_t inner = dec_inner_off(K), conv = inner + (size_t)kLat[K] * 64 + 64;
+  return launch_conv<L>(IntraSrc<L, kLat[K]>{prev, lat, wts + inner, intra_out, h, w}, NchwSwish<L::CO>{out},
+                        wtc + dec_tc_off(K), wts + conv + (size_t)9 * 64 * L::CO, N, 2 * h, 2 * w, s);
+}
+
+static bool shape_ok(int N, int H, int W) {
+  return N > 0 && N <= 65535 && H >= 8 && W >= 8 && H % 8 == 0 && W % 8 == 0 && (long long)H * W < (1ll << 28);
+}
+
+}  // namespace fpn
+}  // namespace mvsf
+
+using namespace mvsf;
+using namespace mvsf::fpn;
+
+extern "C" int mvsf_fpn_tc_bytes(int part, size_t* bytes) {
+  MVSF_REQUIRE(bytes && (part == 0 || part == 1), "fpn_tc_bytes: part must be 0 (encoder) or 1 (decoder)");
+  *bytes = part == 0 ? enc_tc_total() : dec_tc_total();
+  return MVSF_OK;
+}
+
+extern "C" int mvsf_fpn_pack_tc(int part, const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream) {
+  MVSF_REQUIRE(wts && wts_tc && (part == 0 || part == 1), "fpn_pack_tc: bad arguments");
+  MVSF_REQUIRE(wts_tc_bytes >= (part == 0 ? enc_tc_total() : dec_tc_total()), "fpn_pack_tc: wts_tc too small");
+  unsigned char* out = static_cast<unsigned char*>(wts_tc);
+  const int n = part == 0 ? 10 : 3;
+  for (int j = 0; j < n; ++j) {
+    const LayerDesc& d = part == 0 ? kEnc[j + 1] : kDec[j];
+    const float* w = wts + (part == 0 ? enc_off(j + 1) : dec_inner_off(j) + (size_t)kLat[j] * 64 + 64);
+    unsigned char* o = out + (part == 0 ? enc_tc_off(j + 1) : dec_tc_off(j));
+    fpn_pack_kernel<<<cdiv(layer_tc_bytes(d) / 2, 256), 256, 0, (cudaStream_t)stream>>>(
+        w, reinterpret_cast<__half*>(o), d.ci, d.co, d.ks * d.ks, d.ns);
+    MVSF_LAUNCH_CHECK("fpn_pack_tc");
+  }
+  return MVSF_OK;
+}
+
+extern "C" int mvsf_fpn_encoder_workspace_bytes(int N, int H, int W, size_t* bytes) {
+  MVSF_REQUIRE(bytes, "fpn_encoder_workspace_bytes: null pointer");
+  MVSF_REQUIRE(shape_ok(N, H, W), "fpn encoder: H and W must be positive multiples of 8 (got N=%d H=%d W=%d)", N, H, W);
+  *bytes = 2 * (size_t)N * H * W * 16;   // two ping-pong maps of the largest intermediate, [N][H/2][W/2][16] fp32
+  return MVSF_OK;
+}
+
+extern "C" int mvsf_fpn_encoder_forward(const float* x, const float* wts, const void* wts_tc, float* c01, float* c11,
+                                        float* c21, float* c31, void* workspace, size_t workspace_bytes, int N, int H,
+                                        int W, mvsf_stream_t stream) {
+  size_t need = 0;
+  if (mvsf_fpn_encoder_workspace_bytes(N, H, W, &need) != MVSF_OK) return MVSF_ERR_INVALID;
+  MVSF_REQUIRE(x && wts && wts_tc && c01 && c11 && c21 && c31 && workspace, "fpn_encoder_forward: null pointer");
+  if (workspace_bytes < need) return fail(MVSF_ERR_WORKSPACE, "fpn_encoder_forward: workspace %zu < %zu bytes", workspace_bytes, need);
+  cudaStream_t s = (cudaStream_t)stream;
+  const unsigned char* wtc = static_cast<const unsigned char*>(wts_tc);
+  float* t0 = static_cast<float*>(workspace);
+  float* t1 = t0 + (size_t)N * H * W * 4;
+  using L1 = EncL<1>;
+  int rc = launch_conv<L1>(Conv00Src<L1>{x, wts + enc_off(0), H, W}, NhwcLeaky<8>{c01}, wtc + enc_tc_off(1),
+                           wts + enc_off(1) + 25 * 8 * 8, N, H, W, s);
+  if (rc) return rc;
+  if ((rc = enc_layer<2>(c01, t0, wts, wtc, N, H, W, s))) return rc;
+  if ((rc = enc_layer<3>(t0, t1, wts, wtc, N, H / 2, W / 2, s))) return rc;
+  if ((rc = enc_layer<4>(t1, c11, wts, wtc, N, H / 2, W / 2, s))) return rc;
+  if ((rc = enc_layer<5>(c11, t0, wts, wtc, N, H / 2, W / 2, s))) return rc;
+  if ((rc = enc_layer<6>(t0, t1, wts, wtc, N, H / 4, W / 4, s))) return rc;
+  if ((rc = enc_layer<7>(t1, c21, wts, wtc, N, H / 4, W / 4, s))) return rc;
+  if ((rc = enc_layer<8>(c21, t0, wts, wtc, N, H / 4, W / 4, s))) return rc;
+  if ((rc = enc_layer<9>(t0, t1, wts, wtc, N, H / 8, W / 8, s))) return rc;
+  return enc_layer<10>(t1, c31, wts, wtc, N, H / 8, W / 8, s);
+}
+
+extern "C" int mvsf_fpn_decoder_workspace_bytes(int N, int H, int W, size_t* bytes) {
+  MVSF_REQUIRE(bytes, "fpn_decoder_workspace_bytes: null pointer");
+  MVSF_REQUIRE(shape_ok(N, H, W), "fpn decoder: H and W must be positive multiples of 8 (got N=%d H=%d W=%d)", N, H, W);
+  *bytes = (size_t)N * ((size_t)(H / 4) * (W / 4) + (size_t)(H / 2) * (W / 2)) * 64 * 4;   // intra_1, intra_2
+  return MVSF_OK;
+}
+
+extern "C" int mvsf_fpn_decoder_forward(const float* c01, const float* c11, const float* c21, const float* c31,
+                                        const float* wts, const void* wts_tc, float* o0, float* o1, float* o2, float* o3,
+                                        void* workspace, size_t workspace_bytes, int N, int H, int W,
+                                        mvsf_stream_t stream) {
+  size_t need = 0;
+  if (mvsf_fpn_decoder_workspace_bytes(N, H, W, &need) != MVSF_OK) return MVSF_ERR_INVALID;
+  MVSF_REQUIRE(c01 && c11 && c21 && c31 && wts && wts_tc && o0 && o1 && o2 && o3 && workspace,
+               "fpn_decoder_forward: null pointer");
+  if (workspace_bytes < need) return fail(MVSF_ERR_WORKSPACE, "fpn_decoder_forward: workspace %zu < %zu bytes", workspace_bytes, need);
+  cudaStream_t s = (cudaStream_t)stream;
+  const unsigned char* wtc = static_cast<const unsigned char*>(wts_tc);
+  float* intra1 = static_cast<float*>(workspace);
+  float* intra2 = intra1 + (size_t)N * (H / 4) * (W / 4) * 64;
+  const int npix = N * (H / 8) * (W / 8);
+  fpn_out0_kernel<<<cdiv(npix, 128), 128, 0, s>>>(c31, wts, o0, (H / 8) * (W / 8), npix);
+  MVSF_LAUNCH_CHECK("fpn_out0");
+  int rc;
+  if ((rc = dec_level<0>(c31, c21, wts, wtc, intra1, o1, N, H / 8, W / 8, s))) return rc;
+  if ((rc = dec_level<1>(intra1, c11, wts, wtc, intra2, o2, N, H / 4, W / 4, s))) return rc;
+  return dec_level<2>(intra2, c01, wts, wtc, nullptr, o3, N, H / 2, W / 2, s);
+}

@@ -88,6 +88,13 @@ __device__ __forceinline__ void fence_regs(float* d) {
 }
 
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands in shared memory (K-major); acc = 0 overwrites D
+__device__ __forceinline__ void mma_ss_n8(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0,%1,%2,%3}, %4, %5, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(a), "l"(b), "r"(acc));
+}
 __device__ __forceinline__ void mma_ss_n16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
@@ -162,8 +169,9 @@ __device__ __forceinline__ void mma_rs_n40(float* d, const uint32_t (&a)[4], uin
 
 template <int N>
 __device__ __forceinline__ void mma_ss(float* d, uint64_t a, uint64_t b, uint32_t acc) {
-  static_assert(N == 16 || N == 32 || N == 48 || N == 64 || N == 96 || N == 128 || N == 192 || N == 256, "wgmma N");
-  if constexpr (N == 16) mma_ss_n16(d, a, b, acc);
+  static_assert(N == 8 || N == 16 || N == 32 || N == 48 || N == 64 || N == 96 || N == 128 || N == 192 || N == 256, "wgmma N");
+  if constexpr (N == 8) mma_ss_n8(d, a, b, acc);
+  else if constexpr (N == 16) mma_ss_n16(d, a, b, acc);
   else if constexpr (N == 32) mma_ss_n32(d, a, b, acc);
   else if constexpr (N == 48) mma_ss_n48(d, a, b, acc);
   else if constexpr (N == 64) mma_ss_n64(d, a, b, acc);

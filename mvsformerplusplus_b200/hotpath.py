@@ -4,7 +4,9 @@ enqueue libmvsf_b200 kernels.  PyTorch is used for device memory, streams and mo
   StageNet.forward(features, proj_matrices, depth_values, tmp, position3d=None)   <- models/cost_volume.py:51-133
   FMT_with_pathway.forward(features)                                              <- models/FMT.py:164-206
   HotPathNet.forward_features(features, proj_matrices, depth_values, tmp)         <- DINOv2_mvsformer_model.py:117-179
+  FPNEncoder.forward(x) / FPNDecoder.forward(conv01, conv11, conv21, conv31)     <- models/module.py:208-270
   install(model)  rebinds the two module seams of a reference-constructed DINOv2MVSNet        (test.py drop-in)
+  install(model, feature_pyramid=True)  also rebinds model.encoder / model.decoder
 
 Tensors crossing the seams keep the reference's logical shapes ([B,V,C,H,W] features, [B,D,H,W] volumes).  Feature
 maps produced by FMT_with_pathway are channels-last in memory (a permuted view), which StageNet consumes
@@ -18,7 +20,7 @@ import torch.nn as nn
 
 from . import _lib, packing
 from .config import load_args, stage_list, validate_args
-from .params import build_fmt, build_stage
+from .params import build_fmt, build_fpn_decoder, build_fpn_encoder, build_stage
 
 
 def _ptr(t):
@@ -444,10 +446,123 @@ def cascade_forward(fmt_module, fusions, args, features, proj_matrices, depth_va
 
 
 # =====================================================================================================
-def install(model, args=None):
+def _check_fpn_config(feat_chs, norm_type="BN"):
+    if list(feat_chs) != [8, 16, 32, 64]:
+        raise NotImplementedError(f"FPN: only feat_chs [8, 16, 32, 64] is implemented, got {list(feat_chs)}")
+    if norm_type != "BN":
+        raise NotImplementedError(f"FPN: only norm_type 'BN' is implemented, got {norm_type!r}")
+
+
+def _check_fpn_size(H, W):
+    if H % 8 or W % 8 or H < 8 or W < 8:
+        raise ValueError(f"FPN: image height and width must be positive multiples of 8 (the decoder adds exact 2x "
+                         f"upsamplings), got {H}x{W}")
+
+
+def _fpn_pack_tc(part, flat):
+    L = _lib.lib()
+    need = ctypes.c_size_t(0)
+    _lib.check(L.mvsf_fpn_tc_bytes(part, ctypes.byref(need)), "fpn_tc_bytes")
+    out = torch.empty(need.value // 2, device=flat.device, dtype=torch.float16)
+    _lib.check(L.mvsf_fpn_pack_tc(part, _ptr(flat), _ptr(out), ctypes.c_size_t(need.value), _stream()), "fpn_pack_tc")
+    return out
+
+
+class FPNEncoder(_PackedMixin, nn.Module):
+    """Drop-in for the reference FPNEncoder (models/module.py:208-239), eval mode: returns [conv01, conv11, conv21, conv31]
+    as fp32 [N,C,h,w] views of channels-last buffers.  Any float dtype and strides are accepted."""
+
+    def __init__(self, feat_chs, norm_type="BN"):
+        super().__init__()
+        _check_fpn_config(feat_chs, norm_type)
+        build_fpn_encoder(self)
+        self._init_packing()
+
+    def _pack(self, device):
+        if self._packed is None or self._packed["device"] != device:
+            w = packing.pack_fpn_encoder(self.state_dict(), "").to(device)
+            self._packed = {"device": device, "w": w, "tc": _fpn_pack_tc(0, w)}
+        return self._packed
+
+    @torch.no_grad()
+    def forward(self, x):
+        if self.training:
+            raise NotImplementedError("the FPN hot path implements the eval-mode forward; call .eval()")
+        N, C, H, W = x.shape
+        if C != 3:
+            raise AssertionError(f"FPNEncoder expects [N,3,H,W] images, got {tuple(x.shape)}")
+        _check_fpn_size(H, W)
+        _require_cuda(x, "FPNEncoder.forward(x)")
+        L = _lib.lib()
+        pk = self._pack(x.device)
+        x = _f32c(x)
+        f32 = dict(device=x.device, dtype=torch.float32)
+        outs = [torch.empty((N, H // s, W // s, c), **f32) for c, s in ((8, 1), (16, 2), (32, 4), (64, 8))]
+        need = ctypes.c_size_t(0)
+        _lib.check(L.mvsf_fpn_encoder_workspace_bytes(N, H, W, ctypes.byref(need)), "fpn_encoder_workspace_bytes")
+        ws = torch.empty(need.value // 4 + 4, **f32)
+        _lib.check(L.mvsf_fpn_encoder_forward(_ptr(x), _ptr(pk["w"]), _ptr(pk["tc"]), *[_ptr(o) for o in outs], _ptr(ws),
+                                              ctypes.c_size_t(ws.numel() * 4), N, H, W, _stream()), "fpn_encoder_forward")
+        return [o.permute(0, 3, 1, 2) for o in outs]
+
+
+class FPNDecoder(_PackedMixin, nn.Module):
+    """Drop-in for the reference FPNDecoder (models/module.py:242-270), eval mode: returns [out0, out1, out2, out3] as
+    NCHW-contiguous fp32.  Inputs may be any float dtype and strides (bf16 appears under autocast after conv31 + vit_feat)."""
+
+    def __init__(self, feat_chs):
+        super().__init__()
+        _check_fpn_config(feat_chs)
+        build_fpn_decoder(self)
+        self._init_packing()
+
+    def _pack(self, device):
+        if self._packed is None or self._packed["device"] != device:
+            w = packing.pack_fpn_decoder(self.state_dict(), "").to(device)
+            self._packed = {"device": device, "w": w, "tc": _fpn_pack_tc(1, w)}
+        return self._packed
+
+    @torch.no_grad()
+    def forward(self, conv01, conv11, conv21, conv31):
+        if self.training:
+            raise NotImplementedError("the FPN hot path implements the eval-mode forward; call .eval()")
+        N, _, H, W = conv01.shape
+        _check_fpn_size(H, W)
+        ins = (conv01, conv11, conv21, conv31)
+        for t, c, s in zip(ins, (8, 16, 32, 64), (1, 2, 4, 8)):
+            if tuple(t.shape) != (N, c, H // s, W // s):
+                raise AssertionError(f"FPNDecoder: expected a [{N},{c},{H // s},{W // s}] map, got {tuple(t.shape)}")
+            _require_cuda(t, "FPNDecoder.forward")
+        L = _lib.lib()
+        pk = self._pack(conv01.device)
+        ins = [to_nhwc(t) for t in ins]
+        f32 = dict(device=conv01.device, dtype=torch.float32)
+        outs = [torch.empty((N, c, H // s, W // s), **f32) for c, s in ((64, 8), (32, 4), (16, 2), (8, 1))]
+        need = ctypes.c_size_t(0)
+        _lib.check(L.mvsf_fpn_decoder_workspace_bytes(N, H, W, ctypes.byref(need)), "fpn_decoder_workspace_bytes")
+        ws = torch.empty(need.value // 4 + 4, **f32)
+        _lib.check(L.mvsf_fpn_decoder_forward(*[_ptr(t) for t in ins], _ptr(pk["w"]), _ptr(pk["tc"]),
+                                              *[_ptr(o) for o in outs], _ptr(ws), ctypes.c_size_t(ws.numel() * 4),
+                                              N, H, W, _stream()), "fpn_decoder_forward")
+        return outs
+
+
+# =====================================================================================================
+def install(model, args=None, feature_pyramid=False):
     """Rebinds the hot-path seams of a reference-constructed DINOv2MVSNet (models/networks/DINOv2_mvsformer_model.py)
     to the CUDA path: model.FMT_module and model.fusions[i] are replaced by this package's modules carrying the
-    same weights (state_dict round trip, strict).  The rest of the model (ViT, FPN) is untouched.  Returns model."""
+    same weights (state_dict round trip, strict).  With feature_pyramid=True model.encoder and model.decoder (the FPN,
+    DINOv2_mvsformer_model.py:34-35,87-89) are replaced as well.  The ViT and its decoder stay untouched.  Returns model."""
+    if feature_pyramid:
+        feat_chs = (model.args if args is None else load_args(args)).get("feat_chs", [8, 16, 32, 64])
+        if any(isinstance(m, nn.InstanceNorm2d) for m in model.encoder.modules()):
+            raise NotImplementedError("FPN: only norm_type 'BN' is implemented")
+        dev = next(model.encoder.parameters()).device
+        enc, dec = FPNEncoder(feat_chs), FPNDecoder(feat_chs)
+        enc.load_state_dict(model.encoder.state_dict(), strict=True)
+        dec.load_state_dict(model.decoder.state_dict(), strict=True)
+        model.encoder = enc.to(dev).eval()
+        model.decoder = dec.to(dev).eval()
     args = validate_args(load_args(args if args is not None else model.args))
     dev = next(model.parameters()).device
     fmt = FMT_with_pathway(**args["FMT_config"])

@@ -87,6 +87,38 @@ def pack_costreg_tr(sd, p, layers):
     return _cat(parts, pad_to=8)  # multiple of 8 floats: the fp16 hi/lo copies stay 16-byte aligned
 
 
+def fold_conv_bn(sd, conv, bn, bias=None):
+    """Conv2d weight [co, ci, k, k] (+ optional conv bias) followed by eval BatchNorm -> (w [k*k][ci][co], shift [co]) in
+    fp64: BN(conv(x) + b) = conv_{w * scale}(x) + (b - mean) * scale + beta."""
+    w = _d(sd[conv])
+    scale, shift = _fold_bn(sd, bn)
+    if bias is not None:
+        shift = shift + _d(sd[bias]) * scale
+    w = w * scale.view(-1, 1, 1, 1)
+    return w.permute(2, 3, 1, 0).reshape(w.shape[2] * w.shape[3], w.shape[1], w.shape[0]), shift
+
+
+def pack_fpn_encoder(sd, p="encoder."):
+    """models/module.py:208-239 -> per layer (conv00 ... conv31) w [k*k][ci][co] with BN folded, then shift [co]
+    (layout documented in include/mvsf_b200.h, mvsf_fpn_encoder_forward)"""
+    from .params import FPN_ENCODER_LAYERS
+    parts = []
+    for name, *_ in FPN_ENCODER_LAYERS:
+        parts += list(fold_conv_bn(sd, f"{p}{name}.conv.weight", f"{p}{name}.bn."))
+    return _cat(parts)
+
+
+def pack_fpn_decoder(sd, p="decoder."):
+    """models/module.py:242-270 -> out0 [64][64] + shift; per level k = 1..3: inner_k [cl][64] + bias[64], out_k
+    [9][64][c_k] + shift (conv bias and BN folded; layout documented in include/mvsf_b200.h, mvsf_fpn_decoder_forward)"""
+    parts = list(fold_conv_bn(sd, p + "out0.0.weight", p + "out0.1.", p + "out0.0.bias"))
+    for k in (1, 2, 3):
+        wi = _d(sd[f"{p}inner{k}.weight"])  # [64, cl, 1, 1]
+        parts += [wi.reshape(wi.shape[0], wi.shape[1]).t(), _d(sd[f"{p}inner{k}.bias"])]
+        parts += list(fold_conv_bn(sd, f"{p}out{k}.0.weight", f"{p}out{k}.1.", f"{p}out{k}.0.bias"))
+    return _cat(parts)
+
+
 def pack_fmt(sd, p="FMT_module."):
     """layout documented in csrc/fmt.cu"""
     parts = []

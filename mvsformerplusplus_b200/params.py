@@ -156,6 +156,34 @@ def build_stage(args, ndepth, stage_idx):
     return m
 
 
+FPN_CHS = (8, 16, 32, 64)
+# FPNEncoder layers (models/module.py:211-224): name, cin, cout, kernel, stride
+FPN_ENCODER_LAYERS = (("conv00", 3, 8, 7, 1), ("conv01", 8, 8, 5, 1), ("downsample1", 8, 16, 5, 2),
+                      ("conv10", 16, 16, 3, 1), ("conv11", 16, 16, 3, 1), ("downsample2", 16, 32, 5, 2),
+                      ("conv20", 32, 32, 3, 1), ("conv21", 32, 32, 3, 1), ("downsample3", 32, 64, 3, 2),
+                      ("conv30", 64, 64, 3, 1), ("conv31", 64, 64, 3, 1))
+
+
+def build_fpn_encoder(m):
+    """models/module.py:208-224 (norm_type 'BN'): encoder.<layer>.conv.weight, encoder.<layer>.bn.*"""
+    for name, cin, cout, k, _ in FPN_ENCODER_LAYERS:
+        b = Bag()
+        b.conv = nn.Conv2d(cin, cout, k, padding=(k - 1) // 2, bias=False)
+        b.bn = nn.BatchNorm2d(cout)
+        setattr(m, name, b)
+    return m
+
+
+def build_fpn_decoder(m):
+    """models/module.py:242-255: decoder.out{k}.0 conv (+bias), .1 BatchNorm, inner{k} 1x1 conv with bias"""
+    c = FPN_CHS
+    m.out0 = nn.Sequential(nn.Conv2d(c[3], c[3], 1), nn.BatchNorm2d(c[3]))
+    for k, (cl, co) in enumerate(((c[2], c[2]), (c[1], c[1]), (c[0], c[0])), start=1):
+        setattr(m, f"inner{k}", nn.Conv2d(cl, c[3], 1))
+        setattr(m, f"out{k}", nn.Sequential(nn.Conv2d(c[3], co, 3, padding=1), nn.BatchNorm2d(co)))
+    return m
+
+
 def build_hotpath_params(args):
     root = Bag()
     root.FMT_module = build_fmt(args["FMT_config"])

@@ -69,6 +69,20 @@ def make_features(V, H, W, feat_chs=(64, 32, 16, 8), seed=1234, batch=1, smooth=
     return feats
 
 
+def make_images(V, H, W, seed=2024):
+    """[V,3,H,W] image-like inputs of the FPN encoder: a smooth random field (binomial low-pass applied twice) plus a
+    little texture, per channel zero-mean and unit-variance."""
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(V, 3, H, W, generator=g)
+    k = torch.tensor([1.0, 4.0, 6.0, 4.0, 1.0]) / 16.0
+    for _ in range(2):
+        x = F.conv2d(F.pad(x, (2, 2, 0, 0), mode="replicate"), k.view(1, 1, 1, 5).repeat(3, 1, 1, 1), groups=3)
+        x = F.conv2d(F.pad(x, (0, 0, 2, 2), mode="replicate"), k.view(1, 1, 5, 1).repeat(3, 1, 1, 1), groups=3)
+    x = x / x.std() + 0.2 * torch.randn(V, 3, H, W, generator=g)
+    x = x - x.mean(dim=(2, 3), keepdim=True)
+    return (x / x.std(dim=(2, 3), keepdim=True)).contiguous()
+
+
 def randomize_state_dict(module, seed=7, prob_gain=1.0):
     """Seeded re-initialisation of a parameter container (params.build_hotpath_params or the
     reference modules themselves - same key names): seeded normal weights (1/sqrt(fan_in)), randomised BatchNorm
@@ -87,7 +101,7 @@ def randomize_state_dict(module, seed=7, prob_gain=1.0):
             new[k] = 0.2 * r
         elif k.endswith("running_var"):
             new[k] = 0.5 + torch.rand(v.shape, generator=g)
-        elif ".bn." in k or re.search(r"cost_reg\.conv(7|9|11)\.1\.", k):
+        elif ".bn." in k or re.search(r"cost_reg\.conv(7|9|11)\.1\.", k) or re.search(r"(^|\.)decoder\.out[0-3]\.1\.", k):
             new[k] = (1.0 + 0.2 * r) if k.endswith("weight") else 0.1 * r
         elif "norm" in k or ".down.1." in k or ".up.1." in k:
             new[k] = (1.0 + 0.1 * r) if k.endswith("weight") else 0.05 * r
