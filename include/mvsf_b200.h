@@ -169,6 +169,18 @@ int mvsf_attention_forward(const float* qkv, float* out, void* workspace, size_t
  * workspace >= (M+N)*2K*2 + 256 bytes.  gelu != 0 applies the exact-erf GELU. */
 int mvsf_linear_tc_forward(const float* A, const float* W, const float* bias, float* C, void* workspace,
                            size_t workspace_bytes, int M, int N, int K, int gelu, mvsf_stream_t stream);
+/* test seam: the same layer with any of its fused epilogues, as FMT and the transformer regulariser call it.
+ * epi: 0 C = acc + bias, 1 C = gelu(acc + bias), 2 C = col < elu_cols ? elu(acc + bias) + 1 : acc + bias,
+ * 3 C = res + gamma * (acc + bias), 4 C = LN(res + gamma * (acc + bias)), 5 C = LN(acc + bias); LN = LayerNorm over
+ * the row with ln_w, ln_b, ln_eps (epilogues 4 and 5 need N == 64).  A [M][lda] and W [N][K] are fp32 and split into
+ * fp16 hi/lo parts inside the call.  bias [N] may be NULL; res [M][ldres] and gamma [N] are read by epilogues 3 and 4.
+ * Outputs, each optional (C or C2 required): C [M][ldc] fp32; Cpre [M][ldcpre] = the value before the LayerNorm
+ * (epilogues 4 and 5 only, may alias res); C2 [M][ldc2] fp16 = [hi(N) | lo(N)] split of C per row.
+ * Operands and outputs 16-byte aligned.  workspace >= (M+N)*2K*2 + 256 bytes. */
+int mvsf_linear_tc_epilogue(int epi, const float* A, int lda, const float* W, const float* bias, const float* res,
+                            int ldres, const float* gamma, const float* ln_w, const float* ln_b, float ln_eps,
+                            int elu_cols, float* C, int ldc, float* Cpre, int ldcpre, void* C2, int ldc2,
+                            void* workspace, size_t workspace_bytes, int M, int N, int K, mvsf_stream_t stream);
 
 /* ---- S1: models/cost_volume.py:105-117 + models/module.py:649-655 (eval, depth_type 'ce').
  * logits [D][H][W], depth hypotheses [D][H][W] -> prob [D][H][W], depth [H][W], conf [H][W] */

@@ -43,6 +43,7 @@ SIGNATURES = {
     "mvsf_attention_set_precision": ([I], I),
     "mvsf_attention_forward": ([P, P, P, Z, I, F, P], I),
     "mvsf_linear_tc_forward": ([P, P, P, P, P, Z, I, I, I, I, P], I),
+    "mvsf_linear_tc_epilogue": ([I, P, I, P, P, P, I, P, P, P, F, I, P, I, P, I, P, I, P, Z, I, I, I, P], I),
     "mvsf_softargmax": ([P, P, F, P, P, P, I, I, I, P], I),
     "mvsf_conf_accumulate": ([P, I, I, P, I, I, F, I, P], I),
     "mvsf_fmt_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),

@@ -267,7 +267,9 @@ static int launch_tc_n(const TcLinArgs& a, int epi, size_t smem, int grid, cudaS
   return fail(MVSF_ERR_INVALID, "linear_tc: unknown epilogue %d", epi);
 }
 
-int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s) {
+// host-side argument checks of launch_linear_tc; touch no device state, so callers can run them before any launch
+static int check_linear_tc(const TcLinArgs& a, int epi) {
+  MVSF_REQUIRE(epi >= LIN_BIAS && epi <= LIN_LN, "linear_tc: unknown epilogue %d", epi);
   MVSF_REQUIRE(a.Ah && a.Al && a.Bh && a.Bl && (a.C || a.C2) && a.M > 0, "linear_tc: bad arguments");
   MVSF_REQUIRE((a.N == 16 || a.N == 64 || a.N == 128 || a.N == 192 || a.N == 256) && a.K % TC_BK == 0 && a.K >= TC_BK,
                "linear_tc: need N in {16, 64, 128, 192, 256}, K %% 64 == 0");
@@ -284,6 +286,13 @@ int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s) {
                            "linear_tc: Cpre needs a LayerNorm epilogue and 16-byte alignment");
   const size_t smem = tc_smem_bytes(a.N, a.K);
   MVSF_REQUIRE(smem <= 227 * 1024, "linear_tc: N*K too large for resident weights (%zu bytes of shared memory)", smem);
+  return MVSF_OK;
+}
+
+int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s) {
+  int rc;
+  if ((rc = check_linear_tc(a, epi))) return rc;
+  const size_t smem = tc_smem_bytes(a.N, a.K);
   const int num_sms = device_sm_count(current_device());
   const int ntiles = cdiv(a.M, TC_BM);
   const int grid = ntiles < num_sms ? ntiles : num_sms;  // persistent: one CTA per SM, tiles strided by gridDim.x
@@ -338,6 +347,32 @@ extern "C" int mvsf_linear_tc_forward(const float* A, const float* W, const floa
   a.Ah = A2; a.Al = A2 + K; a.lda = 2 * K; a.Bh = B2; a.Bl = B2 + K; a.ldb = 2 * K;
   a.M = M; a.N = N; a.K = K; a.bias = bias; a.C = C; a.ldc = N;
   return launch_linear_tc(a, gelu ? LIN_GELU : LIN_BIAS, s);
+}
+
+extern "C" int mvsf_linear_tc_epilogue(int epi, const float* A, int lda, const float* W, const float* bias,
+                                       const float* res, int ldres, const float* gamma, const float* ln_w,
+                                       const float* ln_b, float ln_eps, int elu_cols, float* C, int ldc, float* Cpre,
+                                       int ldcpre, void* C2, int ldc2, void* workspace, size_t workspace_bytes, int M,
+                                       int N, int K, mvsf_stream_t stream) {
+  MVSF_REQUIRE(A && W && workspace && M > 0 && K > 0, "linear_tc_epilogue: null pointer or empty shape");
+  MVSF_REQUIRE(lda >= K && (lda % 4) == 0 && ((uintptr_t)A & 15) == 0 && ((uintptr_t)W & 15) == 0 &&
+                   ((uintptr_t)workspace & 15) == 0,
+               "linear_tc_epilogue: need lda >= K, lda %% 4 == 0, and A, W and workspace must be 16-byte aligned");
+  const size_t need = ((size_t)M * 2 * K + (size_t)N * 2 * K) * sizeof(__half) + 256;
+  if (workspace_bytes < need) return fail(MVSF_ERR_WORKSPACE, "linear_tc_epilogue: workspace %zu < %zu bytes", workspace_bytes, need);
+  __half* A2 = reinterpret_cast<__half*>(workspace);
+  __half* B2 = A2 + align_up((size_t)M * 2 * K, 64);
+  TcLinArgs a{};
+  a.Ah = A2; a.Al = A2 + K; a.lda = 2 * K; a.Bh = B2; a.Bl = B2 + K; a.ldb = 2 * K;
+  a.M = M; a.N = N; a.K = K; a.bias = bias; a.res = res; a.ldres = ldres; a.gamma = gamma;
+  a.ln_w = ln_w; a.ln_b = ln_b; a.ln_eps = ln_eps; a.elu_cols = elu_cols;
+  a.C = C; a.ldc = ldc; a.Cpre = Cpre; a.ldcpre = ldcpre; a.C2 = reinterpret_cast<__half*>(C2); a.ldc2 = ldc2;
+  int rc;
+  if ((rc = check_linear_tc(a, epi))) return rc;   // every rejection happens before the first launch
+  cudaStream_t s = (cudaStream_t)stream;
+  if ((rc = launch_split_f16(A, lda, A2, 2 * K, M, K, s))) return rc;
+  if ((rc = launch_split_f16(W, K, B2, 2 * K, N, K, s))) return rc;
+  return launch_linear_tc(a, epi, s);
 }
 
 /* fp32 weight blob -> fp16 hi / lo blobs with identical indexing (install time): out16 = [hi(n) | lo(n)] */
