@@ -181,6 +181,14 @@ int mvsf_linear_tc_epilogue(int epi, const float* A, int lda, const float* W, co
                             int ldres, const float* gamma, const float* ln_w, const float* ln_b, float ln_eps,
                             int elu_cols, float* C, int ldc, float* Cpre, int ldcpre, void* C2, int ldc2,
                             void* workspace, size_t workspace_bytes, int M, int N, int K, mvsf_stream_t stream);
+/* test seam: the streamed-weight GEMM the ViT decoder runs on (models/module.py:273-364: its q/k/v, proj, fc1, fc2
+ * linears and conv head), for token rows.  Weights stream through the pipeline with A, so N and K are limited only by
+ * N % 64 == 0 and K % 64 == 0.  epi: 0 bias, 1 gelu, 2 elu+1 on columns < elu_cols, 3 C = res + gamma * (acc + bias),
+ * 6 C = silu(acc + bias); no LayerNorm epilogues.  Arguments and outputs as mvsf_linear_tc_epilogue (no Cpre). */
+int mvsf_linear_tc_streamed_epilogue(int epi, const float* A, int lda, const float* W, const float* bias,
+                                     const float* res, int ldres, const float* gamma, int elu_cols, float* C, int ldc,
+                                     void* C2, int ldc2, void* workspace, size_t workspace_bytes, int M, int N, int K,
+                                     mvsf_stream_t stream);
 
 /* ---- S1: models/cost_volume.py:105-117 + models/module.py:649-655 (eval, depth_type 'ce').
  * logits [D][H][W], depth hypotheses [D][H][W] -> prob [D][H][W], depth [H][W], conf [H][W] */
@@ -220,6 +228,19 @@ int mvsf_fpn_decoder_forward(const float* c01, const float* c11, const float* c2
 /* install time: fp32 blob -> fp16 hi/lo weight tiles of the wgmma convolutions (csrc/fpn.cu); part 0 encoder, 1 decoder */
 int mvsf_fpn_tc_bytes(int part, size_t* bytes);
 int mvsf_fpn_pack_tc(int part, const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
+
+/* ---- V1: models/module.py:273-364 CrossVITDecoder.forward, shipped config (d_model 768, 12 heads, linear attention,
+ *      ffn 768 -> 3072, LayerScale, pre-norm CrossBlocks with pre_norm_query, 3 interval layers, eval-mode BN folded).
+ * x0, x1, x2 [B][V][h*w][768] (the ViT tokens of dinov2.py:249-266 without the cls token, view 0 = reference)
+ * -> out [B*V][4h][4w][64] (NHWC).  wts: packing.pack_vit_decoder (layout in csrc/vit_decoder.cu: the GEMM weights as
+ * [N][K] rows, then norms, biases, LayerScales, prev_values and folded conv biases; 37 863 880 floats).
+ * wts_tc = mvsf_vit_decoder_pack_tc(wts).  Bad shapes (B < 1, V < 2, h or w outside [1, 2048)): -1, nothing launched. */
+int mvsf_vit_decoder_workspace_bytes(int B, int V, int h, int w, size_t* bytes);
+int mvsf_vit_decoder_tc_bytes(size_t* bytes);
+int mvsf_vit_decoder_pack_tc(const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
+int mvsf_vit_decoder_forward(const float* x0, const float* x1, const float* x2, const float* wts, const void* wts_tc,
+                             float* out, void* workspace, size_t workspace_bytes, int B, int V, int h, int w,
+                             mvsf_stream_t stream);
 
 #ifdef __cplusplus
 }

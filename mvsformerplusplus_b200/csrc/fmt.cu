@@ -5,6 +5,7 @@
 // Tokens "(h w) c" of the reference are exactly channels-last pixels, so the stage-1 output is produced directly in
 // the [V][H][W][64] layout the warp kernels consume.  All source views are processed as one batch; the K/V
 // summaries of the two cross layers depend only on the reference view and are computed once.
+#include "linattn.cuh"
 #include "linear.cuh"
 #include "linear_tc.cuh"
 #include "wgmma.cuh"
@@ -19,7 +20,8 @@ constexpr int B_N1W = 0, B_N1B = 64, B_QKV = 128, B_PW = B_QKV + 192 * 64, B_PB 
 // after 4 blocks: dr1[32][64] dr2[16][32] dr3[8][16] sm1[9][32][32] sm2[9][16][16] sm3[9][8][8]   ([tap][ci][co])
 constexpr int P_DR1 = 4 * B_SIZE, P_DR2 = P_DR1 + 32 * 64, P_DR3 = P_DR2 + 16 * 32, P_SM1 = P_DR3 + 8 * 16,
               P_SM2 = P_SM1 + 9 * 32 * 32, P_SM3 = P_SM2 + 9 * 16 * 16, FMT_WTS = P_SM3 + 9 * 8 * 8;
-constexpr int KVSZ = 4 * 16 * 16 + 64;  // KV[h][m][d] + ksum[h][d]
+using FmtAttn = LinAttn<4, 16>;
+constexpr int KVSZ = FmtAttn::KVSZ;  // KV[h][m][d] + ksum[h][d]
 
 // f [V][64][L] (NCHW) + pe [L][64] -> tok [V][L][64]
 __global__ void tokens_add_pe_kernel(const float* __restrict__ f, const float* __restrict__ pe, float* __restrict__ tok,
@@ -37,124 +39,6 @@ __global__ void tokens_add_pe_kernel(const float* __restrict__ f, const float* _
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     int p = p0 + i, c = c0 + threadIdx.x;
     if (p < L) d[(size_t)p * 64 + c] = tile[threadIdx.x][i] + __ldg(pe + (size_t)p * 64 + c);
-  }
-}
-
-// partial[view][blk][KVSZ]: KV[h][m][d] = sum_s k[s,h,d] v[s,h,m] ; ksum[h][d] = sum_s k[s,h,d]  over a 256-token chunk
-constexpr int KV_CHUNK = 256, KV_TILE = 64;
-__global__ void __launch_bounds__(256)
-kv_partial_kernel(const float* __restrict__ kv, int ld, int koff, int voff, int L, float* __restrict__ partial) {
-  __shared__ __align__(16) float ks[KV_TILE][64];
-  __shared__ __align__(16) float vs[KV_TILE][64];
-  const int view = blockIdx.y, blk = blockIdx.x, tid = threadIdx.x;
-  const float* base = kv + (size_t)view * L * ld;
-  const int h = tid >> 6, m = (tid >> 2) & 15, d0 = (tid & 3) * 4;
-  float acc[4] = {0.f, 0.f, 0.f, 0.f}, ksum[4] = {0.f, 0.f, 0.f, 0.f};
-  const int s_begin = blk * KV_CHUNK, s_end = min(L, s_begin + KV_CHUNK);
-  for (int s0 = s_begin; s0 < s_end; s0 += KV_TILE) {
-    __syncthreads();
-    for (int i = tid; i < KV_TILE * 16; i += 256) {
-      int r = i >> 4, c = (i & 15) * 4;
-      float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
-      if (s0 + r < s_end) {
-        a = ldg4(base + (size_t)(s0 + r) * ld + koff + c);
-        b = ldg4(base + (size_t)(s0 + r) * ld + voff + c);
-      }
-      *reinterpret_cast<float4*>(&ks[r][c]) = a;
-      *reinterpret_cast<float4*>(&vs[r][c]) = b;
-    }
-    __syncthreads();
-#pragma unroll 8
-    for (int r = 0; r < KV_TILE; ++r) {
-      float4 k4 = *reinterpret_cast<const float4*>(&ks[r][h * 16 + d0]);
-      float vv = vs[r][h * 16 + m];
-      acc[0] = fmaf(k4.x, vv, acc[0]); acc[1] = fmaf(k4.y, vv, acc[1]);
-      acc[2] = fmaf(k4.z, vv, acc[2]); acc[3] = fmaf(k4.w, vv, acc[3]);
-      ksum[0] += k4.x; ksum[1] += k4.y; ksum[2] += k4.z; ksum[3] += k4.w;
-    }
-  }
-  float* o = partial + ((size_t)view * gridDim.x + blk) * KVSZ;
-  *reinterpret_cast<float4*>(o + (h * 16 + m) * 16 + d0) = make_float4(acc[0], acc[1], acc[2], acc[3]);
-  if (m == 0) *reinterpret_cast<float4*>(o + 1024 + h * 16 + d0) = make_float4(ksum[0], ksum[1], ksum[2], ksum[3]);
-}
-__global__ void kv_final_kernel(const float* __restrict__ partial, int nblk, float* __restrict__ fin) {
-  const int view = blockIdx.y;
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= KVSZ) return;
-  float s = 0.f;
-  for (int b = 0; b < nblk; ++b) s += partial[((size_t)view * nblk + b) * KVSZ + i];
-  fin[(size_t)view * KVSZ + i] = s;
-}
-
-// Row LayerNorm over 64 channels emitting the fp16 hi|lo split [hi(64) | lo(64)] the tensor-core GEMMs consume
-__global__ void __launch_bounds__(256)
-layernorm64_split_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
-                         __half* __restrict__ y2, int M, float eps) {
-  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (row >= M) return;
-  float2 v = ldg2(x + (size_t)row * 64 + lane * 2);
-  float s = v.x + v.y;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float mean = s * (1.0f / 64.0f);
-  float d0 = v.x - mean, d1 = v.y - mean;
-  float q = d0 * d0 + d1 * d1;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-  const float sd = sqrtf(q * (1.0f / 64.0f) + eps);
-  float2 ww = ldg2(w + lane * 2), bb = ldg2(b + lane * 2);
-  const float o0 = __fdiv_rn(d0, sd) * ww.x + bb.x, o1 = __fdiv_rn(d1, sd) * ww.y + bb.y;
-  const __half2 hh = __floats2half2_rn(o0, o1);
-  const float2 hf = __half22float2(hh);
-  *reinterpret_cast<__half2*>(y2 + (size_t)row * 128 + lane * 2) = hh;
-  *reinterpret_cast<__half2*>(y2 + (size_t)row * 128 + 64 + lane * 2) = __floats2half2_rn(o0 - hf.x, o1 - hf.y);
-}
-
-// out[s][h*16+m] = (sum_d q[s,h,d] KV[h][m][d]) / (q[s,h,:] . ksum[h,:] + 1e-6)     (attention.py:281-284)
-__global__ void __launch_bounds__(128)
-linattn_apply_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ kvfin, size_t kv_view_stride,
-                     __half* __restrict__ out2, int L, int M) {
-  __shared__ __align__(16) float kvs[256 + 16];
-  const int h = blockIdx.y;
-  const int s = blockIdx.x * 128 + threadIdx.x;
-  const int view = (blockIdx.x * 128) / L;  // host guarantees L % 128 == 0 or a single view per launch
-  const float* kvp = kvfin + (size_t)view * kv_view_stride;
-  for (int i = threadIdx.x; i < 256; i += 128) kvs[i] = __ldg(kvp + h * 256 + i);
-  if (threadIdx.x < 16) kvs[256 + threadIdx.x] = __ldg(kvp + 1024 + h * 16 + threadIdx.x);
-  __syncthreads();
-  if (s >= M) return;
-  float qv[16];
-  const float* qp = q + (size_t)s * ldq + h * 16;
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    float4 t = ldg4(qp + c * 4);
-    qv[c * 4] = t.x; qv[c * 4 + 1] = t.y; qv[c * 4 + 2] = t.z; qv[c * 4 + 3] = t.w;
-  }
-  float den = 0.f;
-#pragma unroll
-  for (int d = 0; d < 16; ++d) den = fmaf(qv[d], kvs[256 + d], den);
-  const float z = __fdiv_rn(1.0f, den + 1e-6f);
-  __half* op = out2 + (size_t)s * 128 + h * 16;  // fp16 hi|lo split rows [hi(64) | lo(64)]
-#pragma unroll
-  for (int mq = 0; mq < 4; ++mq) {
-    float r[4];
-#pragma unroll
-    for (int mm = 0; mm < 4; ++mm) {
-      const float4* kp = reinterpret_cast<const float4*>(&kvs[(mq * 4 + mm) * 16]);
-      float4 a = kp[0], b = kp[1], c = kp[2], e = kp[3];
-      float t = qv[0] * a.x;
-      t = fmaf(qv[1], a.y, t); t = fmaf(qv[2], a.z, t); t = fmaf(qv[3], a.w, t);
-      t = fmaf(qv[4], b.x, t); t = fmaf(qv[5], b.y, t); t = fmaf(qv[6], b.z, t); t = fmaf(qv[7], b.w, t);
-      t = fmaf(qv[8], c.x, t); t = fmaf(qv[9], c.y, t); t = fmaf(qv[10], c.z, t); t = fmaf(qv[11], c.w, t);
-      t = fmaf(qv[12], e.x, t); t = fmaf(qv[13], e.y, t); t = fmaf(qv[14], e.z, t); t = fmaf(qv[15], e.w, t);
-      r[mm] = t * z;
-    }
-    const __half2 h01 = __floats2half2_rn(r[0], r[1]), h23 = __floats2half2_rn(r[2], r[3]);
-    const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
-    *reinterpret_cast<__half2*>(op + mq * 4) = h01;
-    *reinterpret_cast<__half2*>(op + mq * 4 + 2) = h23;
-    *reinterpret_cast<__half2*>(op + 64 + mq * 4) = __floats2half2_rn(r[0] - f01.x, r[1] - f01.y);
-    *reinterpret_cast<__half2*>(op + 64 + mq * 4 + 2) = __floats2half2_rn(r[2] - f23.x, r[3] - f23.y);
   }
 }
 
@@ -176,7 +60,7 @@ static int run_block(float* x, int nviews, int L, const float* bw, size_t boff, 
   const int M = nviews * L;
   int rc;
   if (!ln1_ready) {
-    layernorm64_split_kernel<<<cdiv(M, 8), 256, 0, s>>>(x, bw + B_N1W, bw + B_N1B, ws.xn2, M, 1e-5f);
+    layernorm_split_kernel<64><<<cdiv(M, 8), 256, 0, s>>>(x, bw + B_N1W, bw + B_N1B, ws.xn2, M, 1e-5f);
     MVSF_LAUNCH_CHECK("fmt_ln1");
   }
   const float* kvsum;
@@ -188,11 +72,7 @@ static int run_block(float* x, int nviews, int L, const float* bw, size_t boff, 
   if (!kvc) {
     a.N = 192; a.ldc = 192; a.elu_cols = 128;
     if ((rc = launch_linear_tc(a, LIN_ELU1, s))) return rc;
-    const int nblk = cdiv(L, KV_CHUNK);
-    kv_partial_kernel<<<dim3(nblk, nviews), 256, 0, s>>>(ws.qkv, 192, 64, 128, L, ws.kvpart);
-    MVSF_LAUNCH_CHECK("fmt_kv_partial");
-    kv_final_kernel<<<dim3(cdiv(KVSZ, 256), nviews), 256, 0, s>>>(ws.kvpart, nblk, ws.kvfin);
-    MVSF_LAUNCH_CHECK("fmt_kv_final");
+    if ((rc = launch_kv_summary<4, 16>(ws.qkv, 192, 64, 128, L, nviews, ws.kvpart, ws.kvfin, s))) return rc;
     kvsum = ws.kvfin; kv_stride = KVSZ; ldq = 192;
   } else {
     a.N = 64; a.ldc = 64; a.elu_cols = 64;
@@ -200,11 +80,11 @@ static int run_block(float* x, int nviews, int L, const float* bw, size_t boff, 
     kvsum = kvc; kv_stride = 0; ldq = 64;
   }
   if (L % 128 == 0 || nviews == 1) {
-    linattn_apply_kernel<<<dim3(cdiv(M, 128), 4), 128, 0, s>>>(ws.qkv, ldq, kvsum, kv_stride, ws.att2, L, M);
+    linattn_apply_kernel<4, 16><<<dim3(cdiv(M, 128), 4), 128, 0, s>>>(ws.qkv, ldq, kvsum, kv_stride, ws.att2, L, M);
     MVSF_LAUNCH_CHECK("fmt_linattn_apply");
   } else {
     for (int v = 0; v < nviews; ++v) {  // views do not align with 128-token blocks: one launch per view
-      linattn_apply_kernel<<<dim3(cdiv(L, 128), 4), 128, 0, s>>>(ws.qkv + (size_t)v * L * ldq, ldq,
+      linattn_apply_kernel<4, 16><<<dim3(cdiv(L, 128), 4), 128, 0, s>>>(ws.qkv + (size_t)v * L * ldq, ldq,
                                                                  kvsum + (size_t)v * kv_stride, 0,
                                                                  ws.att2 + (size_t)v * L * 128, L, L);
       MVSF_LAUNCH_CHECK("fmt_linattn_apply");
@@ -236,19 +116,14 @@ static int run_block(float* x, int nviews, int L, const float* bw, size_t boff, 
 static int run_cross_kv(const float* ref_tok, int L, const float* bw, size_t boff, float* kvc_out, const FmtWs& ws,
                         cudaStream_t s) {
   int rc;
-  layernorm64_split_kernel<<<cdiv(L, 8), 256, 0, s>>>(ref_tok, bw + B_N1W, bw + B_N1B, ws.xn2, L, 1e-5f);
+  layernorm_split_kernel<64><<<cdiv(L, 8), 256, 0, s>>>(ref_tok, bw + B_N1W, bw + B_N1B, ws.xn2, L, 1e-5f);
   MVSF_LAUNCH_CHECK("fmt_ln_key");
   TcLinArgs a{};
   a.Ah = ws.xn2; a.Al = ws.xn2 + 64; a.lda = 128;
   a.Bh = ws.wh + boff + B_QKV + 64 * 64; a.Bl = ws.wl + boff + B_QKV + 64 * 64; a.ldb = 64;
   a.M = L; a.N = 128; a.K = 64; a.C = ws.qkv; a.ldc = 128; a.elu_cols = 64;
   if ((rc = launch_linear_tc(a, LIN_ELU1, s))) return rc;
-  const int nblk = cdiv(L, KV_CHUNK);
-  kv_partial_kernel<<<dim3(nblk, 1), 256, 0, s>>>(ws.qkv, 128, 0, 64, L, ws.kvpart);
-  MVSF_LAUNCH_CHECK("fmt_kv_partial");
-  kv_final_kernel<<<dim3(cdiv(KVSZ, 256), 1), 256, 0, s>>>(ws.kvpart, nblk, kvc_out);
-  MVSF_LAUNCH_CHECK("fmt_kv_final");
-  return MVSF_OK;
+  return launch_kv_summary<4, 16>(ws.qkv, 128, 0, 64, L, 1, ws.kvpart, kvc_out, s);
 }
 
 // 1x1 dim_reduction_k of the pathway (FMT.py:186-189, a bias-free conv = per-pixel CIN -> COUT linear map), channels-last.

@@ -47,6 +47,29 @@ __global__ void split_f16_kernel(const float* __restrict__ x, int ldx, __half* _
 constexpr int TC_NPROD = 128, TC_THREADS = 384;
 constexpr int TC_RING = 4;   // A-tile stages; two fills stay in flight behind the block whose MMAs are being issued
 
+// element-wise epilogue of the two adjacent columns (col, col + 1) of one row, shared by the resident and streamed GEMMs
+template <int EPI>
+__device__ __forceinline__ void epi_pair(const TcLinArgs& a, int col, const float* resrow, bool mvalid, float (&t)[2]) {
+  const float2 b2 = a.bias ? *reinterpret_cast<const float2*>(a.bias + col) : make_float2(0.f, 0.f);
+  t[0] += b2.x; t[1] += b2.y;
+  if (EPI == LIN_RES) {
+    const float2 g2 = *reinterpret_cast<const float2*>(a.gamma + col);
+    const float2 r2 = mvalid ? *reinterpret_cast<const float2*>(resrow + col) : make_float2(0.f, 0.f);
+    t[0] = r2.x + g2.x * t[0]; t[1] = r2.y + g2.y * t[1];
+  }
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    if (EPI == LIN_GELU) t[e] = gelu_erf_lean(t[e]);
+    if (EPI == LIN_ELU1) t[e] = (col + e < a.elu_cols) ? ((t[e] > 0.f ? t[e] : expm1f(t[e])) + 1.0f) : t[e];
+    if (EPI == LIN_SILU) t[e] = __fdiv_rn(t[e], 1.0f + expf(-t[e]));
+  }
+}
+// fp32 and / or fp16 hi|lo stores of the pair; the lo part of the split row sits lo_off halves after the hi part
+__device__ __forceinline__ void epi_store2(float* crow, __half* c2row, int lo_off, int col, const float (&t)[2]) {
+  if (crow) *reinterpret_cast<float2*>(crow + col) = make_float2(t[0], t[1]);
+  if (c2row) split_store2(c2row + col, c2row + lo_off + col, t[0], t[1]);
+}
+
 template <int N, int EPI>
 __device__ __forceinline__ void tc_epilogue(const TcLinArgs& a, const float (&acc)[N / 2], int row0, int lane) {
   const int q = lane & 3;
@@ -101,22 +124,9 @@ __device__ __forceinline__ void tc_epilogue(const TcLinArgs& a, const float (&ac
 #pragma unroll
       for (int b = 0; b < N / 8; ++b) {
         const int col = 8 * b + 2 * q;
-        const float2 b2 = a.bias ? *reinterpret_cast<const float2*>(a.bias + col) : make_float2(0.f, 0.f);
-        float t[2] = {acc[4 * b + 2 * h] + b2.x, acc[4 * b + 2 * h + 1] + b2.y};
-        if (EPI == LIN_RES) {
-          const float2 g2 = *reinterpret_cast<const float2*>(a.gamma + col);
-          const float2 r2 = mvalid ? *reinterpret_cast<const float2*>(resrow + col) : make_float2(0.f, 0.f);
-          t[0] = r2.x + g2.x * t[0]; t[1] = r2.y + g2.y * t[1];
-        }
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          if (EPI == LIN_GELU) t[e] = gelu_erf_lean(t[e]);
-          if (EPI == LIN_ELU1) t[e] = (col + e < a.elu_cols) ? ((t[e] > 0.f ? t[e] : expm1f(t[e])) + 1.0f) : t[e];
-        }
-        if (mvalid) {
-          if (crow) *reinterpret_cast<float2*>(crow + col) = make_float2(t[0], t[1]);
-          if (c2row) split_store2(c2row + col, c2row + N + col, t[0], t[1]);
-        }
+        float t[2] = {acc[4 * b + 2 * h], acc[4 * b + 2 * h + 1]};
+        epi_pair<EPI>(a, col, resrow, mvalid, t);
+        if (mvalid) epi_store2(crow, c2row, N, col, t);
       }
     }
   }
@@ -305,6 +315,244 @@ int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Streamed-weight GEMM (launch_linear_tcs, TcsArgs in linear_tc.cuh).  Same split-operand arithmetic and warpgroup
+// roles as linear_tc_kernel, but the weights stream too: a ring stage holds the 128-row A block and the BN-row W block of
+// one K-block (hi and lo tiles of each), and persistent CTAs walk (M tile, N tile) pairs, N tiles fastest, so CTAs that
+// run at the same time share A rows in L2.
+//   * BN = 128: a stage is 64.5 KB, three stages fit in shared memory (BN = 256 would allow two, and one stage in flight
+//     behind the one being multiplied does not hide the L2 latency of a 96 KB block).  Prefetch depth: stage g + 1 is
+//     filled while the MMA warpgroups multiply stage g and stage g - 1 retires.  BN = 64 serves N = 64 (conv head).
+//   * Two independent accumulator chains per warpgroup (even and odd K-blocks), added with round-to-nearest in the
+//     epilogue: the tensor core's fp32 accumulation truncates, and fc2 (K = 3072) and the 3x3 head conv (K = 6912) would
+//     otherwise chain 576 / 1296 products into one accumulator.  2 x 64 accumulator registers at BN = 128.
+//   * The producer (56 registers after setmaxnreg; the grid positions of a tile's rows sit in shared memory) resolves
+//     every A row through the implicit-GEMM grid with zero fill, so one kernel runs the token linears, the 3x3
+//     convolution and the four parity classes of a transposed convolution.
+constexpr int TCS_RING = 3;
+
+__device__ __forceinline__ size_t tcs_store_row(const TcsArgs& a, int m) {
+  const int hw = a.H * a.W, img = m / hw, rem = m - img * hw, y = rem / a.W, x = rem - y * a.W;
+  return ((size_t)img * (a.sy * a.H) + a.sy * y + a.py) * (size_t)(a.sx * a.W) + a.sx * x + a.px;
+}
+
+template <int BN>
+__device__ __forceinline__ void tcs_mma_block(float* acc, uint32_t sa, uint32_t sb) {
+  constexpr uint32_t a_bytes = tile_bytes(TC_BM), b_bytes = tile_bytes(BN), lbo_a = tile_lbo(TC_BM), lbo_b = tile_lbo(BN);
+#pragma unroll
+  for (int i = 0; i < TC_BK / 16; ++i) {
+    const uint64_t ah = make_desc(sa + 2 * i * lbo_a, lbo_a, 128);
+    const uint64_t al = make_desc(sa + a_bytes + 2 * i * lbo_a, lbo_a, 128);
+    const uint64_t bh = make_desc(sb + 2 * i * lbo_b, lbo_b, 128);
+    const uint64_t bl = make_desc(sb + b_bytes + 2 * i * lbo_b, lbo_b, 128);
+    mma_ss<BN>(acc, al, bh, 1u);
+    mma_ss<BN>(acc, ah, bl, 1u);
+    mma_ss<BN>(acc, ah, bh, 1u);
+  }
+}
+
+template <int BN, int EPI>
+__device__ __forceinline__ void tcs_epilogue(const TcsArgs& a, const float (&acc)[BN / 2], int row0, int n0, int lane) {
+  const int q = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = row0 + 8 * h;
+    const bool mvalid = m < a.M;
+    const size_t p = tcs_store_row(a, mvalid ? m : 0);
+    const float* resrow = EPI == LIN_RES ? a.res + p * a.ldres : nullptr;
+    float* crow = a.C ? a.C + p * a.ldc : nullptr;
+    __half* c2row = a.C2 ? a.C2 + p * a.ldc2 : nullptr;
+#pragma unroll
+    for (int b = 0; b < BN / 8; ++b) {
+      const int col = n0 + 8 * b + 2 * q;
+      float t[2] = {acc[4 * b + 2 * h], acc[4 * b + 2 * h + 1]};
+      epi_pair<EPI>(a, col, resrow, mvalid, t);
+      if (mvalid) epi_store2(crow, c2row, a.N, col, t);
+    }
+  }
+}
+
+template <int BN, int EPI>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+linear_tcs_kernel(TcsArgs a) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const int nkb = a.K / TC_BK, kpt = a.cin / TC_BK;
+  constexpr uint32_t a_bytes = tile_bytes(TC_BM), b_bytes = tile_bytes(BN), st_bytes = 2 * a_bytes + 2 * b_bytes;
+  const uint32_t sbase = smem_u32(smem);
+  const uint32_t bar_full = sbase + TCS_RING * st_bytes, bar_empty = bar_full + 8 * TCS_RING;
+  if (tid == 0) {
+    for (int i = 0; i < TCS_RING; ++i) { mbar_init(bar_full + 8 * i, TC_NPROD); mbar_init(bar_empty + 8 * i, 2); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  const int ntn = a.N / BN, ntiles = ((a.M + TC_BM - 1) / TC_BM) * ntn;
+  const int my_tiles = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+
+  if (wg == 0) {
+    // ------------------------------------------------------------------ producers
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+    constexpr uint32_t lbo_a = tile_lbo(TC_BM), lbo_b = tile_lbo(BN);
+    const int c = tid & 7, r0 = tid >> 3;   // this thread copies 16-byte chunk c of rows r0 + 16 j
+    const int hw = a.H * a.W;
+    int* syx = reinterpret_cast<int*>(smem + TCS_RING * st_bytes + 16 * TCS_RING);   // [2][128] row grid positions
+    auto publish = [&](int gb) {
+      fence_proxy_async();
+      mbar_arrive(bar_full + 8 * (gb % TCS_RING));
+    };
+    int g = 0;
+    for (int t_it = 0; t_it < my_tiles; ++t_it) {
+      const int t = (int)blockIdx.x + t_it * (int)gridDim.x;
+      const int m0 = (t / ntn) * TC_BM, n0 = (t % ntn) * BN;
+      int* yx = syx + 128 * (t_it & 1);   // (y << 16 | x) of the tile's rows; rows past M get a y no tap reaches
+      {
+        const int m = m0 + tid, rem = m % hw, y = rem / a.W;
+        yx[tid] = m < a.M ? (y << 16) | (rem - y * a.W) : (0x4000 << 16);
+      }
+      named_bar_sync(1, TC_NPROD);
+      for (int kb = 0; kb < nkb; ++kb, ++g) {
+        const int st = g % TCS_RING;
+        mbar_wait(bar_empty + 8 * st, (uint32_t)(((g / TCS_RING) & 1) ^ 1));
+        const uint32_t s0 = sbase + st * st_bytes;
+        const int tap = kb / kpt;
+        const int nib = (int)((a.taps >> (4 * tap)) & 15ull), dy = (nib & 3) - 1, dx = (nib >> 2) - 1;
+        const long long toff = (long long)(dy * a.W + dx) * a.lda + (kb - tap * kpt) * TC_BK + c * 8;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int r = r0 + 16 * j, p = yx[r], y = (p >> 16) + dy, x = (p & 0xffff) + dx;
+          const bool ok = (unsigned)y < (unsigned)a.H && (unsigned)x < (unsigned)a.W;
+          const size_t off = ok ? (size_t)((long long)(m0 + r) * a.lda + toff) : 0;
+          const uint32_t dst = s0 + c * lbo_a + (r >> 3) * 128 + (r & 7) * 16;
+          cp_async16_zfill(dst, a.Ah + off, ok);
+          cp_async16_zfill(dst + a_bytes, a.Al + off, ok);
+        }
+        const size_t boff = (size_t)n0 * a.ldb + kb * TC_BK + c * 8;
+#pragma unroll
+        for (int j = 0; j < BN / 16; ++j) {
+          const int r = r0 + 16 * j;
+          const uint32_t dst = s0 + 2 * a_bytes + c * lbo_b + (r >> 3) * 128 + (r & 7) * 16;
+          cp_async16_zfill(dst, a.Bh + boff + (size_t)r * a.ldb, true);
+          cp_async16_zfill(dst + b_bytes, a.Bl + boff + (size_t)r * a.ldb, true);
+        }
+        cp_async_commit_group();
+        if (g >= 1) {
+          cp_async_wait_group<1>();
+          publish(g - 1);
+        }
+      }
+    }
+    if (g >= 1) {
+      cp_async_wait_group<0>();
+      publish(g - 1);
+    }
+  } else {
+    // ------------------------------------------------------------------ MMA + epilogue warpgroups
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
+    const int half = wg - 1;
+    const int t128 = tid & 127, lane = tid & 31;
+    const int row_in_tile = 64 * half + 16 * (t128 >> 5) + (lane >> 2);
+    float acc0[BN / 2], acc1[BN / 2];
+    auto release = [&](int gb) { if (t128 == 0) mbar_arrive(bar_empty + 8 * (gb % TCS_RING)); };
+    int g = 0;
+    for (int t_it = 0; t_it < my_tiles; ++t_it) {
+      const int t = (int)blockIdx.x + t_it * (int)gridDim.x;
+      const int m0 = (t / ntn) * TC_BM, n0 = (t % ntn) * BN;
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+      int pend = -1;
+      auto step = [&](float* acc) {   // multiply ring block g into acc, keep it in flight, retire the previous block
+        const int st = g % TCS_RING;
+        mbar_wait(bar_full + 8 * st, (uint32_t)((g / TCS_RING) & 1));
+        const uint32_t sa = sbase + st * st_bytes + (uint32_t)half * 1024u, sb = sbase + st * st_bytes + 2 * a_bytes;
+        wg_fence();
+        tcs_mma_block<BN>(acc, sa, sb);
+        wg_commit();
+        if (pend >= 0) {
+          wg_wait<1>();
+          release(pend);
+        }
+        pend = g++;
+      };
+      int kb = 0;
+      for (; kb + 1 < nkb; kb += 2) {   // even K-blocks into acc0, odd ones into acc1
+        step(acc0);
+        step(acc1);
+      }
+      if (kb < nkb) step(acc0);
+      wg_wait<0>();
+      fence_regs<BN / 2>(acc0);
+      fence_regs<BN / 2>(acc1);
+      release(pend);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc0[i] = __fadd_rn(acc0[i], acc1[i]);
+      tcs_epilogue<BN, EPI>(a, acc0, m0 + row_in_tile, n0, lane);
+    }
+  }
+}
+
+static size_t tcs_smem_bytes(int BN) {   // ring, mbarriers, row grid positions
+  return (size_t)TCS_RING * (2 * tile_bytes(TC_BM) + 2 * tile_bytes(BN)) + 16 * TCS_RING + 2 * 128 * sizeof(int);
+}
+
+template <int BN, int EPI>
+static int launch_tcs(const TcsArgs& a, cudaStream_t s) {
+  static DeviceOnce once;
+  const int dev = current_device();
+  const size_t smem = tcs_smem_bytes(BN);
+  if (once.need(dev)) {
+    MVSF_CUDA_OK(cudaFuncSetAttribute(linear_tcs_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    once.done(dev);
+  }
+  const int ntiles = cdiv(a.M, TC_BM) * (a.N / BN), num_sms = device_sm_count(dev);
+  linear_tcs_kernel<BN, EPI><<<ntiles < num_sms ? ntiles : num_sms, TC_THREADS, smem, s>>>(a);
+  MVSF_LAUNCH_CHECK("linear_tcs");
+  return MVSF_OK;
+}
+
+template <int BN>
+static int launch_tcs_bn(const TcsArgs& a, int epi, cudaStream_t s) {
+  switch (epi) {
+    case LIN_BIAS: return launch_tcs<BN, LIN_BIAS>(a, s);
+    case LIN_GELU: return launch_tcs<BN, LIN_GELU>(a, s);
+    case LIN_ELU1: return launch_tcs<BN, LIN_ELU1>(a, s);
+    case LIN_RES: return launch_tcs<BN, LIN_RES>(a, s);
+    case LIN_SILU: return launch_tcs<BN, LIN_SILU>(a, s);
+    default: return fail(MVSF_ERR_INVALID, "linear_tcs: unknown epilogue %d", epi);
+  }
+}
+
+void tcs_token_rows(TcsArgs& a) {
+  a.H = a.W = 1; a.cin = a.K; a.ntaps = 1; a.taps = 0x5ull; a.sy = a.sx = 1; a.py = a.px = 0;
+}
+
+// host-side argument checks of launch_linear_tcs; touch no device state
+static int check_linear_tcs(const TcsArgs& a, int epi) {
+  MVSF_REQUIRE(epi == LIN_BIAS || epi == LIN_GELU || epi == LIN_ELU1 || epi == LIN_RES || epi == LIN_SILU,
+               "linear_tcs: unknown epilogue %d (streamed epilogues: 0 bias, 1 gelu, 2 elu+1, 3 residual, 6 silu)", epi);
+  MVSF_REQUIRE(a.Ah && a.Al && a.Bh && a.Bl && (a.C || a.C2) && a.M > 0, "linear_tcs: bad arguments");
+  MVSF_REQUIRE(a.N > 0 && a.N % 64 == 0 && a.cin > 0 && a.cin % TC_BK == 0 && a.ntaps >= 1 && a.ntaps <= 9 &&
+                   a.K == a.ntaps * a.cin, "linear_tcs: need N %% 64 == 0, K = taps * cin, cin %% 64 == 0, 1 <= taps <= 9");
+  MVSF_REQUIRE(a.H > 0 && a.W > 0 && a.H < 8192 && a.W < 8192 && a.M % (a.H * a.W) == 0 && a.sy >= 1 && a.sy <= 2 &&
+                   a.sx >= 1 && a.sx <= 2 && a.py >= 0 && a.py < a.sy && a.px >= 0 && a.px < a.sx,
+               "linear_tcs: bad implicit-GEMM grid");
+  MVSF_REQUIRE((a.lda % 8) == 0 && (a.ldb % 8) == 0 && ((uintptr_t)a.Ah & 15) == 0 && ((uintptr_t)a.Al & 15) == 0 &&
+                   ((uintptr_t)a.Bh & 15) == 0 && ((uintptr_t)a.Bl & 15) == 0, "linear_tcs: operands must be 16-byte aligned");
+  if (a.C) MVSF_REQUIRE((a.ldc % 4) == 0 && ((uintptr_t)a.C & 15) == 0, "linear_tcs: C must be 16-byte aligned");
+  if (a.C2) MVSF_REQUIRE((a.ldc2 % 8) == 0 && ((uintptr_t)a.C2 & 15) == 0, "linear_tcs: C2 must be 16-byte aligned");
+  if (epi == LIN_RES)
+    MVSF_REQUIRE(a.res && a.gamma && ((uintptr_t)a.res & 15) == 0 && ((uintptr_t)a.gamma & 15) == 0 && (a.ldres % 4) == 0,
+                 "linear_tcs: residual epilogue needs 16-byte aligned res and gamma");
+  if (a.bias) MVSF_REQUIRE(((uintptr_t)a.bias & 15) == 0, "linear_tcs: bias must be 16-byte aligned");
+  MVSF_REQUIRE(!a.Cpre, "linear_tcs: no LayerNorm epilogues");
+  return MVSF_OK;
+}
+
+int launch_linear_tcs(const TcsArgs& a, int epi, cudaStream_t s) {
+  int rc;
+  if ((rc = check_linear_tcs(a, epi))) return rc;
+  return a.N % 128 == 0 ? launch_tcs_bn<128>(a, epi, s) : launch_tcs_bn<64>(a, epi, s);
+}
+
 __global__ void split_blob_f16_kernel(const float* __restrict__ x, __half* __restrict__ hi, __half* __restrict__ lo, size_t n) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -373,6 +621,32 @@ extern "C" int mvsf_linear_tc_epilogue(int epi, const float* A, int lda, const f
   if ((rc = launch_split_f16(A, lda, A2, 2 * K, M, K, s))) return rc;
   if ((rc = launch_split_f16(W, K, B2, 2 * K, N, K, s))) return rc;
   return launch_linear_tc(a, epi, s);
+}
+
+extern "C" int mvsf_linear_tc_streamed_epilogue(int epi, const float* A, int lda, const float* W, const float* bias,
+                                                const float* res, int ldres, const float* gamma, int elu_cols, float* C,
+                                                int ldc, void* C2, int ldc2, void* workspace, size_t workspace_bytes,
+                                                int M, int N, int K, mvsf_stream_t stream) {
+  MVSF_REQUIRE(A && W && workspace && M > 0 && K > 0 && N > 0, "linear_tc_streamed_epilogue: null pointer or empty shape");
+  MVSF_REQUIRE(lda >= K && (lda % 4) == 0 && ((uintptr_t)A & 15) == 0 && ((uintptr_t)W & 15) == 0 &&
+                   ((uintptr_t)workspace & 15) == 0,
+               "linear_tc_streamed_epilogue: need lda >= K, lda %% 4 == 0, and A, W and workspace must be 16-byte aligned");
+  const size_t need = ((size_t)M * 2 * K + (size_t)N * 2 * K) * sizeof(__half) + 256;
+  if (workspace_bytes < need)
+    return fail(MVSF_ERR_WORKSPACE, "linear_tc_streamed_epilogue: workspace %zu < %zu bytes", workspace_bytes, need);
+  __half* A2 = reinterpret_cast<__half*>(workspace);
+  __half* B2 = A2 + align_up((size_t)M * 2 * K, 64);
+  TcsArgs a{};
+  a.Ah = A2; a.Al = A2 + K; a.lda = 2 * K; a.Bh = B2; a.Bl = B2 + K; a.ldb = 2 * K;
+  a.M = M; a.N = N; a.K = K; a.bias = bias; a.res = res; a.ldres = ldres; a.gamma = gamma; a.elu_cols = elu_cols;
+  a.C = C; a.ldc = ldc; a.C2 = reinterpret_cast<__half*>(C2); a.ldc2 = ldc2;
+  tcs_token_rows(a);
+  int rc;
+  if ((rc = check_linear_tcs(a, epi))) return rc;   // every rejection happens before the first launch
+  cudaStream_t s = (cudaStream_t)stream;
+  if ((rc = launch_split_f16(A, lda, A2, 2 * K, M, K, s))) return rc;
+  if ((rc = launch_split_f16(W, K, B2, 2 * K, N, K, s))) return rc;
+  return launch_linear_tcs(a, epi, s);
 }
 
 /* fp32 weight blob -> fp16 hi / lo blobs with identical indexing (install time): out16 = [hi(n) | lo(n)] */

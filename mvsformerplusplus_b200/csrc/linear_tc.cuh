@@ -22,6 +22,21 @@ struct TcLinArgs {
 };
 
 int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s);
+
+// Streamed-weight GEMM (weights too large to stay resident: N, K in the thousands).  N % 64 == 0, K = taps * cin.
+// Row m of A is an implicit-GEMM row: m = (img * H + y) * W + x enumerates an H x W grid per image, and K-block kb reads
+// channels [c, c + 64) of tap t = kb / (cin / 64) at input pixel (y + dy_t, x + dx_t) of the same grid, zero outside it:
+// A element (m, t * cin + c) = Ah[(m + dy_t * W + dx_t) * lda + c].  A token linear is one tap (0, 0) on a 1 x 1 grid.
+// Row m is stored at output pixel (img, sy * y + py, sx * x + px) of an (sy H) x (sx W) map (the parity classes of a
+// stride-2 transposed convolution); C / C2 / res rows are indexed by that pixel.  Epilogues: LIN_BIAS, LIN_GELU,
+// LIN_ELU1, LIN_RES, LIN_SILU; the C2 split of row p is [hi(0..N) | lo(0..N)].
+struct TcsArgs : TcLinArgs {
+  int H, W, cin, ntaps;
+  unsigned long long taps;   // tap t: bits [4t, 4t+2) = dy + 1, [4t+2, 4t+4) = dx + 1  (dy, dx in {-1, 0, 1})
+  int sy, sx, py, px;
+};
+void tcs_token_rows(TcsArgs& a);   // one tap (0, 0) on a 1 x 1 grid: plain rows of A, stored in place
+int launch_linear_tcs(const TcsArgs& a, int epi, cudaStream_t s);
 // out row m = [hi(0..K) | lo(0..K)] (ldo >= 2K)
 int launch_split_f16(const float* x, int ldx, __half* out, int ldo, int M, int K, cudaStream_t s);
 // element-wise split of a flat fp32 blob into two fp16 blobs with the same indexing (weights, done once at install time)

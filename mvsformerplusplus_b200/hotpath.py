@@ -7,6 +7,8 @@ enqueue libmvsf_b200 kernels.  PyTorch is used for device memory, streams and mo
   FPNEncoder.forward(x) / FPNDecoder.forward(conv01, conv11, conv21, conv31)     <- models/module.py:208-270
   install(model)  rebinds the two module seams of a reference-constructed DINOv2MVSNet        (test.py drop-in)
   install(model, feature_pyramid=True)  also rebinds model.encoder / model.decoder
+  CrossVITDecoder.forward(x, Fmats=None, vit_shape=None)                          <- models/module.py:273-364
+  install(model, vit_decoder=True)  also rebinds model.decoder_vit
 
 Tensors crossing the seams keep the reference's logical shapes ([B,V,C,H,W] features, [B,D,H,W] volumes).  Feature
 maps produced by FMT_with_pathway are channels-last in memory (a permuted view), which StageNet consumes
@@ -20,7 +22,7 @@ import torch.nn as nn
 
 from . import _lib, packing
 from .config import load_args, stage_list, validate_args
-from .params import build_fmt, build_fpn_decoder, build_fpn_encoder, build_stage
+from .params import build_fmt, build_fpn_decoder, build_fpn_encoder, build_stage, build_vit_decoder
 
 
 def _ptr(t):
@@ -548,11 +550,96 @@ class FPNDecoder(_PackedMixin, nn.Module):
 
 
 # =====================================================================================================
-def install(model, args=None, feature_pyramid=False):
+# the shipped decoder_cfg (config/mvsformer++.json); the last five default to these values in the reference
+# (module.py:280-298, block.py:332-333)
+_VIT_DECODER_CFG = dict(d_model=768, nhead=12, attention_type="Linear", ffn_type="ffn", self_cross_types=None,
+                        post_norm=False, pre_norm_query=True, no_combine_norm=False)
+_VIT_DECODER_OPTIONAL = ("ffn_type", "self_cross_types", "post_norm", "pre_norm_query", "no_combine_norm")
+
+
+def _check_vit_decoder_config(args):
+    dino = args["dino_cfg"]
+    cfg = dino["decoder_cfg"]
+    for k, want in _VIT_DECODER_CFG.items():
+        got = cfg.get(k, want) if k in _VIT_DECODER_OPTIONAL else cfg[k]
+        if got != want:
+            raise NotImplementedError(f"CrossVITDecoder: only the shipped decoder_cfg is implemented ({k} = {want!r}), "
+                                      f"got {k} = {got!r}")
+    if cfg.get("init_values") is None:
+        raise NotImplementedError("CrossVITDecoder: decoder_cfg init_values must be set (LayerScale)")
+    if dino.get("cross_interval_layers") != 3:
+        raise NotImplementedError(f"CrossVITDecoder: only cross_interval_layers = 3 is implemented, got "
+                                  f"{dino.get('cross_interval_layers')!r}")
+    for k, want in (("vit_ch", 768), ("out_ch", 64)):
+        if args.get(k) != want:
+            raise NotImplementedError(f"CrossVITDecoder: only {k} = {want} is implemented, got {args.get(k)!r}")
+
+
+class CrossVITDecoder(_PackedMixin, nn.Module):
+    """Drop-in for the reference CrossVITDecoder (models/module.py:273-364), eval mode, shipped decoder_cfg: same
+    constructor argument (arch.args), parameter names and forward signature.  x = [x0, x1, x2], each [B,V,h*w,768] in any
+    float dtype and strides (bf16 under autocast, non-contiguous [:, 1:] slices); vit_shape = (B, V, h, w, 768).  Returns
+    fp32 [B*V,64,4h,4w] as a view of a channels-last buffer.  Fmats is accepted and ignored, as in the reference."""
+
+    def __init__(self, args):
+        super().__init__()
+        _check_vit_decoder_config(args)
+        cfg = args["dino_cfg"]["decoder_cfg"]
+        build_vit_decoder(self, init_values=cfg["init_values"], prev_values=cfg.get("prev_values", 0.5))
+        self._init_packing()
+
+    def _pack(self, device):
+        if self._packed is None or self._packed["device"] != device:
+            L = _lib.lib()
+            w = packing.pack_vit_decoder(self.state_dict()).to(device)
+            need = ctypes.c_size_t(0)
+            _lib.check(L.mvsf_vit_decoder_tc_bytes(ctypes.byref(need)), "vit_decoder_tc_bytes")
+            tc = torch.empty(need.value // 2, device=device, dtype=torch.float16)
+            _lib.check(L.mvsf_vit_decoder_pack_tc(_ptr(w), _ptr(tc), ctypes.c_size_t(need.value), _stream()),
+                       "vit_decoder_pack_tc")
+            self._packed = {"device": device, "w": w, "tc": tc}
+        return self._packed
+
+    @torch.no_grad()
+    def forward(self, x, Fmats=None, vit_shape=None):
+        if self.training:
+            raise NotImplementedError("the ViT decoder implements the eval-mode forward; call .eval()")
+        B, V, h, w, C = vit_shape
+        if len(x) != 3:
+            raise AssertionError(f"CrossVITDecoder expects the three interval feature maps, got {len(x)}")
+        for t in x:
+            if tuple(t.shape) != (B, V, h * w, C) or C != 768:
+                raise AssertionError(f"CrossVITDecoder: expected [{B},{V},{h * w},768] tokens, got {tuple(t.shape)}")
+            _require_cuda(t, "CrossVITDecoder.forward(x)")
+        xs = []
+        for t in x:
+            t = _f32c(t)
+            xs.append(t if t.data_ptr() % 16 == 0 else t.clone())
+        L = _lib.lib()
+        dev = xs[0].device
+        pk = self._pack(dev)
+        f32 = dict(device=dev, dtype=torch.float32)
+        out = torch.empty((B * V, 4 * h, 4 * w, 64), **f32)
+        need = ctypes.c_size_t(0)
+        _lib.check(L.mvsf_vit_decoder_workspace_bytes(B, V, h, w, ctypes.byref(need)), "vit_decoder_workspace_bytes")
+        ws = torch.empty(need.value // 4 + 4, **f32)
+        _lib.check(L.mvsf_vit_decoder_forward(*[_ptr(t) for t in xs], _ptr(pk["w"]), _ptr(pk["tc"]), _ptr(out), _ptr(ws),
+                                              ctypes.c_size_t(ws.numel() * 4), B, V, h, w, _stream()),
+                   "vit_decoder_forward")
+        return out.permute(0, 3, 1, 2)
+
+
+# =====================================================================================================
+def install(model, args=None, feature_pyramid=False, vit_decoder=False):
     """Rebinds the hot-path seams of a reference-constructed DINOv2MVSNet (models/networks/DINOv2_mvsformer_model.py)
     to the CUDA path: model.FMT_module and model.fusions[i] are replaced by this package's modules carrying the
     same weights (state_dict round trip, strict).  With feature_pyramid=True model.encoder and model.decoder (the FPN,
-    DINOv2_mvsformer_model.py:34-35,87-89) are replaced as well.  The ViT and its decoder stay untouched.  Returns model."""
+    DINOv2_mvsformer_model.py:34-35,87-89) are replaced as well, and with vit_decoder=True model.decoder_vit
+    (CrossVITDecoder, DINOv2_mvsformer_model.py:43,64).  The ViT itself stays untouched.  Returns model."""
+    if vit_decoder:
+        dec = CrossVITDecoder(getattr(model, "vit_args", model.args) if args is None else load_args(args))
+        dec.load_state_dict(model.decoder_vit.state_dict(), strict=True)
+        model.decoder_vit = dec.to(next(model.decoder_vit.parameters()).device).eval()
     if feature_pyramid:
         feat_chs = (model.args if args is None else load_args(args)).get("feat_chs", [8, 16, 32, 64])
         if any(isinstance(m, nn.InstanceNorm2d) for m in model.encoder.modules()):

@@ -138,3 +138,48 @@ def pack_fmt(sd, p="FMT_module."):
         w = _d(sd[f"{p}smooth_{k}.weight"])  # [co, ci, 3, 3] -> [tap][ci][co]
         parts.append(w.permute(2, 3, 1, 0).reshape(9, w.shape[1], w.shape[0]))
     return _cat(parts, pad_to=8)
+
+
+VIT_DECODER_BLOCKS = tuple(f"self_attn_blocks.{i}." for i in range(2)) + tuple(f"cross_attn_blocks.{i}." for i in range(3))
+VIT_DECODER_WTS = 37863880   # floats of the packed blob (csrc/vit_decoder.cu N_WTS)
+
+
+def deconv_class_taps(py):
+    """ConvTranspose2d(k4, s2, p1) in gather form along one axis: output 2 y + py reads input y + d with kernel index k,
+    for the class's two taps (d, k) (csrc/vit_decoder.cu deconv_taps)."""
+    return ((0, 1), (-1, 3)) if py == 0 else ((0, 2), (1, 0))
+
+
+def pack_vit_decoder(sd, p=""):
+    """models/module.py:273-364 -> the fp32 blob of mvsf_vit_decoder_forward (layout in csrc/vit_decoder.cu).
+    GEMM weights as [N][K] rows: per block (self0, self1, cross0, cross1, cross2) [q; k; v] [2304][768], proj, fc1, fc2;
+    the 3x3 proj conv [256][tap * 768 + ci] (tap = ky * 3 + kx) and, per parity class (py, px) of the two transposed
+    convs, [co][tap * ci_n + ci] over the class's 2 x 2 gather taps; BN scale folded into every conv.  Then per block
+    norm1 w, b, proj bias, ls1, norm2 w, b, fc1 bias, fc2 bias, ls2; norm_layers; prev_values (padded to 8); the folded
+    conv biases [256], [128], [64]."""
+    g, small = [], []
+    for b in VIT_DECODER_BLOCKS:
+        q = p + b
+        g += [torch.cat([_d(sd[q + "attn.q_proj.weight"]), _d(sd[q + "attn.k_proj.weight"]),
+                         _d(sd[q + "attn.v_proj.weight"])], 0),
+              _d(sd[q + "attn.proj.weight"]), _d(sd[q + "mlp.fc1.weight"]), _d(sd[q + "mlp.fc2.weight"])]
+        small += [_d(sd[q + k]) for k in ("norm1.weight", "norm1.bias", "attn.proj.bias", "ls1.gamma", "norm2.weight",
+                                          "norm2.bias", "mlp.fc1.bias", "mlp.fc2.bias", "ls2.gamma")]
+    scale, shift = _fold_bn(sd, p + "proj.1.")
+    w = _d(sd[p + "proj.0.weight"]) * scale.view(-1, 1, 1, 1)          # [256, 768, 3, 3]
+    g.append(w.permute(0, 2, 3, 1).reshape(w.shape[0], -1))
+    biases = [shift + _d(sd[p + "proj.0.bias"]) * scale]
+    for name in ("upsampler0", "upsampler1"):
+        scale, shift = _fold_bn(sd, f"{p}{name}.1.")
+        w = _d(sd[f"{p}{name}.0.weight"]) * scale.view(1, -1, 1, 1)    # [ci, co, 4, 4]
+        for py in (0, 1):
+            for px in (0, 1):
+                taps = [w[:, :, ky, kx] for _, ky in deconv_class_taps(py) for _, kx in deconv_class_taps(px)]
+                g.append(torch.stack(taps, 0).permute(2, 0, 1).reshape(w.shape[1], -1))   # [co][tap][ci]
+        biases.append(shift + _d(sd[f"{p}{name}.0.bias"]) * scale)
+    for i in range(2):
+        small += [_d(sd[f"{p}norm_layers.{i}.weight"]), _d(sd[f"{p}norm_layers.{i}.bias"])]
+    small += [torch.stack([_d(sd[f"{p}prev_values.{i}"]).reshape(()) for i in range(2)]), torch.zeros(6, dtype=torch.float64)]
+    out = _cat(g + small + biases, pad_to=8)
+    assert out.numel() == VIT_DECODER_WTS, out.numel()
+    return out

@@ -184,6 +184,25 @@ def build_fpn_decoder(m):
     return m
 
 
+def build_vit_decoder(m, init_values=1.0, prev_values=0.5):
+    """models/module.py:273-313 (CrossVITDecoder, shipped decoder_cfg): self_attn_blocks.{0,1}, cross_attn_blocks.{0,1,2}
+    (CrossBlock d 768, mlp 3072), norm_layers.{0,1} (LayerNorm eps 1e-6), prev_values.{0,1} (scalars), and the conv head
+    proj / upsampler0 / upsampler1 (.0 conv with bias, .1 BatchNorm, .2 SiLU)."""
+    d, ch = 768, 64
+    m.self_attn_blocks = nn.ModuleList([_cross_block(d, 4 * d) for _ in range(2)])
+    m.cross_attn_blocks = nn.ModuleList([_cross_block(d, 4 * d) for _ in range(3)])
+    for blk in list(m.self_attn_blocks) + list(m.cross_attn_blocks):
+        nn.init.constant_(blk.ls1.gamma, init_values)
+        nn.init.constant_(blk.ls2.gamma, init_values)
+    m.norm_layers = nn.ModuleList([nn.LayerNorm(d, eps=1e-6) for _ in range(2)])
+    m.prev_values = nn.ParameterList([nn.Parameter(torch.tensor(float(prev_values))) for _ in range(2)])
+    m.proj = nn.Sequential(nn.Conv2d(d, ch * 4, 3, stride=1, padding=1), nn.BatchNorm2d(ch * 4), nn.SiLU())
+    m.upsampler0 = nn.Sequential(nn.ConvTranspose2d(ch * 4, ch * 2, 4, stride=2, padding=1), nn.BatchNorm2d(ch * 2),
+                                 nn.SiLU())
+    m.upsampler1 = nn.Sequential(nn.ConvTranspose2d(ch * 2, ch, 4, stride=2, padding=1), nn.BatchNorm2d(ch), nn.SiLU())
+    return m
+
+
 def build_hotpath_params(args):
     root = Bag()
     root.FMT_module = build_fmt(args["FMT_config"])

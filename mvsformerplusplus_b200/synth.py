@@ -101,7 +101,8 @@ def randomize_state_dict(module, seed=7, prob_gain=1.0):
             new[k] = 0.2 * r
         elif k.endswith("running_var"):
             new[k] = 0.5 + torch.rand(v.shape, generator=g)
-        elif ".bn." in k or re.search(r"cost_reg\.conv(7|9|11)\.1\.", k) or re.search(r"(^|\.)decoder\.out[0-3]\.1\.", k):
+        elif ".bn." in k or re.search(r"cost_reg\.conv(7|9|11)\.1\.", k) or re.search(r"(^|\.)decoder\.out[0-3]\.1\.", k) \
+                or re.search(r"(^|\.)decoder_vit\.(proj|upsampler0|upsampler1)\.1\.", k):
             new[k] = (1.0 + 0.2 * r) if k.endswith("weight") else 0.1 * r
         elif "norm" in k or ".down.1." in k or ".up.1." in k:
             new[k] = (1.0 + 0.1 * r) if k.endswith("weight") else 0.05 * r

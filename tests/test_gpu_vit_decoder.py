@@ -1,0 +1,203 @@
+"""GPU tests of the ViT feature decoder (csrc/vit_decoder.cu through hotpath.CrossVITDecoder) and of the streamed-weight
+GEMM it runs on (csrc/linear_tc.cu, mvsf_linear_tc_streamed_epilogue) against fp64 references, the reference-executed
+fixtures, the fp32 restatement at full size, and through install() with the reference's glue.
+Bar: every output within 1e-4 * max(1, max|ref|); errors go to rec()."""
+import ctypes
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+from mvsformerplusplus_b200 import synth
+from oracle import vit_decoder as OV
+from tests.common import load_golden, max_abs, rec
+from tests.fpn_common import fpn_state_dict
+from tests.vit_decoder_common import (CASES, OracleFPNDecoder, OracleFPNEncoder, OracleViTDecoder, cuda_decoder,
+                                      make_tokens, shipped_args, vit_state_dict)
+
+pytestmark = pytest.mark.gpu
+BIAS, GELU, ELU1, RES, SILU = 0, 1, 2, 3, 6
+
+
+@pytest.fixture(scope="module")
+def dev():
+    from mvsformerplusplus_b200.build import build
+    build()
+    return torch.device("cuda:0")
+
+
+def _p(t):
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+# (epilogue, M, N, K, elu_cols, write C2): every epilogue at N 768 and 3072, K 768 / 3072 / 6912, M not a multiple of 128
+GEMM_CASES = [
+    (BIAS, 1728, 768, 768, 0, False), (BIAS, 6913, 3072, 6912, 0, True), (GELU, 2040, 3072, 768, 0, True),
+    (GELU, 1728, 768, 3072, 0, False), (ELU1, 2040, 768, 768, 768, False), (ELU1, 1728, 3072, 768, 1536, False),
+    (ELU1, 6913, 3072, 3072, 37, True), (RES, 6913, 768, 3072, 0, False), (RES, 2040, 3072, 6912, 0, True),
+    (SILU, 1728, 768, 6912, 0, True), (SILU, 2040, 3072, 3072, 0, False), (SILU, 6913, 64, 512, 0, False),
+    (BIAS, 1, 128, 1024, 0, True),
+]
+
+
+@pytest.mark.parametrize("epi,M,N,K,elu_cols,c2", GEMM_CASES)
+def test_streamed_gemm_vs_fp64(dev, epi, M, N, K, elu_cols, c2):
+    from mvsformerplusplus_b200 import _lib
+    L = _lib.lib()
+    g = torch.Generator(device=dev).manual_seed(M + N + K + epi)
+    A = torch.randn(M, K + 4, device=dev, generator=g)[:, :K]            # lda = K + 4: strided rows
+    W = torch.randn(N, K, device=dev, generator=g) / K ** 0.5
+    bias = 0.1 * torch.randn(N, device=dev, generator=g)
+    res = torch.randn(M, N, device=dev, generator=g) if epi == RES else None
+    gamma = 1.0 + 0.1 * torch.randn(N, device=dev, generator=g) if epi == RES else None
+    ldc = N + 8
+    C = torch.full((M, ldc), float("nan"), device=dev)
+    C2 = torch.full((M, 2 * N + 8), float("nan"), device=dev, dtype=torch.float16) if c2 else None
+    ws = torch.empty(((M + N) * 2 * K * 2 + 256) // 4 + 64, device=dev)
+    rc = L.mvsf_linear_tc_streamed_epilogue(epi, _p(A), K + 4, _p(W), _p(bias), _p(res), N, _p(gamma), elu_cols, _p(C),
+                                            ldc, _p(C2), 2 * N + 8, _p(ws), ctypes.c_size_t(ws.numel() * 4), M, N, K,
+                                            ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+    _lib.check(rc, "linear_tc_streamed_epilogue")
+    t = A.double() @ W.double().t() + bias.double()
+    if epi == GELU:
+        t = F.gelu(t)
+    elif epi == ELU1:
+        t = torch.cat([F.elu(t[:, :elu_cols]) + 1, t[:, elu_cols:]], 1)
+    elif epi == RES:
+        t = res.double() + gamma.double() * t
+    elif epi == SILU:
+        t = F.silu(t)
+    got = C[:, :N]
+    assert bool(torch.isfinite(got).all()) and bool(torch.isnan(C[:, N:]).all())
+    scale = max(1.0, float(t.abs().max()))
+    e = dict(C=float((got.double() - t).abs().max()) / scale)
+    if c2:
+        hi, lo = C2[:, :N], C2[:, N:2 * N]
+        assert torch.equal(hi, got.half()) and torch.equal(lo, (got - hi.float()).half())
+        assert bool(torch.isnan(C2[:, 2 * N:]).all())
+        e["C2"] = float((hi.double() + lo.double() - t).abs().max()) / scale
+    rec(f"streamed_gemm_epi{epi}_{M}x{N}x{K}", **e)
+    assert max(e.values()) < 1e-4, e
+
+
+def _run(dec, x, B, V, h, w):
+    return dec(x, vit_shape=(B, V, h, w, 768))
+
+
+@pytest.mark.parametrize("B,V,h,w,harsh", [(1, 3, 4, 6, False), (1, 2, 5, 7, False), (2, 2, 3, 5, False),
+                                           (1, 5, 12, 16, False), (2, 3, 9, 11, False), (1, 3, 8, 8, True)])
+def test_vit_decoder_vs_fp64_oracle(dev, B, V, h, w, harsh):
+    sd = vit_state_dict(31)
+    x = make_tokens(dict(B=B, V=V, h=h, w=w, xseed=B * 100 + V * 10 + h + w, harsh=harsh))
+    got = _run(cuda_decoder(sd, dev), [t.to(dev) for t in x], B, V, h, w)
+    want = OV.vit_decoder([t.to(dev).double() for t in x], sd, (B, V, h, w, 768))
+    e = float((got.double() - want).abs().max()) / max(1.0, float(want.abs().max()))
+    rec(f"vit_decoder_fp64_{B}x{V}x{h}x{w}{'_harsh' if harsh else ''}", rel=e, max_ref=float(want.abs().max()))
+    assert e < 1e-4
+
+
+@pytest.mark.parametrize("name", sorted(CASES))
+def test_vit_decoder_vs_reference_fixture(dev, name):
+    gold, meta = load_golden(name)
+    x = make_tokens(meta)
+    got = _run(cuda_decoder(vit_state_dict(meta["wseed"]), dev), [t.to(dev) for t in x], meta["B"], meta["V"],
+               meta["h"], meta["w"]).cpu()
+    want = gold["out"]
+    e = max_abs(got, want) / max(1.0, float(want.abs().max()))
+    rec(f"vit_decoder_fixture_{name}", rel=e)
+    assert e < 1e-4
+
+
+@pytest.mark.parametrize("V,h,w", [(5, 36, 48), (10, 34, 60)])
+def test_vit_decoder_full_size_vs_fp32_torch(dev, V, h, w):
+    sd = vit_state_dict(32)
+    sd_dev = {k: v.to(dev) for k, v in sd.items()}
+    g = torch.Generator(device=dev).manual_seed(V)
+    x = [torch.randn(1, V, h * w, 768, device=dev, generator=g) for _ in range(3)]
+    got = _run(cuda_decoder(sd, dev), x, 1, V, h, w)
+    tf32 = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    try:
+        with torch.no_grad():
+            want = OV.vit_decoder(x, sd_dev, (1, V, h, w, 768))
+    finally:
+        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = tf32
+    e = float((got - want).abs().max()) / max(1.0, float(want.abs().max()))
+    rec(f"vit_decoder_fullsize_{V}x{h}x{w}", rel=e, max_ref=float(want.abs().max()))
+    assert got.shape == (V, 64, 4 * h, 4 * w) and got.permute(0, 2, 3, 1).is_contiguous()
+    assert e < 1e-4
+
+
+def test_vit_decoder_bf16_and_strided_inputs(dev):
+    sd = vit_state_dict(33)
+    dec = cuda_decoder(sd, dev)
+    B, V, h, w = 1, 3, 6, 8
+    g = torch.Generator(device=dev).manual_seed(5)
+    with_cls = [torch.randn(B, V, 1 + h * w, 768, device=dev, generator=g) for _ in range(3)]
+    strided = [t[:, :, 1:] for t in with_cls]               # the reference drops the cls token with a slice
+    assert not strided[0].is_contiguous()
+    e = {}
+    for tag, x in (("strided_fp32", strided), ("bf16", [t.bfloat16() for t in strided]),
+                   ("strided_bf16", [t.bfloat16()[:, :, 1:] for t in with_cls])):
+        got = _run(dec, x, B, V, h, w)
+        want = OV.vit_decoder([t.double() for t in x], sd, (B, V, h, w, 768))
+        e[tag] = float((got.double() - want).abs().max()) / max(1.0, float(want.abs().max()))
+    rec("vit_decoder_input_dtypes_strides", **e)
+    assert max(e.values()) < 1e-4, e
+
+
+def test_install_vit_decoder_and_fpn_under_bf16_autocast(dev):
+    """install(stub, feature_pyramid=True, vit_decoder=True) on a stub with the reference's glue (decoder -> bilinear
+    resize to H/8 x W/8 -> conv31 + vit_feat -> FPN decoder, DINOv2_mvsformer_model.py:78-98) under bf16 autocast, against
+    the unswapped stub (fp32 torch modules) outside autocast."""
+    from mvsformerplusplus_b200 import hotpath
+    from mvsformerplusplus_b200.config import default_args
+    from mvsformerplusplus_b200.params import build_hotpath_params
+
+    class Stub(torch.nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.args, self.vit_args = default_args(), shipped_args()
+            hp = build_hotpath_params(self.args)
+            self.FMT_module, self.fusions = hp.FMT_module, hp.fusions
+            self.encoder, self.decoder, self.decoder_vit = OracleFPNEncoder(), OracleFPNDecoder(), OracleViTDecoder()
+
+        def forward(self, imgs, tokens, vit_hw):
+            B, V, _, H, W = imgs.shape
+            vit_feat = self.decoder_vit(tokens, vit_shape=[B, V, vit_hw[0], vit_hw[1], 768])
+            vit_feat = F.interpolate(vit_feat, size=(H // 8, W // 8), mode="bilinear", align_corners=False)
+            feats = [[], [], [], []]
+            for vi in range(V):
+                c01, c11, c21, c31 = self.encoder(imgs[:, vi])
+                c31 = c31 + vit_feat[vi].unsqueeze(0)
+                for k, f in enumerate(self.decoder.forward(c01, c11, c21, c31)):
+                    feats[k].append(f)
+            return [torch.stack(f, 1) for f in feats]
+
+    stub = Stub()
+    wrap = torch.nn.Module()
+    wrap.encoder, wrap.decoder = stub.encoder, stub.decoder
+    wrap.load_state_dict(fpn_state_dict(25), strict=True)
+    wrap = torch.nn.Module()
+    wrap.decoder_vit = stub.decoder_vit
+    wrap.load_state_dict(vit_state_dict(26), strict=True)
+    stub = stub.to(dev).eval()
+    V, H, W, vh, vw = 3, 128, 160, 7, 9        # 7 x 9 tokens -> 28 x 36 -> resized to 16 x 20
+    imgs = synth.make_images(V, H, W, seed=93).unsqueeze(0).to(dev)
+    g = torch.Generator(device=dev).manual_seed(94)
+    tokens = [torch.randn(1, V, vh * vw, 768, device=dev, generator=g).bfloat16() for _ in range(3)]   # ViT output
+    tf32 = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    try:
+        with torch.no_grad():
+            want = stub(imgs, [t.float() for t in tokens], (vh, vw))
+    finally:
+        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = tf32
+    hotpath.install(stub, feature_pyramid=True, vit_decoder=True)
+    assert isinstance(stub.decoder_vit, hotpath.CrossVITDecoder) and isinstance(stub.encoder, hotpath.FPNEncoder)
+    with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
+        got = stub(imgs, tokens, (vh, vw))
+    e = {f"stage{k + 1}": float((g_.float() - w_).abs().max()) / max(1.0, float(w_.abs().max()))
+         for k, (g_, w_) in enumerate(zip(got, want))}
+    rec("vit_decoder_install_autocast", **e)
+    assert max(e.values()) < 1e-4, e
