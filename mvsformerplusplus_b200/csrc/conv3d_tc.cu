@@ -19,8 +19,10 @@
 //   * stride-(SD,2,2) convolutions keep four parity planes (even/odd h x even/odd w, one strided tensor map each) so
 //     that every tap is again a dense plane access; transposed convolutions run in gather form over INPUT cells with
 //     four accumulators, one per output parity class (every (kh, kw) tap feeds exactly one class).  Taps that read the
-//     same input shift (dih, diw) are fused along N: the class accumulators sit in the order [0, 1, 3, 2] so that the
-//     4 / 2 / 2 / 1 classes fed by the shifts (0,0) / (0,1) / (1,0) / (1,1) are contiguous column ranges;
+//     same input shift (dih, diw) are fused along N: every shift is ONE MMA of N = 4 * NPAD over all four class
+//     accumulators (in the order [0, 1, 3, 2]), with zero weight blocks for the classes it does not feed (9 of the 16
+//     blocks are taps).  Each MMA thus writes the same register tuple with the same N, which is what lets ptxas keep
+//     the MMAs in flight; MMAs into overlapping sub-ranges of one tuple with different N are serialised (C7511);
 //   * persistent, warp-specialised CTAs (one per SM, tiles strided by gridDim.x): warpgroup 0 = TMA producer (one
 //     thread), warpgroups 1-2 = MMA + epilogue (bias (folded BatchNorm), ReLU, skip add, fp16 hi|lo split or the fused
 //     1x1x1 `prob` conv).  Ring: full[s] / empty[s]; each MMA warpgroup keeps one unit of MMAs in flight while it issues
@@ -53,7 +55,8 @@ struct Geo {
   static constexpr uint32_t PITCH = PC * 16;
 };
 __host__ __device__ inline int npad(int cout) { return cout < 16 ? 16 : cout; }
-__host__ __device__ inline uint32_t slab_bytes(int cout) { return (uint32_t)npad(cout) * 576u; }  // 9 blocks x 2 variants x (2 x NPAD x 16 B)
+// one (kd, channel group) weight slab: 9 (conv) or 16 (transposed conv) blocks x 2 variants x (2 x NPAD x 16 B)
+__host__ __device__ inline uint32_t slab_bytes(int mode, int cout) { return (uint32_t)npad(cout) * (mode == DECONV_S2 ? 1024u : 576u); }
 
 struct alignas(64) Maps { CUtensorMap m[4]; };   // CONV_S2: one map per (h, w) parity; otherwise m[0]
 
@@ -134,7 +137,7 @@ conv3d_tc_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, in
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int CIN = a.CIN, SD = a.SD, ID = a.ID, IH = a.IH, IW = a.IW;
   const int KG = a.KG;                                            // channel octets per unit
-  const uint32_t b_bytes = c3::slab_bytes(NPAD);
+  const uint32_t b_bytes = c3::slab_bytes(MODE, NPAD);
   const uint32_t a_bytes = (uint32_t)KG * G::OCT_BYTES;
   const uint32_t stage_bytes = (a_bytes + b_bytes + 127u) / 128u * 128u;
   const uint32_t sbase = smem_u32(smem);
@@ -197,41 +200,38 @@ conv3d_tc_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, in
       const int s = g % NS;
       mbar_wait(bar_full + 8 * s, (uint32_t)((g / NS) & 1));
       const uint32_t sA = sbase + s * stage_bytes + (uint32_t)half * 8u * G::PITCH, sB = sbase + s * stage_bytes + a_bytes;
-      // one fused tap group: A start offset, first weight block, NB blocks (N = NB * NPAD), first accumulator column
-      auto issue = [&](auto nb_c, uint32_t aoff, int bstart, auto dcol_c, bool overwrite) {
-        constexpr int NB = decltype(nb_c)::value, DCOL = decltype(dcol_c)::value;
-        constexpr uint32_t n = (uint32_t)(NB * NPAD);
-        const uint32_t t0 = sB + (uint32_t)bstart * 2u * blk, t1 = t0 + (uint32_t)NB * blk;
+      // one tap (conv) or input shift (transposed conv): A start offset, first weight block; N = NCLS * NPAD = all of acc[t]
+      auto issue = [&](uint32_t aoff, int bstart, bool overwrite) {
+        constexpr uint32_t n = (uint32_t)(NCLS * NPAD);
+        const uint32_t t0 = sB + (uint32_t)bstart * 2u * blk, t1 = t0 + (uint32_t)NCLS * blk;
         const uint64_t b0 = make_desc(t0, n * 16u, 128), b1 = make_desc(t1, n * 16u, 128);
         // consecutive MMAs go to different accumulators (M-tiles): back-to-back MMAs on one accumulator serialise
         if (KG == 1) {
 #pragma unroll
           for (int t = 0; t < NT; ++t)                                                       // K = [hi | lo] of one octet
-            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + aoff + t * 128, G::SUB_BYTES, G::PITCH), b0, overwrite ? 0u : 1u);  // x [w_hi ; w_hi]
+            mma_ss<n>(acc[t], make_desc(sA + aoff + t * 128, G::SUB_BYTES, G::PITCH), b0, overwrite ? 0u : 1u);  // x [w_hi ; w_hi]
 #pragma unroll
           for (int t = 0; t < NT; ++t)
-            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + aoff + t * 128, G::SUB_BYTES, G::PITCH), b1, 1u);                 // x [w_lo ; 0]
+            mma_ss<n>(acc[t], make_desc(sA + aoff + t * 128, G::SUB_BYTES, G::PITCH), b1, 1u);                 // x [w_lo ; 0]
         } else {
 #pragma unroll
           for (int t = 0; t < NT; ++t)                                                       // K = two octets; lo planes
-            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + G::SUB_BYTES + aoff + t * 128, G::OCT_BYTES, G::PITCH), b0, overwrite ? 0u : 1u);  // x_lo * w_hi
+            mma_ss<n>(acc[t], make_desc(sA + G::SUB_BYTES + aoff + t * 128, G::OCT_BYTES, G::PITCH), b0, overwrite ? 0u : 1u);  // x_lo * w_hi
 #pragma unroll
           for (int t = 0; t < NT; ++t)
-            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + aoff + t * 128, G::OCT_BYTES, G::PITCH), b1, 1u);                 // x_hi * w_lo
+            mma_ss<n>(acc[t], make_desc(sA + aoff + t * 128, G::OCT_BYTES, G::PITCH), b1, 1u);                 // x_hi * w_lo
 #pragma unroll
           for (int t = 0; t < NT; ++t)
-            mma_ss<n>(acc[t] + DCOL / 2, make_desc(sA + aoff + t * 128, G::OCT_BYTES, G::PITCH), b0, 1u);                 // x_hi * w_hi
+            mma_ss<n>(acc[t], make_desc(sA + aoff + t * 128, G::OCT_BYTES, G::PITCH), b0, 1u);                 // x_hi * w_hi
         }
       };
-      using I1 = std::integral_constant<int, 1>;
-      using I0 = std::integral_constant<int, 0>;
       wg_fence();
       if constexpr (MODE == DECONV_S2) {
-        // input shift (dih, diw) -> fused classes; weight blocks in conv3d_tc_pack's order
-        issue(std::integral_constant<int, 4>{}, 0u, 0, I0{}, u == 0);                                              // (0,0): taps (1,1) (1,2) (2,2) (2,1) -> classes 0 1 3 2
-        issue(std::integral_constant<int, 2>{}, 16u, 4, std::integral_constant<int, NPAD>{}, false);                // (0,1): taps (1,0) (2,0)             -> classes 1 3
-        issue(std::integral_constant<int, 2>{}, (uint32_t)PC * 16u, 6, std::integral_constant<int, 2 * NPAD>{}, false);        // (1,0): taps (0,2) (0,1) -> classes 3 2
-        issue(I1{}, (uint32_t)(PC + 1) * 16u, 8, std::integral_constant<int, 2 * NPAD>{}, false);                  // (1,1): tap  (0,0)                   -> class 3
+        // input shift (dih, diw) -> classes [0, 1, 3, 2]; weight blocks in conv3d_tc_pack's order, zero where a class is not fed
+        issue(0u, 0, u == 0);                               // (0,0): taps (1,1) (1,2) (2,2) (2,1)
+        issue(16u, 4, false);                               // (0,1): -      (1,0) (2,0) -
+        issue((uint32_t)PC * 16u, 8, false);                // (1,0): -      -     (0,2) (0,1)
+        issue((uint32_t)(PC + 1) * 16u, 12, false);         // (1,1): -      -     (0,0) -
       } else {
 #pragma unroll
         for (int kh = 0; kh < 3; ++kh) {
@@ -242,7 +242,7 @@ conv3d_tc_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, in
               sub = (kh == 1 ? 0 : 2) + (kw == 1 ? 0 : 1);
               rs = kh == 2 ? 1 : 0; cs = kw == 2 ? 1 : 0;
             }
-            issue(I1{}, (uint32_t)sub * G::PAIR + (uint32_t)(rs * PC + cs) * 16u, kh * 3 + kw, I0{}, u == 0 && kh == 0 && kw == 0);
+            issue((uint32_t)sub * G::PAIR + (uint32_t)(rs * PC + cs) * 16u, kh * 3 + kw, u == 0 && kh == 0 && kw == 0);
           }
         }
       }
@@ -287,10 +287,11 @@ conv3d_tc_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, in
 // CostRegNet).  The MMAs above are bound by the shared-memory read of the A operand, so instead of visiting an input
 // slice three times - once per output slice it feeds - a work item is a COLUMN: a tile x a run of output depth slices
 // [d0, d1).  Input slice `id` is loaded ONCE and one MMA per tap multiplies it with [W(kd=2) ; W(kd=1) ; W(kd=0)]
-// (N = 3 * Cout), feeding the accumulators of the output slices id-1, id, id+1 at once.  The accumulators live in a ring
-// of 4 slots per M-tile (slot = od % 4, consecutive slots are contiguous registers, a window that wraps is issued as two
-// MMAs); slice id-1 is complete once the MMAs of input slice id have retired and goes through the epilogue before the
-// next input slice is multiplied.  3x fewer A-operand reads and TMA bytes.
+// (N = 3 * Cout), feeding the accumulators of the output slices id-1, id, id+1 at once.  The accumulators are a window
+// of those three slices per M-tile, written whole by every MMA (one register tuple, one N: the MMAs stay pipelined);
+// slice id-1 is complete once the MMAs of input slice id have retired and goes through the epilogue, then the window
+// moves down one slice and its last third is zeroed before the next input slice is multiplied.  Thirds that fall
+// outside the depth run [d0, d1) are computed and thrown away.  3x fewer A-operand reads and TMA bytes.
 template <int MODE, int NT, int NPAD>
 __global__ void __launch_bounds__(c3::THREADS, 1)
 conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, int wres, int OH, int OW, int tiles_w,
@@ -362,65 +363,37 @@ conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, i
   if (wres) mbar_wait(bar_w, 0u);
   constexpr uint32_t btile = (uint32_t)NPAD * 96u;    // one (tap, variant) weight tile: 2 k-chunks x 3*NPAD rows x 16 B
   constexpr uint32_t blbo = (uint32_t)NPAD * 48u;     // k-chunk stride inside a weight tile
-  float acc[NT][4 * NPAD / 2];                        // [M-tile][slot 0..3 x NPAD columns]
+  constexpr int SL = NPAD / 2;                        // accumulator registers of one output slice
+  float acc[NT][3 * SL];                              // [M-tile][output slices id-1, id, id+1 x NPAD columns]
   auto release = [&](uint32_t gb) { if (t128 == 0) mbar_arrive(bar_empty + 8 * (gb % NS)); };
-  auto epilogue = [&](int od, int th, int tw) {       // output slice od (slot od % 4) is complete
-    const int slot = od & 3;
+  auto epilogue = [&](int od, int th, int tw, auto third_c) {   // output slice od (window third third_c) is complete
 #pragma unroll
-    for (int sl = 0; sl < 4; ++sl) {
-      if (sl != slot) continue;
+    for (int t = 0; t < NT; ++t)
 #pragma unroll
-      for (int t = 0; t < NT; ++t)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int ch = th * 16 + 8 * half + 2 * wq + h;
-          const int cw = tw * G::TW + t * 8 + (lane >> 2);
-          const bool valid = ch < OH && cw < OW;
-          const size_t vox = valid ? ((size_t)od * OH + ch) * OW + cw : 0;
-          conv_epilogue_frag<OUT_SPLIT, NPAD>(a, acc[t] + sl * (NPAD / 2), h, q, valid, vox);
-        }
-    }
+      for (int h = 0; h < 2; ++h) {
+        const int ch = th * 16 + 8 * half + 2 * wq + h;
+        const int cw = tw * G::TW + t * 8 + (lane >> 2);
+        const bool valid = ch < OH && cw < OW;
+        const size_t vox = valid ? ((size_t)od * OH + ch) * OW + cw : 0;
+        conv_epilogue_frag<OUT_SPLIT, NPAD>(a, acc[t] + decltype(third_c)::value * SL, h, q, valid, vox);
+      }
   };
   uint32_t g = 0;
   for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
     const int tw = item % tiles_w, th = (item / tiles_w) % tiles_h, ck = item / tiles_hw;
     const int d0 = ck * DC, d1 = min(D, d0 + DC);
     const int first_id = max(d0 - 1, 0), last_id = min(d1, D - 1);
+#pragma unroll
+    for (int t = 0; t < NT; ++t)
+#pragma unroll
+      for (int i = 0; i < 3 * SL; ++i) acc[t][i] = 0.f;
     for (int id = first_id; id <= last_id; ++id) {
-      const int oa = max(id - 1, d0), ob = min(id + 1, d1 - 1);       // output slices fed by this input slice
-      const int fa = id == first_id ? oa : id + 1;                    // [fa, ob]: slices that receive their FIRST contribution
       int pend = -1;
       for (int grp = 0; grp < ngroups; ++grp, ++g) {
         const int s = g % NS;
         mbar_wait(bar_full + 8 * s, (uint32_t)((g / NS) & 1));
         const uint32_t sA = ring + s * stage_bytes + (uint32_t)half * 8u * G::PITCH;
         const uint32_t sB = wres ? wbase + grp * slab : ring + s * stage_bytes + a_bytes;
-        // MMAs of one (tap, variant) over the output slices [x, y]; a window that wraps around the 4-slot ring is split.
-        // Accumulator registers must be indexed statically: the (first slot, length) pair selects one unrolled case.
-        auto mma_range = [&](int x, int y, bool overwrite, uint32_t astart, uint32_t albo, uint32_t tile) {
-          while (x <= y) {
-            const int sx = x & 3;
-            const int len = min(y - x + 1, 4 - sx);
-            const uint64_t bd = make_desc(tile + (uint32_t)((x - id + 1) * NPAD) * 16u, blbo, 128);
-            const uint32_t accf = overwrite ? 0u : 1u;
-#pragma unroll
-            for (int c0 = 0; c0 < 4; ++c0) {
-#pragma unroll
-              for (int ln = 1; ln <= 3; ++ln) {
-                if (c0 + ln > 4 || c0 != sx || ln != len) continue;
-#pragma unroll
-                for (int t = 0; t < NT; ++t) {
-                  const uint64_t ad = make_desc(astart + t * 128, albo, G::PITCH);
-                  float* d = acc[t] + c0 * (NPAD / 2);
-                  if (ln == 1) mma_ss<NPAD>(d, ad, bd, accf);
-                  else if (ln == 2) mma_ss<2 * NPAD>(d, ad, bd, accf);
-                  else mma_ss<3 * NPAD>(d, ad, bd, accf);
-                }
-              }
-            }
-            x += len;
-          }
-        };
         wg_fence();
 #pragma unroll
         for (int kh = 0; kh < 3; ++kh) {
@@ -433,7 +406,6 @@ conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, i
             }
             const uint32_t aoff = sA + (uint32_t)sub * G::PAIR + (uint32_t)(rs * PC + cs) * 16u;
             const uint32_t t0 = sB + (uint32_t)(kh * 3 + kw) * 2u * btile, t1 = t0 + btile;   // w_hi tile, w_lo tile
-            const bool first = grp == 0 && kh == 0 && kw == 0;
             // variant list: (A start, A k-chunk stride, weight tile)
             const uint32_t va[3] = {KG == 1 ? aoff : aoff + G::SUB_BYTES, KG == 1 ? aoff : aoff, aoff};
             const uint32_t vl = KG == 1 ? G::SUB_BYTES : G::OCT_BYTES;
@@ -442,12 +414,9 @@ conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, i
 #pragma unroll
             for (int v = 0; v < 3; ++v) {
               if (v >= nv) break;
-              if (first && v == 0) {
-                if (fa > oa) mma_range(oa, fa - 1, false, va[v], vl, vt[v]);
-                if (fa <= ob) mma_range(fa, ob, true, va[v], vl, vt[v]);
-              } else {
-                mma_range(oa, ob, false, va[v], vl, vt[v]);
-              }
+              const uint64_t bd = make_desc(vt[v], blbo, 128);
+#pragma unroll
+              for (int t = 0; t < NT; ++t) mma_ss<3 * NPAD>(acc[t], make_desc(va[v] + t * 128, vl, G::PITCH), bd, 1u);
             }
           }
         }
@@ -462,8 +431,16 @@ conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, i
 #pragma unroll
       for (int t = 0; t < NT; ++t) fence_acc(acc[t]);
       release((uint32_t)pend);
-      if (id - 1 >= d0) epilogue(id - 1, th, tw);
-      if (id == last_id && id <= d1 - 1) epilogue(id, th, tw);
+      if (id - 1 >= d0) epilogue(id - 1, th, tw, std::integral_constant<int, 0>{});
+      if (id == last_id && id <= d1 - 1) epilogue(id, th, tw, std::integral_constant<int, 1>{});
+#pragma unroll
+      for (int t = 0; t < NT; ++t)
+#pragma unroll
+        for (int i = 0; i < SL; ++i) {
+          acc[t][i] = acc[t][SL + i];
+          acc[t][SL + i] = acc[t][2 * SL + i];
+          acc[t][2 * SL + i] = 0.f;
+        }
     }
   }
 }
@@ -473,12 +450,13 @@ int conv3d_tc_kg(int mode, int cin) { return (mode != CONV_S2 && cin >= 16) ? 2 
 // depth-streaming kernel: convolutions with depth stride 1 whose 3*Cout-wide weight tiles still fit shared memory
 int conv3d_tc_col(int mode, int sd, int cout) { return (mode == CONV_S1 || (mode == CONV_S2 && sd == 1)) && c3::npad(cout) <= 32; }
 
-size_t conv3d_tc_packed_halves(int mode, int cin, int cout) {   // the same for both layouts
-  return (size_t)3 * (cin / 8 / conv3d_tc_kg(mode, cin)) * (c3::slab_bytes(cout) / 2);
+size_t conv3d_tc_packed_halves(int mode, int cin, int cout) {   // the same for the col layout
+  return (size_t)3 * (cin / 8 / conv3d_tc_kg(mode, cin)) * (c3::slab_bytes(mode, cout) / 2);
 }
 
-// slab (kd, channel group g) = 9 weight blocks of [2 MMA variants][2 k-chunks][NPAD rows][8 halves]; blocks that are fused
-// into one MMA are interleaved as [variant][k-chunk][nb * NPAD rows][8] (conv: nb = 1; deconv: 4, 2, 2, 1)
+// slab (kd, channel group g) = weight blocks of [2 MMA variants][2 k-chunks][NPAD rows][8 halves]; blocks that are fused
+// into one MMA are interleaved as [variant][k-chunk][nb * NPAD rows][8] (conv: 9 taps, nb = 1; deconv: 4 input shifts,
+// nb = 4 classes in the order [0, 1, 3, 2], zero where the shift does not feed the class)
 // col layout (depth-streaming kernel): slab (channel group g) = [9 taps][2 variants][2 k-chunks][kd = 2, 1, 0][NPAD rows][8]
 __global__ void conv3d_tc_pack_kernel(const float* __restrict__ w32, __half* __restrict__ out, int cin, int cout, int NPAD,
                                       int KG, int deconv, int col, size_t total) {
@@ -486,11 +464,12 @@ __global__ void conv3d_tc_pack_kernel(const float* __restrict__ w32, __half* __r
   if (i >= total) return;
   const int e = (int)(i & 7);
   const size_t q = i >> 3;                           // 16-byte chunk
-  const int per_slab = col ? NPAD * 108 : NPAD * 36;
+  const int per_slab = col ? NPAD * 108 : (deconv ? NPAD * 64 : NPAD * 36);
   const int slab = (int)(q / per_slab), c = (int)(q % per_slab);
   const int ngroups = cin / 8 / KG;
   int kd = slab / ngroups, g = slab % ngroups;
-  int mm, kc, n, kh, kw;
+  int mm, kc, n, kh = 0, kw = 0;
+  bool tap = true;
   if (col) {
     g = slab;
     n = c % NPAD;
@@ -506,23 +485,21 @@ __global__ void conv3d_tc_pack_kernel(const float* __restrict__ w32, __half* __r
     mm = r & 1; r >>= 1;
     kh = r / 3; kw = r % 3;
   } else {
-    const int bs[4] = {0, 4, 6, 8}, nbs[4] = {4, 2, 2, 1};
-    const int tkh[4][4] = {{1, 1, 2, 2}, {1, 2, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}};
-    const int tkw[4][4] = {{1, 2, 2, 1}, {0, 0, 0, 0}, {2, 1, 0, 0}, {0, 0, 0, 0}};
-    int t = 3;
-    for (int k = 0; k < 3; ++k)
-      if (c < bs[k + 1] * 4 * NPAD) { t = k; break; }
-    const int cc = c - bs[t] * 4 * NPAD, nb = nbs[t];
-    mm = cc / (2 * nb * NPAD);
-    kc = (cc / (nb * NPAD)) & 1;
-    const int nn = cc % (nb * NPAD);
+    // tap (kh, kw) of input shift t feeding class column b; -1: zero block
+    const int tkh[4][4] = {{1, 1, 2, 2}, {-1, 1, 2, -1}, {-1, -1, 0, 0}, {-1, -1, 0, -1}};
+    const int tkw[4][4] = {{1, 2, 2, 1}, {-1, 0, 0, -1}, {-1, -1, 2, 1}, {-1, -1, 0, -1}};
+    const int t = c / (16 * NPAD), cc = c % (16 * NPAD);
+    mm = cc / (8 * NPAD);
+    kc = (cc / (4 * NPAD)) & 1;
+    const int nn = cc % (4 * NPAD);
     const int b = nn / NPAD;
     n = nn % NPAD;
     kh = tkh[t][b]; kw = tkw[t][b];
+    tap = kh >= 0;
   }
   const int ci = (KG == 1 ? g : g * 2 + kc) * 8 + e;
   float w = 0.f;
-  if (n < cout) w = w32[((size_t)((kd * 3 + kh) * 3 + kw) * cin + ci) * cout + n];
+  if (tap && n < cout) w = w32[((size_t)((kd * 3 + kh) * 3 + kw) * cin + ci) * cout + n];
   const __half hi = __float2half_rn(w);
   const __half lo = __float2half_rn(w - __half2float(hi));
   __half v;
@@ -658,7 +635,7 @@ static int launch_mode(const ConvTcArgs& a, cudaStream_t s) {
   else { OD = a.ID * a.SD; OH = a.IH * 2; OW = a.IW * 2; cells_h = a.IH; cells_w = a.IW; }
   const int num_sms = device_sm_count(current_device());
   const int NPAD = c3::npad(a.COUT);
-  const uint32_t b_bytes = c3::slab_bytes(a.COUT);
+  const uint32_t b_bytes = c3::slab_bytes(MODE, a.COUT);
   const int ncls = MODE == DECONV_S2 ? 4 : 1;
   // tile width: the widest tile (least halo) whose accumulators fit the registers of the MMA warpgroups and that keeps
   // the persistent CTAs busy
@@ -735,7 +712,7 @@ static int launch_col(const ConvTcArgs& a, cudaStream_t s) {
   const int nts[3] = {4, 2, 1};
   for (int k = 0; k < 3; ++k) {
     const int nt = nts[k];
-    if (4 * nt * NPAD > 128) continue;                          // accumulator registers: 4 slots x NT x NPAD / 2 <= 64 (more spill)
+    if (3 * nt * NPAD > 128) continue;                          // accumulator registers: 3 slices x NT x NPAD / 2 <= 64
     const uint32_t oct = nt == 4 ? c3::Geo<MODE, 4>::OCT_BYTES : (nt == 2 ? c3::Geo<MODE, 2>::OCT_BYTES : c3::Geo<MODE, 1>::OCT_BYTES);
     const size_t stage = align_up((size_t)a.KG * oct + (wres ? 0 : slab), 128);
     const size_t fixed = (wres ? wres_bytes : 0) + 256;

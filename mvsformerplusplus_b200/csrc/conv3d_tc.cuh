@@ -25,7 +25,8 @@ struct ConvTcArgs {
 
 int conv3d_tc_kg(int mode, int cin);                           // 2 (16 channels per unit) for cin >= 16 except strided convs
 size_t conv3d_tc_packed_halves(int mode, int cin, int cout);   // number of fp16 elements of one layer's packed slabs
-// w32: [27][cin][cout] fp32 (BN folded) -> slabs [kd][channel group][9 weight blocks x 2 MMA variants x 2 k-chunks x NPAD x 8]
+// w32: [27][cin][cout] fp32 (BN folded) -> slabs [kd][channel group][9 (transposed: 16) weight blocks x 2 MMA variants x
+// 2 k-chunks x NPAD x 8]
 int conv3d_tc_col(int mode, int sd, int cout);                 // 1: depth-streaming kernel (depth stride 1, Cout <= 32)
 int conv3d_tc_pack(const float* w32, __half* out, int mode, int sd, int cin, int cout, cudaStream_t s);
 int launch_conv3d_tc(const ConvTcArgs& a, int mode, int out_mode, cudaStream_t s);
