@@ -30,8 +30,6 @@
 //     epilogue of the current one runs.
 #include "conv3d_tc.cuh"
 
-#include <cuda.h>
-
 #include <type_traits>
 
 #include "linear_tc.cuh"
@@ -59,13 +57,6 @@ __host__ __device__ inline int npad(int cout) { return cout < 16 ? 16 : cout; }
 __host__ __device__ inline uint32_t slab_bytes(int mode, int cout) { return (uint32_t)npad(cout) * (mode == DECONV_S2 ? 1024u : 576u); }
 
 struct alignas(64) Maps { CUtensorMap m[4]; };   // CONV_S2: one map per (h, w) parity; otherwise m[0]
-
-// TMA tile load of a 5-D box (c, w, h, d, hi/lo); out-of-range coordinates (the conv padding) are filled with zeros
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, int c4, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-               : "memory");
-}
 }  // namespace c3
 
 // depth taps (kd, id) of output slice od
@@ -174,7 +165,7 @@ conv3d_tc_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, in
                 if (MODE == CONV_S1) { w0 = c0w - 1; h0 = c0h - 1; }
                 else if (MODE == CONV_S2) { w0 = c0w - (sub & 1); h0 = c0h - (sub >> 1); }   // odd plane: index j <-> 2j + 1
                 else { w0 = c0w; h0 = c0h; }
-                c3::tma_load_5d(st + (uint32_t)(og * NSUB + sub) * G::PAIR, &maps.m[sub], c, w0, h0, dt.id[ds], 0, full);
+                tma_load_5d(st + (uint32_t)(og * NSUB + sub) * G::PAIR, &maps.m[sub], c, w0, h0, dt.id[ds], 0, full);
               }
             }
             bulk_load(st + a_bytes, a.wtc + (size_t)(dt.kd[ds] * ngroups + grp) * (b_bytes / 2), b_bytes, full);
@@ -347,7 +338,7 @@ conv3d_col_kernel(const __grid_constant__ c3::Maps maps, ConvTcArgs a, int NS, i
                 int w0, h0;
                 if (MODE == CONV_S1) { w0 = c0w - 1; h0 = c0h - 1; }
                 else { w0 = c0w - (sub & 1); h0 = c0h - (sub >> 1); }
-                c3::tma_load_5d(st + (uint32_t)(og * NSUB + sub) * G::PAIR, &maps.m[sub], c, w0, h0, id, 0, full);
+                tma_load_5d(st + (uint32_t)(og * NSUB + sub) * G::PAIR, &maps.m[sub], c, w0, h0, id, 0, full);
               }
             }
             if (!wres) bulk_load(st + a_bytes, a.wtc + (size_t)grp * (slab / 2), slab, full);
@@ -552,20 +543,6 @@ int launch_merge_vec8(const __half* hi, const __half* lo, float* x, size_t n, cu
   merge_vec8_kernel<<<cdiv((long long)(n / 8), 256), 256, 0, s>>>(hi, lo, x, n / 8);
   MVSF_LAUNCH_CHECK("merge_vec8");
   return MVSF_OK;
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
 }
 
 // 5-D map (c, w, h, d, hi|lo) over the fp16 activation pair; sh/sw = 2 and (ph, pw) select one parity plane of (h, w)

@@ -10,7 +10,6 @@
 #include <cuda_fp16.h>
 #include <float.h>
 
-#include "linear.cuh"
 #include "linear_tc.cuh"
 #include "wgmma.cuh"
 

@@ -5,10 +5,9 @@
 // Tokens "(h w) c" of the reference are exactly channels-last pixels, so the stage-1 output is produced directly in
 // the [V][H][W][64] layout the warp kernels consume.  All source views are processed as one batch; the K/V
 // summaries of the two cross layers depend only on the reference view and are computed once.
+#include "conv2d_tc.cuh"
 #include "linattn.cuh"
-#include "linear.cuh"
 #include "linear_tc.cuh"
-#include "wgmma.cuh"
 
 namespace mvsf {
 
@@ -41,8 +40,6 @@ __global__ void tokens_add_pe_kernel(const float* __restrict__ f, const float* _
     if (p < L) d[(size_t)p * 64 + c] = tile[threadIdx.x][i] + __ldg(pe + (size_t)p * 64 + c);
   }
 }
-
-#include "fmt_smooth_tc.cuh"   // fused upsample + lateral add + 3x3 smooth conv on wgmma
 
 struct FmtWs {
   __half *xn2, *att2, *hid2;   // fp16 hi|lo split activations: [M][128], [M][128], [M][512]
@@ -161,15 +158,82 @@ reduce1x1_kernel(const float* __restrict__ x, const float* __restrict__ w, float
   }
 }
 
+// Phase 1 of smooth_k on the conv2d_tc template: pre = lateral + bilinear_up2(red) on the halo of the tile, written as the
+// planes of the single parity; red [V][h][w][C] (NHWC), lat [V][C][2h][2w] (NCHW).  The upsampled + added tensor never
+// goes to HBM.
+template <class L>
+struct PathwaySrc {
+  const float* red;
+  const float* lat;
+  int h, w;
+  static constexpr uint32_t EXTRA = 0;
+  static_assert(L::CI == L::CO && L::KS == 3 && L::S == 1, "pathway smooth conv: C -> C, 3x3, stride 1");
+  __device__ void fill(unsigned char* smem, int v, int y0, int x0, int tid) const {
+    constexpr int C = L::CI, PR = L::PR, PC = L::PC;
+    const int H = 2 * h, W = 2 * w;
+    const float* lv = lat + (size_t)v * C * H * W;
+    const float* rv = red + (size_t)v * h * w * C;
+    for (int i = tid; i < L::NO * PR * PC; i += 256) {
+      const int o = i / (PR * PC), pix = i - o * (PR * PC);
+      const int r = pix / PC, c = pix - r * PC;
+      const int y = y0 - 1 + r, x = x0 - 1 + c;
+      float pre[8];
+      if (y >= 0 && y < H && x >= 0 && x < W) {
+        // ATen area_pixel_compute_source_index(scale=0.5, align_corners=False): src = 0.5*(dst+0.5)-0.5, clamped at 0
+        const float sy = fmaxf(0.5f * ((float)y + 0.5f) - 0.5f, 0.0f);
+        const int ya = (int)sy, yb = ya + ((ya < h - 1) ? 1 : 0);
+        const float ly1 = sy - (float)ya, ly0 = 1.0f - ly1;
+        const float sx = fmaxf(0.5f * ((float)x + 0.5f) - 0.5f, 0.0f);
+        const int xa = (int)sx, xb = xa + ((xa < w - 1) ? 1 : 0);
+        const float lx1 = sx - (float)xa, lx0 = 1.0f - lx1;
+        const float* p00 = rv + ((size_t)ya * w + xa) * C + o * 8;
+        const float* p01 = rv + ((size_t)ya * w + xb) * C + o * 8;
+        const float* p10 = rv + ((size_t)yb * w + xa) * C + o * 8;
+        const float* p11 = rv + ((size_t)yb * w + xb) * C + o * 8;
+#pragma unroll
+        for (int q4 = 0; q4 < 2; ++q4) {
+          const float4 v00 = ldg4(p00 + q4 * 4), v01 = ldg4(p01 + q4 * 4), v10 = ldg4(p10 + q4 * 4), v11 = ldg4(p11 + q4 * 4);
+          const float a00[4] = {v00.x, v00.y, v00.z, v00.w}, a01[4] = {v01.x, v01.y, v01.z, v01.w};
+          const float a10[4] = {v10.x, v10.y, v10.z, v10.w}, a11[4] = {v11.x, v11.y, v11.z, v11.w};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float up = ly0 * (lx0 * a00[e] + lx1 * a01[e]) + ly1 * (lx0 * a10[e] + lx1 * a11[e]);
+            pre[q4 * 4 + e] = up + __ldg(lv + ((size_t)(o * 8 + q4 * 4 + e) * H + y) * W + x);
+          }
+        }
+      } else {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) pre[e] = 0.f;
+      }
+      __half* p = reinterpret_cast<__half*>(smem + L::plane(0, o, 0) + (uint32_t)pix * 16u);
+      split_store8(p, p + L::PLANE / 2, pre);   // hi plane of octet o, then its lo plane (+ PLANE bytes)
+    }
+  }
+};
+
+template <int C>
+struct NhwcOut {   // smooth_k has no bias and no activation: [V][H][W][C]
+  float* out;
+  static constexpr bool BIAS = false;
+  __device__ void store(int v, int H, int W, int y, int x, int ch, float a, float b) const {
+    *reinterpret_cast<float2*>(out + (((size_t)v * H + y) * W + x) * C + ch) = make_float2(a, b);
+  }
+};
+
+// smooth-conv weight tiles (sm_tc) come from c2d::pack_conv2d_tc
 template <int CIN, int COUT>
-static int run_pathway_level(const float* prev, const float* lat, const float* dr_w, const float* sm_w, float* red,
-                             float* pre, float* out, int V, int h, int w, cudaStream_t s) {
+static int run_pathway_level(const float* prev, const float* lat, const float* dr_w, const void* sm_tc, float* red,
+                             float* out, int V, int h, int w, cudaStream_t s) {
   const int M = V * h * w;
   reduce1x1_kernel<CIN, COUT><<<cdiv(M, 128), 128, 0, s>>>(prev, dr_w, red, M);
   MVSF_LAUNCH_CHECK("fmt_reduce1x1");
-  (void)pre;
-  return launch_fmt_smooth_tc<COUT>(red, lat, sm_w, out, V, h, w, s);
+  using L = c2d::Conv<COUT, COUT, 3, 1, 16, COUT>;
+  return c2d::launch_conv<L>(PathwaySrc<L>{red, lat, h, w}, NhwcOut<COUT>{out}, sm_tc, nullptr, V, 2 * h, 2 * w, s);
 }
+
+// packed smooth_1..3 weight tiles at the end of the workspace
+constexpr size_t SM_TC1 = c2d::conv2d_tc_bytes(32, 32, 3), SM_TC2 = c2d::conv2d_tc_bytes(16, 16, 3),
+                 SM_TC = SM_TC1 + SM_TC2 + c2d::conv2d_tc_bytes(8, 8, 3);
 
 }  // namespace mvsf
 
@@ -182,7 +246,7 @@ int mvsf_fmt_workspace_bytes(int V, int H1, int W1, size_t* bytes) {
   size_t L = (size_t)H1 * W1, VL = (size_t)V * L;
   size_t nblk = (L + KV_CHUNK - 1) / KV_CHUNK;
   size_t n = 640 * VL + 64 * L + (size_t)V * nblk * KVSZ + (size_t)(V + 2) * KVSZ + 64;
-  *bytes = n * sizeof(float);
+  *bytes = n * sizeof(float) + SM_TC;
   return MVSF_OK;
 }
 
@@ -204,7 +268,7 @@ int mvsf_fmt_forward(const float* f1, const float* f2, const float* f3, const fl
   ws.xn2 = reinterpret_cast<__half*>(base);                  // [V*L][128] halves (= 64 floats / token)
   ws.qkv = base + 64 * VL;                                   // [V*L][192]
   ws.att2 = reinterpret_cast<__half*>(ws.qkv + 192 * VL);    // [V*L][128] halves
-  ws.hid2 = ws.att2 + 128 * VL;                              // [V*L][512] halves  (576 VL floats in total; the pathway reuses 640 VL)
+  ws.hid2 = ws.att2 + 128 * VL;                              // [V*L][512] halves  (576 VL floats in total; the pathway reuses the first 128 VL)
   ws.wh = reinterpret_cast<const __half*>(wts16);
   ws.wl = ws.wh + n_wts;
   ws.ref0 = base + 640 * VL;          // [L][64]
@@ -232,11 +296,14 @@ int mvsf_fmt_forward(const float* f1, const float* f2, const float* f3, const fl
   if ((rc = run_block(xs, V - 1, L, b3, 3 * (size_t)B_SIZE, ws.kvc + KVSZ, ws, s, true, nullptr))) return rc;
 
   // top-down pathway (FMT.py:195-197), all views batched
+  unsigned char* sm_tc = static_cast<unsigned char*>(workspace) + need - SM_TC;
+  if ((rc = c2d::pack_conv2d_tc(wts + P_SM1, sm_tc, 32, 32, 3, 32, s))) return rc;
+  if ((rc = c2d::pack_conv2d_tc(wts + P_SM2, sm_tc + SM_TC1, 16, 16, 3, 16, s))) return rc;
+  if ((rc = c2d::pack_conv2d_tc(wts + P_SM3, sm_tc + SM_TC1 + SM_TC2, 8, 8, 3, 8, s))) return rc;
   float* red = base;                  // <= 128 VL floats
-  float* pre = base + 128 * VL;       // <= 512 VL floats
-  if ((rc = run_pathway_level<64, 32>(o1, f2, wts + P_DR1, wts + P_SM1, red, pre, o2, V, H1, W1, s))) return rc;
-  if ((rc = run_pathway_level<32, 16>(o2, f3, wts + P_DR2, wts + P_SM2, red, pre, o3, V, 2 * H1, 2 * W1, s))) return rc;
-  if ((rc = run_pathway_level<16, 8>(o3, f4, wts + P_DR3, wts + P_SM3, red, pre, o4, V, 4 * H1, 4 * W1, s))) return rc;
+  if ((rc = run_pathway_level<64, 32>(o1, f2, wts + P_DR1, sm_tc, red, o2, V, H1, W1, s))) return rc;
+  if ((rc = run_pathway_level<32, 16>(o2, f3, wts + P_DR2, sm_tc + SM_TC1, red, o3, V, 2 * H1, 2 * W1, s))) return rc;
+  if ((rc = run_pathway_level<16, 8>(o3, f4, wts + P_DR3, sm_tc + SM_TC1 + SM_TC2, red, o4, V, 4 * H1, 4 * W1, s))) return rc;
   return MVSF_OK;
 }
 }

@@ -1,45 +1,19 @@
 // FPN feature pyramid: models/module.py:208-239 FPNEncoder and :242-270 FPNDecoder (eval, feat_chs [8,16,32,64], BN folded).
-// Every 3x3 / 5x5 convolution is one launch of fpn_conv_kernel, an implicit GEMM on wgmma in the scheme of vis_cnn.cu and
-// fmt_smooth_tc.cuh:
-//   phase 1 (SIMT)   a "source" writes the input of the layer for one output tile plus its halo as fp16 hi|lo voxel-octet
-//                    PLANES in shared memory (plane[row][col] = 8 channels = 16 B; zero outside the image = the padding), so
-//                    a tap is a descriptor start address.  Strided layers use S x S PARITY planes (conv3d_tc.cu): plane
-//                    (py, px) holds input rows S i + py, columns S j + px, and tap (kh, kw) of output (r, c) is row
-//                    r + kh / S, column c + kw / S of parity plane (kh % S, kw % S).
-//   phase 2 (wgmma)  M = 8 x 8 output pixels per m64 block, N = NS output channels of the CTA's N block.  Per 16 input
-//                    channels: x_hi x [w_hi | w_lo] (N = 2 NS) and x_lo x w_hi (N = NS, onto the first half); 8 input
-//                    channels: one MMA [x_hi | x_lo] x [[w_hi; w_hi] | [w_lo; 0]].  fp32 accumulators in registers.
-//   phase 3          folded bias (+ BN) and LeakyReLU(0.1) -> NHWC fp32 (encoder), or Swish -> NCHW fp32 (decoder).
+// Every 3x3 / 5x5 convolution is one launch of the implicit-GEMM template conv2d_tc_kernel (conv2d_tc.cuh) with a source
+// and a destination of this file.
 // Sources: an NHWC fp32 tensor (encoder layers), conv00 computed in SIMT from the [N][3][H][W] image (fused conv00 + conv01:
 // conv00's output never reaches HBM), and the decoder's intra_k = up2(intra_{k-1}) + inner_k(lateral_k) (align_corners=True
 // bilinear + 1x1 conv with bias; the tile interior of intra_1 / intra_2 is also stored for the next level, the
-// full-resolution intra_3 is not).  out0 (1x1 at 1/8 resolution) is a small SIMT kernel.
-#include "common.cuh"
+// full-resolution intra_3 is not).  Epilogue: folded bias (+ BN), then the destination's LeakyReLU(0.1) -> NHWC fp32
+// (encoder) or Swish -> NCHW fp32 (decoder).  out0 (1x1 at 1/8 resolution) is a small SIMT kernel.
+#include "conv2d_tc.cuh"
 #include "linear_tc.cuh"
-#include "wgmma.cuh"
 
 namespace mvsf {
 namespace fpn {
-using namespace gmma;
+using namespace c2d;
 
-// one layer: CI -> CO channels, KS x KS kernel, stride S, output tile TR rows x 32 columns, NS output channels per CTA
-template <int CI_, int CO_, int KS_, int S_, int TR_, int NS_>
-struct Conv {
-  static constexpr int CI = CI_, CO = CO_, KS = KS_, S = S_, TR = TR_, NS = NS_;
-  static constexpr int PAD = (KS - 1) / 2, HALO = (KS - 1) / S;
-  static constexpr int PR = TR + HALO, PC = 32 + HALO;          // plane rows / columns
-  static constexpr int NO = CI / 8, NP = S * S, NG = CI < 16 ? 1 : CI / 16, NB = CO / NS;
-  static constexpr uint32_t PLANE = PR * PC * 16, PITCH = PC * 16;
-  static constexpr uint32_t BT = 64 * NS;                      // (tap, group) weight tile: [2 k-chunks][2 NS rows][8 halves]
-  static constexpr uint32_t WBYTES = KS * KS * NG * BT;        // weight tiles of one N block
-  static constexpr uint32_t OFF_W = NP * NO * 2 * PLANE, SMEM = OFF_W + WBYTES;
-  static_assert(CI % 8 == 0 && (CI == 8 || CI % 16 == 0) && CO % NS == 0 && TR % 8 == 0, "fpn conv shape");
-  static_assert(NS == 8 || NS == 16 || NS == 32, "fpn conv N block");
-  // plane of parity `par`, channel octet o, part hl (0 hi, 1 lo): groups of 16 channels are [hi o | lo o | hi o+1 | lo o+1]
-  __device__ static constexpr uint32_t plane(int par, int o, int hl) { return (uint32_t)((par * NO + o) * 2 + hl) * PLANE; }
-};
-
-// ---- sources (phase 1).  fill() is called by all 256 threads; the planes it writes are read after a fence + barrier.
+// ---- sources (phase 1)
 // input NHWC fp32 [N][IH][IW][CI]
 template <class L>
 struct NhwcSrc {
@@ -179,10 +153,11 @@ struct IntraSrc {
   }
 };
 
-// ---- destinations (phase 3): two consecutive channels ch, ch + 1 of one output pixel, bias already added
+// ---- destinations (phase 3): two consecutive channels ch, ch + 1 of one output pixel, folded bias b[CO] already added
 template <int CO>
 struct NhwcLeaky {   // encoder: LeakyReLU(0.1), [N][OH][OW][CO]
   float* out;
+  static constexpr bool BIAS = true;
   __device__ void store(int n, int OH, int OW, int y, int x, int ch, float a, float b) const {
     a = a > 0.f ? a : 0.1f * a;
     b = b > 0.f ? b : 0.1f * b;
@@ -193,88 +168,13 @@ __device__ __forceinline__ float swish(float v) { return v / (1.0f + expf(-v)); 
 template <int CO>
 struct NchwSwish {   // decoder: Swish, [N][CO][OH][OW]
   float* out;
+  static constexpr bool BIAS = true;
   __device__ void store(int n, int OH, int OW, int y, int x, int ch, float a, float b) const {
     float* p = out + (((size_t)n * CO + ch) * OH + y) * OW + x;
     p[0] = swish(a);
     p[(size_t)OH * OW] = swish(b);
   }
 };
-
-template <class L, class Src, class Dst>
-__global__ void __launch_bounds__(256)
-fpn_conv_kernel(const Src src, const Dst dst, const __half* __restrict__ wtc, const float* __restrict__ bias, int OH, int OW,
-                int tiles_x, int tiles_y, int ntiles) {
-  constexpr int NS = L::NS, KS = L::KS, S = L::S, NG = L::NG;
-  extern __shared__ __align__(128) unsigned char smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nb = blockIdx.y;
-  const uint32_t sb = smem_u32(smem);
-  // ---- once per CTA: the weight tiles of N block nb (packed at install time by mvsf_fpn_pack_tc)
-  {
-    const uint4* wsrc = reinterpret_cast<const uint4*>(wtc) + (size_t)nb * (L::WBYTES / 16);
-    uint4* wdst = reinterpret_cast<uint4*>(smem + L::OFF_W);
-    for (int i = tid; i < (int)(L::WBYTES / 16); i += 256) wdst[i] = __ldg(wsrc + i);
-  }
-  const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
-  float acc[2][NS];   // the m64 blocks of column groups 2 wg and 2 wg + 1: N = 2 NS accumulator columns [first | second]
-
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, n = tile / (tiles_x * tiles_y);
-    const int x0 = tx * 32, y0 = ty * L::TR;
-    src.fill(smem, n, y0, x0, tid);
-    fence_proxy_async();
-    __syncthreads();
-#pragma unroll 1
-    for (int rg = 0; rg < L::TR / 8; ++rg) {
-      wg_fence();
-#pragma unroll
-      for (int kh = 0; kh < KS; ++kh) {
-#pragma unroll
-        for (int kw = 0; kw < KS; ++kw) {
-          const int par = (kh % S) * S + (kw % S);
-          const uint32_t aoff = (uint32_t)((8 * rg + kh / S) * L::PC + kw / S) * 16u;
-#pragma unroll
-          for (int g = 0; g < NG; ++g) {
-            const uint64_t wb = make_desc(sb + L::OFF_W + (uint32_t)((kh * KS + kw) * NG + g) * L::BT, 2 * NS * 16, 128);
-            const uint32_t first = (kh | kw | g) ? 1u : 0u;
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              const uint32_t arow = sb + aoff + (uint32_t)(2 * wg + k) * 128u;
-              if constexpr (L::CI == 8) {   // K = [hi | lo] planes of the single octet
-                mma_ss<2 * NS>(acc[k], make_desc(arow + L::plane(par, 0, 0), L::PLANE, L::PITCH), wb, first);
-              } else {                      // K chunks = the hi (or lo) planes of octets 2 g and 2 g + 1
-                const uint32_t ah = arow + L::plane(par, 2 * g, 0);
-                mma_ss<2 * NS>(acc[k], make_desc(ah, 2 * L::PLANE, L::PITCH), wb, first);
-                mma_ss<NS>(acc[k], make_desc(ah + L::PLANE, 2 * L::PLANE, L::PITCH), wb, 1u);
-              }
-            }
-          }
-        }
-      }
-      wg_commit();
-      wg_wait<0>();
-      fence_regs<NS>(acc[0]);
-      fence_regs<NS>(acc[1]);
-      // ---- epilogue: accumulator i of this thread = row 16 wq + lane / 4 + 8 h of the m64 block (pixel row 2 wq + h,
-      //      column lane / 4), column 8 b + 2 q + e (+ NS for the x_hi w_lo half)
-#pragma unroll
-      for (int k = 0; k < 2; ++k)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int y = y0 + 8 * rg + 2 * wq + h, x = x0 + 8 * (2 * wg + k) + (lane >> 2);
-          if (y >= OH || x >= OW) continue;
-#pragma unroll
-          for (int b = 0; b < NS / 8; ++b) {
-            const int ch = nb * NS + 8 * b + 2 * q;
-            const float o0 = acc[k][4 * b + 2 * h] + acc[k][4 * b + 2 * h + NS / 2] + __ldg(bias + ch);
-            const float o1 = acc[k][4 * b + 2 * h + 1] + acc[k][4 * b + 2 * h + 1 + NS / 2] + __ldg(bias + ch + 1);
-            dst.store(n, OH, OW, y, x, ch, o0, o1);
-          }
-        }
-    }
-    __syncthreads();   // planes are free again
-  }
-}
 
 // out0 = Swish(BN(conv1x1(conv31) + b)):  c31 [N][h][w][64] -> out [N][64][h][w];  w = [64 ci][64 co] then b[64]
 __global__ void __launch_bounds__(128) fpn_out0_kernel(const float* __restrict__ c31, const float* __restrict__ w,
@@ -300,28 +200,6 @@ __global__ void __launch_bounds__(128) fpn_out0_kernel(const float* __restrict__
   }
 }
 
-// install time: fp32 [KS*KS taps][CI][CO] -> the weight tiles of fpn_conv_kernel, [N block][tap][group][2 kc][2 NS rows][8]
-__global__ void fpn_pack_kernel(const float* __restrict__ w, __half* __restrict__ out, int CI, int CO, int KK, int NS) {
-  const int NG = CI < 16 ? 1 : CI / 16;
-  const long long total = (long long)KK * NG * 64 * CO / 2;   // halves
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int e = (int)(i & 7);
-    long long rest = i >> 3;
-    const int row = (int)(rest % (2 * NS)); rest /= 2 * NS;
-    const int kc = (int)(rest & 1); rest >>= 1;
-    const int g = (int)(rest % NG); rest /= NG;
-    const int tap = (int)(rest % KK), nb = (int)(rest / KK);
-    const int part = row / NS, co = nb * NS + row % NS;
-    const int ci = CI == 8 ? e : g * 16 + kc * 8 + e;
-    const float wv = w[((size_t)tap * CI + ci) * CO + co];
-    const __half hi = __float2half_rn(wv), lo = __float2half_rn(wv - __half2float(hi));
-    __half v;
-    if (CI == 8) v = part == 0 ? hi : (kc == 0 ? lo : __float2half_rn(0.f));
-    else v = part == 0 ? hi : lo;
-    out[i] = v;
-  }
-}
-
 // ---- layer table.  fp32 blobs (packing.pack_fpn_encoder / pack_fpn_decoder): per layer w [KS*KS][CI][CO] then b[CO]
 struct LayerDesc { int ci, co, ks, ns; };
 constexpr LayerDesc kEnc[11] = {{3, 8, 7, 0},    {8, 8, 5, 8},    {8, 16, 5, 16},  {16, 16, 3, 16},
@@ -336,7 +214,7 @@ template <int I> using EncL = Conv<kEnc[I].ci, kEnc[I].co, kEnc[I].ks, (I == 2 |
 template <int K> using DecL = Conv<64, kDec[K].co, 3, 1, K == 0 ? 8 : 16, kDec[K].ns>;
 
 constexpr size_t layer_floats(const LayerDesc& d) { return (size_t)d.ks * d.ks * d.ci * d.co + d.co; }
-constexpr size_t layer_tc_bytes(const LayerDesc& d) { return (size_t)d.ks * d.ks * (d.ci < 16 ? 1 : d.ci / 16) * 64 * d.co; }
+constexpr size_t layer_tc_bytes(const LayerDesc& d) { return conv2d_tc_bytes(d.ci, d.co, d.ks); }
 static size_t enc_off(int i) { size_t o = 0; for (int j = 0; j < i; ++j) o += layer_floats(kEnc[j]); return o; }
 static size_t enc_tc_off(int i) { size_t o = 0; for (int j = 1; j < i; ++j) o += layer_tc_bytes(kEnc[j]); return o; }
 static size_t dec_inner_off(int k) {   // float offset of inner_{k+1}
@@ -348,40 +226,14 @@ static size_t dec_tc_off(int k) { size_t o = 0; for (int j = 0; j < k; ++j) o +=
 static size_t enc_tc_total() { return enc_tc_off(11); }
 static size_t dec_tc_total() { return dec_tc_off(3); }
 
-template <class L, class Src, class Dst>
-static int launch_conv(const Src& src, const Dst& dst, const void* wtc, const float* bias, int N, int OH, int OW,
-                       cudaStream_t s) {
-  constexpr uint32_t smem = L::SMEM + Src::EXTRA;
-  static_assert(smem <= 227 * 1024, "fpn conv: shared memory");
-  auto kern = fpn_conv_kernel<L, Src, Dst>;
-  static DeviceOnce once;
-  static int per_sm = 1;
-  const int dev = current_device();
-  if (once.need(dev)) {
-    MVSF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    MVSF_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem));
-    if (per_sm < 1) per_sm = 1;
-    once.done(dev);
-  }
-  const int tiles_x = cdiv(OW, 32), tiles_y = cdiv(OH, L::TR);
-  const long long ntiles = (long long)tiles_x * tiles_y * N;
-  MVSF_REQUIRE(ntiles < (1ll << 30), "fpn: image too large");
-  long long cap = (long long)per_sm * device_sm_count(dev) / L::NB;
-  if (cap < 1) cap = 1;
-  dim3 grid((unsigned)(ntiles < cap ? ntiles : cap), L::NB);
-  kern<<<grid, 256, smem, s>>>(src, dst, reinterpret_cast<const __half*>(wtc), bias, OH, OW, tiles_x, tiles_y, (int)ntiles);
-  MVSF_LAUNCH_CHECK("fpn_conv");
-  return MVSF_OK;
-}
-
 // encoder layer I (>= 2) reading an NHWC map of the previous layer's size
 template <int I>
 static int enc_layer(const float* in, float* out, const float* wts, const unsigned char* wtc, int N, int IH, int IW,
                      cudaStream_t s) {
   using L = EncL<I>;
   const int OH = IH / L::S, OW = IW / L::S;
-  return launch_conv<L>(NhwcSrc<L>{in, IH, IW}, NhwcLeaky<L::CO>{out}, wtc + enc_tc_off(I),
-                        wts + enc_off(I) + (size_t)L::KS * L::KS * L::CI * L::CO, N, OH, OW, s);
+  const float* bias = wts + enc_off(I) + (size_t)L::KS * L::KS * L::CI * L::CO;
+  return launch_conv<L>(NhwcSrc<L>{in, IH, IW}, NhwcLeaky<L::CO>{out}, wtc + enc_tc_off(I), bias, N, OH, OW, s);
 }
 
 template <int K>
@@ -389,8 +241,8 @@ static int dec_level(const float* prev, const float* lat, const float* wts, cons
                      float* out, int N, int h, int w, cudaStream_t s) {
   using L = DecL<K>;
   const size_t inner = dec_inner_off(K), conv = inner + (size_t)kLat[K] * 64 + 64;
-  return launch_conv<L>(IntraSrc<L, kLat[K]>{prev, lat, wts + inner, intra_out, h, w}, NchwSwish<L::CO>{out},
-                        wtc + dec_tc_off(K), wts + conv + (size_t)9 * 64 * L::CO, N, 2 * h, 2 * w, s);
+  return launch_conv<L>(IntraSrc<L, kLat[K]>{prev, lat, wts + inner, intra_out, h, w},
+                        NchwSwish<L::CO>{out}, wtc + dec_tc_off(K), wts + conv + (size_t)9 * 64 * L::CO, N, 2 * h, 2 * w, s);
 }
 
 static bool shape_ok(int N, int H, int W) {
@@ -418,9 +270,8 @@ extern "C" int mvsf_fpn_pack_tc(int part, const float* wts, void* wts_tc, size_t
     const LayerDesc& d = part == 0 ? kEnc[j + 1] : kDec[j];
     const float* w = wts + (part == 0 ? enc_off(j + 1) : dec_inner_off(j) + (size_t)kLat[j] * 64 + 64);
     unsigned char* o = out + (part == 0 ? enc_tc_off(j + 1) : dec_tc_off(j));
-    fpn_pack_kernel<<<cdiv(layer_tc_bytes(d) / 2, 256), 256, 0, (cudaStream_t)stream>>>(
-        w, reinterpret_cast<__half*>(o), d.ci, d.co, d.ks * d.ks, d.ns);
-    MVSF_LAUNCH_CHECK("fpn_pack_tc");
+    const int rc = pack_conv2d_tc(w, o, d.ci, d.co, d.ks, d.ns, (cudaStream_t)stream);
+    if (rc) return rc;
   }
   return MVSF_OK;
 }

@@ -19,12 +19,11 @@
 //   * taps outside the staged window (depth outliers) fall back to global loads for that lane only.
 // warp_corr.cu's spill plan (gather once, stream the stored correlations) is the default of the cascade; these kernels
 // serve the two-gather plan (plane sweeps, spill buffers over budget).
-#include <cuda.h>
 #include <float.h>
 #include <limits.h>
 #include <stdlib.h>
 
-#include "common.cuh"
+#include "wgmma.cuh"
 
 #ifndef MVSF_PS_BLOCKS8
 #define MVSF_PS_BLOCKS8 2        // resident CTAs per SM of the C = 8 pipeline kernel (ring of MVSF_PS_NBUF8 windows of 32 KB each);
@@ -39,6 +38,7 @@
 
 namespace mvsf {
 namespace wt {
+using namespace gmma;
 
 constexpr int TW = 32, TH = 8, THREADS = 256;   // reference-pixel tile: one warp per tile row
 constexpr int DCH = 8;                          // hypotheses per window (register-resident tap coordinates)
@@ -55,33 +55,14 @@ struct Cfg {
   static constexpr uint32_t BYTES = (WY / 2) * P;    // 32 KB (C = 8), 64 KB (C = 16)
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-               : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  return ok != 0;
-}
 // one lane polls, the warp reconverges; bounded so that a mis-programmed pipeline traps instead of hanging the GPU
 __device__ __forceinline__ void mbar_wait_warp(uint32_t bar, uint32_t parity) {
   if ((threadIdx.x & 31) == 0) {
     uint32_t it = 0;
     while (!mbar_try_wait(bar, parity))
-      if (++it > (1u << 26)) __trap();
+      if (++it > (1u << MVSF_MBAR_SPIN_LOG2)) __trap();
   }
   __syncwarp();
-}
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, int c4, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-               : "memory");
 }
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
   float4 v;
@@ -600,9 +581,7 @@ warp_stream_entropy_store_kernel(const __grid_constant__ CUtensorMap map, const 
         mx = fmaxf(mx, s);
       }
       __syncwarp();
-      if (lane == 0) {   // this warp is done with the window
-        asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(smem_u32(&sh.empty[buf])) : "memory");
-      }
+      if (lane == 0) mbar_arrive(smem_u32(&sh.empty[buf]));   // this warp is done with the window
       // softmax over D -> entropy (cost_volume.py:90-92).  Intrinsic exp / log (ex2 / lg2 based, ~1e-6 relative here: the
       // arguments are <= 0 resp. in (1e-7, 1]); the entropy feeds a CNN whose output is compared at 5e-4.
       float Z = 0.f, ent = 0.f;
@@ -693,20 +672,6 @@ warp_stream_select_kernel(const float* __restrict__ homs, const float* __restric
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
 // 5-D view (c, y&1, x, y/2, view) of the channels-last feature tensor [V][H][W][C] (H even)
 template <int C>
 static int make_window_map(CUtensorMap* m, const float* feat, int V, int H, int W) {

@@ -6,12 +6,14 @@
 //     (128 threads, warps 4k .. 4k+3).  Accumulator element i of thread t (warp w = t/32 of the warpgroup, lane l):
 //       row 16 w + l/4 + 8 ((i/2) % 2),  column 8 (i/4) + 2 (l%4) + (i%2);
 //     the first N'/2 registers of an m64nN accumulator are the m64nN' accumulator of its first N' columns;
-//   - mbarrier waits (bounded: trap instead of hanging the GPU), named barriers, cp.async fills of operand tiles.
+//   - mbarrier waits (bounded: trap instead of hanging the GPU), named barriers, cp.async fills of operand tiles, TMA
+//     tensor loads and the driver's tensor-map encoder.
 // Field layouts follow the PTX ISA (matrix descriptor of wgmma, section "Matrix Descriptor Format").
 #pragma once
 #ifndef MVSF_MBAR_SPIN_LOG2
 #define MVSF_MBAR_SPIN_LOG2 26   // bounded mbarrier waits: ~1.5 s of polling before the trap
 #endif
+#include <cuda.h>
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -59,6 +61,12 @@ __device__ __forceinline__ void expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+// TMA tile load of a 5-D box; coordinates outside the tensor are zero-filled
+__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, int c4, uint32_t bar) {
+  asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
+               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+               : "memory");
 }
 // named barrier among a subset of the CTA's warps (id 1..15; id 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
@@ -214,6 +222,21 @@ __device__ __forceinline__ void split_store2(__half* hi_dst, __half* lo_dst, flo
   const float2 hf = __half22float2(h);
   *reinterpret_cast<__half2*>(hi_dst) = h;
   *reinterpret_cast<__half2*>(lo_dst) = __floats2half2_rn(a - hf.x, b - hf.y);
+}
+
+// cuTensorMapEncodeTiled from the driver the runtime uses (nullptr if it has none)
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+inline EncodeTiledFn encode_tiled_fn() {
+  static EncodeTiledFn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+  }
+  return fn;
 }
 
 }  // namespace gmma
