@@ -18,7 +18,7 @@
 #include <atomic>
 #include <mutex>
 
-#include "common.cuh"
+#include "warp_geom.cuh"
 
 namespace mvsf {
 
@@ -30,7 +30,7 @@ int warp_tile_aggregate(const float* feat, const float* homs, const float* depth
                         int D, int H, int W, cudaStream_t s);
 bool warp_stream_store_supported(const float* feat, const float* corr, int C, int G, int D, int H, int W);
 int warp_stream_entropy_store(const float* feat, const float* homs, const float* depth, float* entropy, float* corr, int V,
-                              int C, int D, int H, int W, int* select, int max_miss_permille, cudaStream_t s);
+                              int H, int W, int* select, int max_miss_permille, cudaStream_t s);
 
 constexpr int kMaxGenericD = 512;
 
@@ -53,9 +53,8 @@ struct __align__(16) TapTable {
 
 // phase 1 for one (view, chunk): taps t = lane and lane+32, t = di*P + pi
 template <int C>
-__device__ __forceinline__ void build_taps(TapTable& tb, const float* __restrict__ depth, const Hom& m, float rx, float ry,
-                                           float rz, const CoordConst& cc, int p1, int d0, int D, int HW, int H, int W,
-                                           int lane) {
+__device__ __forceinline__ void build_taps(TapTable& tb, const float* __restrict__ depth, const Hom& m, const float3& ray,
+                                           const CoordConst& cc, int p1, int d0, int D, int HW, int H, int W, int lane) {
   constexpr int P = WC<C>::P;
 #pragma unroll
   for (int k = 0; k < 2; ++k) {
@@ -63,7 +62,7 @@ __device__ __forceinline__ void build_taps(TapTable& tb, const float* __restrict
     const int d = d0 + t / P;
     const float dv = (d < D) ? __ldg(depth + (size_t)d * HW + p1) : 1.0f;
     float ix, iy;
-    warp_coord_fast(rx, ry, rz, m, dv, cc, ix, iy);
+    warp_coord_fast(ray, m, dv, cc, ix, iy);
     int4 off;
     float4 wt;
     make_tap_fast(ix, iy, W, H, C, off, wt);
@@ -119,9 +118,9 @@ warp_corr_entropy_kernel(const float* __restrict__ feat, const float* __restrict
   TapTable& tb = tables[warp];
   const int HW = H * W;
   const int v = blockIdx.y;
-  // STRIDED (the adaptive launch behind the selection kernel, C = 8): a capped grid strides over the 8-warp pixel blocks, so
-  // that the launch that finds skip_if set costs microseconds instead of 55 000 exiting CTAs (and the kernel itself is
-  // faster at C = 8, T&T 1.43 -> 1.24 ms; at C = 16..64 the loop costs registers - 143 at C = 64 - and is not used)
+  // STRIDED (the adaptive launch behind the selection kernel, C = 8 only): a capped grid strides over the 8-warp pixel
+  // blocks, so that the launch that finds skip_if set costs microseconds instead of 55 000 exiting CTAs (and the kernel
+  // itself is faster at C = 8, T&T 1.43 -> 1.24 ms; at C = 16..64 the loop costs registers - 143 at C = 64)
   int bx = blockIdx.x;
   do {
   const int pix0 = (bx * 8 + warp) * P;
@@ -135,10 +134,7 @@ warp_corr_entropy_kernel(const float* __restrict__ feat, const float* __restrict
   const Hom m = load_hom(homs + (size_t)v * 12);
   const CoordConst cc = make_coord_const(W, H);
   const int y1 = p1 / W, x1 = p1 - y1 * W;
-  const float fx = (float)x1, fy = (float)y1;
-  const float rx = __fadd_rn(fmaf(m.r01, fy, __fmul_rn(m.r00, fx)), m.r02);
-  const float ry = __fadd_rn(fmaf(m.r11, fy, __fmul_rn(m.r10, fx)), m.r12);
-  const float rz = __fadd_rn(fmaf(m.r21, fy, __fmul_rn(m.r20, fx)), m.r22);
+  const float3 ray = ref_ray(m, (float)x1, (float)y1);
   const float4 r = ldg4(feat + (size_t)p2 * C + lip * 4);
   const float* __restrict__ src = feat + (size_t)(v + 1) * HW * C + lip * 4;
   const float gscale = (float)G / (float)C;
@@ -147,7 +143,7 @@ warp_corr_entropy_kernel(const float* __restrict__ feat, const float* __restrict
   const int nch = GENERIC ? (D + DCH - 1) / DCH : 1;
   for (int ch = 0; ch < nch; ++ch) {
     const int d0 = ch * DCH;
-    build_taps<C>(tb, depth, m, rx, ry, rz, cc, p1, d0, D, HW, H, W, lane);
+    build_taps<C>(tb, depth, m, ray, cc, p1, d0, D, HW, H, W, lane);
     __syncwarp();
     float part[DCH];
     const int pi = lane / LPP;
@@ -243,10 +239,8 @@ warp_corr_aggregate_kernel(const float* __restrict__ feat, const float* __restri
     float wsum = 0.f;
     for (int v = 0; v < V - 1; ++v) {
       const Hom m = load_hom(homs + (size_t)v * 12);
-      const float rx = __fadd_rn(fmaf(m.r01, fy, __fmul_rn(m.r00, fx)), m.r02);
-      const float ry = __fadd_rn(fmaf(m.r11, fy, __fmul_rn(m.r10, fx)), m.r12);
-      const float rz = __fadd_rn(fmaf(m.r21, fy, __fmul_rn(m.r20, fx)), m.r22);
-      build_taps<C>(tb, depth, m, rx, ry, rz, cc, p1, d0, D, HW, H, W, lane);
+      const float3 ray = ref_ray(m, fx, fy);
+      build_taps<C>(tb, depth, m, ray, cc, p1, d0, D, HW, H, W, lane);
       __syncwarp();
       const float* __restrict__ src = feat + (size_t)(v + 1) * HW * C + lip * 4;
       const float w = __ldg(vis + (size_t)v * HW + p2);
@@ -312,13 +306,10 @@ __global__ void homo_warp_kernel(const float* __restrict__ src, const float* __r
   if (p >= HW) return;
   int y = p / W, x = p - y * W;
   const Hom m = load_hom(hom);
-  const float fx = (float)x, fy = (float)y;
-  const float rx = __fadd_rn(fmaf(m.r01, fy, __fmul_rn(m.r00, fx)), m.r02);
-  const float ry = __fadd_rn(fmaf(m.r11, fy, __fmul_rn(m.r10, fx)), m.r12);
-  const float rz = __fadd_rn(fmaf(m.r21, fy, __fmul_rn(m.r20, fx)), m.r22);
+  const float3 ray = ref_ray(m, (float)x, (float)y);
   const float half_w = (float)(W - 1) * 0.5f, half_h = (float)(H - 1) * 0.5f;
   float ix, iy, z;
-  warp_coord(rx, ry, rz, m, __ldg(depth + (size_t)d * HW + p), half_w, half_h, (float)(W - 1), (float)(H - 1), ix, iy, z);
+  warp_coord(ray, m, __ldg(depth + (size_t)d * HW + p), half_w, half_h, (float)(W - 1), (float)(H - 1), ix, iy, z);
   Tap t = make_tap(ix, iy, W, H, C);
   for (int c = 0; c < C; ++c) {
     float a = __ldg(src + t.o00 + c), b = __ldg(src + t.o01 + c), cc = __ldg(src + t.o10 + c), dd = __ldg(src + t.o11 + c);
@@ -332,30 +323,31 @@ __global__ void homo_warp_kernel(const float* __restrict__ src, const float* __r
 }
 
 template <int C>
-static int launch_entropy(const float* feat, const float* homs, const float* depth, float* entropy, float* corr, int V, int G,
-                          int D, int H, int W, cudaStream_t s, const int* skip_if = nullptr) {
+static void launch_entropy(const float* feat, const float* homs, const float* depth, float* entropy, float* corr, int V, int G,
+                           int D, int H, int W, cudaStream_t s) {
   constexpr int P = WC<C>::P;
   dim3 grid(cdiv((long long)H * W, 8 * P), V - 1);
-  if (skip_if) {   // adaptive launch (may find nothing to do): a capped, grid-strided grid
-    const int cap = device_sm_count(current_device()) * 16;
-    if ((int)grid.x > cap) grid.x = cap;
-    if (corr && D == WC<C>::DCH) {
-      warp_corr_entropy_kernel<C, false, C / 8, true><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, corr, G, D, H, W, skip_if);
-      return 0;
-    }
-    return -1;   // only the spill plan's fixed-D instance is launched this way
-  }
   if (corr) {   // G == 8 (checked by the caller)
     if (D == WC<C>::DCH)
-      warp_corr_entropy_kernel<C, false, C / 8><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, corr, G, D, H, W, skip_if);
+      warp_corr_entropy_kernel<C, false, C / 8><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, corr, G, D, H, W, nullptr);
     else
-      warp_corr_entropy_kernel<C, true, C / 8><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, corr, G, D, H, W, skip_if);
+      warp_corr_entropy_kernel<C, true, C / 8><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, corr, G, D, H, W, nullptr);
   } else if (D == WC<C>::DCH) {
-    warp_corr_entropy_kernel<C, false, 0><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, nullptr, G, D, H, W, skip_if);
+    warp_corr_entropy_kernel<C, false, 0><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, nullptr, G, D, H, W, nullptr);
   } else {
-    warp_corr_entropy_kernel<C, true, 0><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, nullptr, G, D, H, W, skip_if);
+    warp_corr_entropy_kernel<C, true, 0><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, nullptr, G, D, H, W, nullptr);
   }
-  return 0;
+}
+
+// The spill plan's L1 kernel at C = 8, D = 4 behind the selection kernel: returns at once unless skip_if[0] == 0.  It may
+// find nothing to do, so it runs as a capped, grid-strided grid.
+static void launch_entropy_behind_select(const float* feat, const float* homs, const float* depth, float* entropy, float* corr,
+                                         int V, int H, int W, cudaStream_t s, const int* skip_if) {
+  constexpr int P = WC<8>::P;
+  dim3 grid(cdiv((long long)H * W, 8 * P), V - 1);
+  const int cap = device_sm_count(current_device()) * 16;
+  if ((int)grid.x > cap) grid.x = cap;
+  warp_corr_entropy_kernel<8, false, 1, true><<<grid, 256, 0, s>>>(feat, homs, depth, entropy, corr, 8, WC<8>::DCH, H, W, skip_if);
 }
 
 // volume[d][p][g] = sum_v vis[v][p] * corr[v][d][p][g] / (sum_v vis[v][p] + 1e-6)   (cost_volume.py:95-101), G = 8
@@ -483,25 +475,25 @@ static int warp_corr_entropy_impl(const float* feat, const float* homs, const fl
   MVSF_REQUIRE(C % G == 0 && (C == 8 || C == 16 || C == 32 || C == 64), "warp_corr_entropy: C must be 8/16/32/64, C %% G == 0");
   MVSF_REQUIRE(D <= kMaxGenericD, "warp_corr_entropy: D <= %d", kMaxGenericD);
   cudaStream_t s = (cudaStream_t)stream;
-  if (corr && g_use_tile && warp_stream_store_supported(feat, corr, C, G, D, H, W)) {
-    // finest stage of the cascade (C = 8, D = 4): persistent TMA producer / consumer pipeline kernel, as long as the taps of
-    // this call fit its windows (decided on the device, per call: see warp_stream_select_kernel).  The C = 16, D = 8
-    // instance is not faster than the L1 kernel on either workload (DTU 0.345 vs 0.336 ms, T&T 1.88 vs 0.94 ms) and only
-    // runs when forced (mvsf_warp_corr_set_tile_path(2)).
-    const bool forced = g_use_tile == 2;
-    if (forced || C == 8) {
-      int* select = forced ? nullptr : select_slot();
-      if (forced || select) {
-        int rc = warp_stream_entropy_store(feat, homs, depth, entropy, corr, V, C, D, H, W, select, g_max_miss_permille, s);
-        if (rc) return rc;
-        MVSF_LAUNCH_CHECK("warp_stream_entropy_store");
-        if (forced) return MVSF_OK;
-        count_launch();   // the selection kernel
-        launch_entropy<8>(feat, homs, depth, entropy, corr, V, G, D, H, W, s, select);   // returns at once unless select[0] == 0
-        MVSF_LAUNCH_CHECK("warp_corr_entropy");
-        return MVSF_OK;
-      }
-    }
+  // finest stage of the cascade (C = 8, D = 4): persistent TMA producer / consumer pipeline kernel, as long as the taps of
+  // this call fit its windows (decided on the device, per call: see warp_stream_select_kernel).  C = 16, D = 8 stays on the
+  // L1 kernel: the pipeline was not faster on either workload (DTU 0.345 vs 0.336 ms, T&T 1.88 vs 0.94 ms).
+  const bool pipeline = corr && g_use_tile && warp_stream_store_supported(feat, corr, C, G, D, H, W);
+  if (pipeline && g_use_tile == 2) {   // forced
+    int rc = warp_stream_entropy_store(feat, homs, depth, entropy, corr, V, H, W, nullptr, g_max_miss_permille, s);
+    if (rc) return rc;
+    MVSF_LAUNCH_CHECK("warp_stream_entropy_store");
+    return MVSF_OK;
+  }
+  int* select = pipeline ? select_slot() : nullptr;
+  if (select) {   // adaptive: the selection kernel, the pipeline kernel and the L1 kernel; the one not chosen returns at once
+    int rc = warp_stream_entropy_store(feat, homs, depth, entropy, corr, V, H, W, select, g_max_miss_permille, s);
+    if (rc) return rc;
+    count_launch();   // the selection kernel
+    MVSF_LAUNCH_CHECK("warp_stream_entropy_store");
+    launch_entropy_behind_select(feat, homs, depth, entropy, corr, V, H, W, s, select);
+    MVSF_LAUNCH_CHECK("warp_corr_entropy");
+    return MVSF_OK;
   }
   if (!corr && g_use_tile && warp_tile_supported(feat, C, G, D, H, W)) {
     int rc = warp_tile_entropy(feat, homs, depth, entropy, V, C, D, H, W, s);

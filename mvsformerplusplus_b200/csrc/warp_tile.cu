@@ -21,28 +21,21 @@
 // serve the two-gather plan (plane sweeps, spill buffers over budget).
 #include <float.h>
 #include <limits.h>
-#include <stdlib.h>
 
+#include "warp_geom.cuh"
 #include "wgmma.cuh"
-
-#ifndef MVSF_PS_BLOCKS8
-#define MVSF_PS_BLOCKS8 2        // resident CTAs per SM of the C = 8 pipeline kernel (ring of MVSF_PS_NBUF8 windows of 32 KB each);
-                                 // measured at DTU stage 4: 2 CTAs x 3 windows 0.367 ms, 3 CTAs x 2 windows 0.444 ms
-#endif
-#ifndef MVSF_PS_NBUF8
-#define MVSF_PS_NBUF8 3
-#endif
-#ifndef MVSF_WT_PASSB_BLOCKS
-#define MVSF_WT_PASSB_BLOCKS 3   // resident CTAs per SM of the C = 8, D <= 4 aggregation kernel (3 costs ~20 spilled registers)
-#endif
 
 namespace mvsf {
 namespace wt {
 using namespace gmma;
 
-constexpr int TW = 32, TH = 8, THREADS = 256;   // reference-pixel tile: one warp per tile row
-constexpr int DCH = 8;                          // hypotheses per window (register-resident tap coordinates)
+constexpr int TW = 32, THREADS = 256;   // reference-pixel tile: one warp per tile row
 constexpr int kMaxD = 512;
+// resident CTAs per SM of the C = 8, D <= 4 aggregation kernel (3 costs ~20 spilled registers)
+constexpr int kPassBBlocks8 = 3;
+// resident CTAs per SM of the pipeline kernel and its ring of windows (32 KB each); measured at DTU stage 4:
+// 2 CTAs x 3 windows 0.367 ms, 3 CTAs x 2 windows 0.444 ms
+constexpr int kPsBlocks = 2, kPsNbuf = 3;
 
 template <int C>
 struct Cfg {
@@ -80,6 +73,26 @@ struct Lane {
   bool b0, b1, b2;      // bits of (lane & 7) that are XORed into the bank-group index of a round
   uint32_t base[2];     // window base + 16-byte piece offset for rounds with i0 = 0 / 1
 };
+// Lane constants for a window at shared address `win`, and the first channel of the lane's quad A / quad B
+// (sub = which 8-channel slice of its pixel the lane owns).
+template <int C>
+__device__ __forceinline__ Lane make_lane(int lane, int sub, uint32_t win, int& chA, int& chB) {
+  Lane L;
+  if (C == 8) {
+    L.b0 = lane & 1; L.b1 = (lane >> 1) & 1; L.b2 = (lane >> 2) & 1;
+    L.base[0] = win + (L.b0 ? 16 : 0);
+    L.base[1] = win + (L.b0 ? 0 : 16);
+    chA = L.b0 ? 4 : 0; chB = L.b0 ? 0 : 4;
+  } else {
+    // lanes 2j, 2j+1 = the two channel halves of one pixel; bits 1-2 of the lane = tap slot inside an LDS.128 phase
+    L.b0 = false; L.b1 = (lane >> 1) & 1; L.b2 = (lane >> 2) & 1;
+    const int q0 = 2 * sub + (L.b1 ? 1 : 0), q1 = 2 * sub + (L.b1 ? 0 : 1);
+    L.base[0] = win + q0 * 16;
+    L.base[1] = win + q1 * 16;
+    chA = q0 * 4; chB = q1 * 4;
+  }
+  return L;
+}
 
 // One tap (4 corners x 8 channels of this lane) from the staged window: sA / sB receive the bilinear sample of the lane's
 // two channel quads (quad A = the one read in rounds with i0 = 0).  (lx, ly) = integer tap position relative to the window
@@ -144,22 +157,32 @@ __device__ __forceinline__ void gather_global(const float* __restrict__ srcA, co
   fma4(sA, wt.w, ldg4(srcA + off.w)); fma4(sB, wt.w, ldg4(srcB + off.w));
 }
 
-struct TapCoord {
-  float fx, fy;
-  int x0, y0;
-  bool inb;   // sample position inside (-1, W) x (-1, H): otherwise every corner is outside the image -> contributes 0
+// Bounding box {min x0, max x0, min y0, max y0} of the in-image taps added to it (empty: x0 > x1)
+struct Bbox {
+  int x0 = INT_MAX, x1 = INT_MIN, y0 = INT_MAX, y1 = INT_MIN;
+  __device__ __forceinline__ void add(const TapCoord& t) {
+    if (t.inb) { x0 = min(x0, t.x0); x1 = max(x1, t.x0); y0 = min(y0, t.y0); y1 = max(y1, t.y0); }
+  }
+  __device__ __forceinline__ void reduce_warp() {
+    x0 = __reduce_min_sync(0xffffffffu, x0);
+    x1 = __reduce_max_sync(0xffffffffu, x1);
+    y0 = __reduce_min_sync(0xffffffffu, y0);
+    y1 = __reduce_max_sync(0xffffffffu, y1);
+  }
 };
-__device__ __forceinline__ TapCoord split_coord(float ix, float iy, int W, int H) {
-  TapCoord t;
-  t.inb = (ix > -1.0f) && (ix < (float)W) && (iy > -1.0f) && (iy < (float)H);   // false for NaN / Inf
-  const float sx = t.inb ? ix : 0.0f, sy = t.inb ? iy : 0.0f;
-  const float MAGIC = 12582912.0f;   // 1.5 * 2^23: round-down add = floor (|s| < 2^22)
-  const float tx = __fadd_rd(sx, MAGIC), ty = __fadd_rd(sy, MAGIC);
-  t.x0 = __float_as_int(tx) - 0x4B400000;
-  t.y0 = __float_as_int(ty) - 0x4B400000;
-  t.fx = sx - (tx - MAGIC);
-  t.fy = sy - (ty - MAGIC);
-  return t;
+// Origin (ox, oy even) of the WX x WY window centred on a bounding box of tap corners (0, 0 for an empty box)
+template <int C>
+__device__ __forceinline__ int2 window_origin(const Bbox& b) {
+  using K = Cfg<C>;
+  if (b.x0 > b.x1) return make_int2(0, 0);
+  const int slack_x = K::WX - (b.x1 + 2 - b.x0), slack_y = K::WY - (b.y1 + 2 - b.y0);
+  return make_int2(b.x0 - (slack_x > 0 ? slack_x / 2 : 0), (b.y0 - (slack_y > 0 ? slack_y / 2 : 0)) & ~1);
+}
+// an in-image tap (inb) whose corner (lx, ly), relative to the window origin, puts all four corners inside the window
+template <int C>
+__device__ __forceinline__ bool in_window(bool inb, int lx, int ly) {
+  using K = Cfg<C>;
+  return inb && (unsigned)lx <= (unsigned)(K::WX - 2) && (unsigned)ly <= (unsigned)(K::WY - 2);
 }
 
 struct Shared {
@@ -171,26 +194,20 @@ struct Shared {
 // waits for it.  Returns the window origin (ox, oy even) to every thread.  `slot` alternates per call.
 template <int C>
 __device__ __forceinline__ void stage_window(const CUtensorMap* map, Shared& sh, uint32_t win, int slot, uint32_t& phase, int view,
-                                             int mnx, int mxx, int mny, int mxy, int& ox, int& oy) {
+                                             Bbox b, int& ox, int& oy) {
   using K = Cfg<C>;
-  mnx = __reduce_min_sync(0xffffffffu, mnx);
-  mxx = __reduce_max_sync(0xffffffffu, mxx);
-  mny = __reduce_min_sync(0xffffffffu, mny);
-  mxy = __reduce_max_sync(0xffffffffu, mxy);
+  b.reduce_warp();
   if ((threadIdx.x & 31) == 0) {
-    atomicMin(&sh.bbox[slot][0], mnx);
-    atomicMax(&sh.bbox[slot][1], mxx);
-    atomicMin(&sh.bbox[slot][2], mny);
-    atomicMax(&sh.bbox[slot][3], mxy);
+    atomicMin(&sh.bbox[slot][0], b.x0);
+    atomicMax(&sh.bbox[slot][1], b.x1);
+    atomicMin(&sh.bbox[slot][2], b.y0);
+    atomicMax(&sh.bbox[slot][3], b.y1);
   }
   __syncthreads();   // bbox complete; every lane has also finished reading the previous window
-  const int bx0 = sh.bbox[slot][0], bx1 = sh.bbox[slot][1], by0 = sh.bbox[slot][2], by1 = sh.bbox[slot][3];
-  if (bx0 > bx1) { ox = 0; oy = 0; }
-  else {
-    const int slack_x = K::WX - (bx1 + 2 - bx0), slack_y = K::WY - (by1 + 2 - by0);
-    ox = bx0 - (slack_x > 0 ? slack_x / 2 : 0);
-    oy = (by0 - (slack_y > 0 ? slack_y / 2 : 0)) & ~1;
-  }
+  b.x0 = sh.bbox[slot][0]; b.x1 = sh.bbox[slot][1]; b.y0 = sh.bbox[slot][2]; b.y1 = sh.bbox[slot][3];
+  const int2 o = window_origin<C>(b);
+  ox = o.x;
+  oy = o.y;
   if (threadIdx.x == 0) {
     sh.bbox[slot ^ 1][0] = INT_MAX; sh.bbox[slot ^ 1][1] = INT_MIN;   // reset the other slot for the next window
     sh.bbox[slot ^ 1][2] = INT_MAX; sh.bbox[slot ^ 1][3] = INT_MIN;
@@ -206,7 +223,7 @@ __device__ __forceinline__ void stage_window(const CUtensorMap* map, Shared& sh,
 template <int C>
 struct ViewCtx {
   Hom m;
-  float rx, ry, rz;
+  float3 ray;
   const float* srcA;
   const float* srcB;
 };
@@ -220,22 +237,21 @@ template <int C, int DCHT, typename F>
 __device__ __forceinline__ void process_chunk(const CUtensorMap* map, Shared& sh, uint32_t win, int& slot, uint32_t& phase,
                                               const Lane& L, const ViewCtx<C>& vc, int view, const float* __restrict__ depth_p,
                                               int HW, int d0, int n, bool active, const CoordConst& cc, int W, int H, F&& consume) {
-  using K = Cfg<C>;
   float ix, iy;
-  warp_coord_lean(vc.rx, vc.ry, vc.rz, vc.m, __ldg(depth_p + (size_t)d0 * HW), cc, ix, iy);
+  warp_coord_lean(vc.ray, vc.m, __ldg(depth_p + (size_t)d0 * HW), cc, ix, iy);
   TapCoord tF = split_coord(ix, iy, W, H);
   tF.inb = tF.inb && active;
   TapCoord tL = tF;
   if (n > 1) {
-    warp_coord_lean(vc.rx, vc.ry, vc.rz, vc.m, __ldg(depth_p + (size_t)(d0 + n - 1) * HW), cc, ix, iy);
+    warp_coord_lean(vc.ray, vc.m, __ldg(depth_p + (size_t)(d0 + n - 1) * HW), cc, ix, iy);
     tL = split_coord(ix, iy, W, H);
     tL.inb = tL.inb && active;
   }
-  int mnx = INT_MAX, mxx = INT_MIN, mny = INT_MAX, mxy = INT_MIN;
-  if (tF.inb) { mnx = mxx = tF.x0; mny = mxy = tF.y0; }
-  if (tL.inb) { mnx = min(mnx, tL.x0); mxx = max(mxx, tL.x0); mny = min(mny, tL.y0); mxy = max(mxy, tL.y0); }
+  Bbox b;
+  b.add(tF);
+  b.add(tL);
   int ox, oy;
-  stage_window<C>(map, sh, win, slot, phase, view, mnx, mxx, mny, mxy, ox, oy);
+  stage_window<C>(map, sh, win, slot, phase, view, b, ox, oy);
   slot ^= 1;
 #pragma unroll
   for (int k = 0; k < DCHT; ++k) {
@@ -244,18 +260,18 @@ __device__ __forceinline__ void process_chunk(const CUtensorMap* map, Shared& sh
       if (k == 0) t = tF;
       else if (k == n - 1) t = tL;
       else {
-        warp_coord_lean(vc.rx, vc.ry, vc.rz, vc.m, __ldg(depth_p + (size_t)(d0 + k) * HW), cc, ix, iy);
+        warp_coord_lean(vc.ray, vc.m, __ldg(depth_p + (size_t)(d0 + k) * HW), cc, ix, iy);
         t = split_coord(ix, iy, W, H);
         t.inb = t.inb && active;
       }
       float4 sA = make_float4(0.f, 0.f, 0.f, 0.f), sB = sA;
       const int lx = t.x0 - ox, ly = t.y0 - oy;
-      const bool inwin = t.inb && (unsigned)lx <= (unsigned)(K::WX - 2) && (unsigned)ly <= (unsigned)(K::WY - 2);
+      const bool inwin = in_window<C>(t.inb, lx, ly);
       gather_window<C>(L, inwin ? lx : 0, inwin ? ly : 0, t.fx, t.fy, sA, sB);
       if (!inwin) {
         sA = make_float4(0.f, 0.f, 0.f, 0.f); sB = sA;
         if (t.inb) {   // rare: sample through global memory (coordinates recomputed: they are not kept in registers)
-          warp_coord_lean(vc.rx, vc.ry, vc.rz, vc.m, __ldg(depth_p + (size_t)(d0 + k) * HW), cc, ix, iy);
+          warp_coord_lean(vc.ray, vc.m, __ldg(depth_p + (size_t)(d0 + k) * HW), cc, ix, iy);
           gather_global<C>(vc.srcA, vc.srcB, ix, iy, W, H, sA, sB);
         }
       }
@@ -270,7 +286,7 @@ __device__ __forceinline__ void process_chunk(const CUtensorMap* map, Shared& sh
 // DCHT: hypotheses per window (4 or 8).  GENERIC (pass A only): D > DCHT, similarities parked in a per-thread array.
 // ----------------------------------------------------------------------------------------------------------------------
 template <int C, int MODE, int DCHT, bool GENERIC>
-__global__ void __launch_bounds__(THREADS, (C == 8 && (MODE == 0 || (DCHT == 4 && MVSF_WT_PASSB_BLOCKS == 3))) ? 3 : 2)
+__global__ void __launch_bounds__(THREADS, C != 8 ? 2 : (MODE == 0 ? 3 : (DCHT == 4 ? kPassBBlocks8 : 2)))
 warp_tile_kernel(const __grid_constant__ CUtensorMap map, const float* __restrict__ feat, const float* __restrict__ homs,
                  const float* __restrict__ depth, const float* __restrict__ vis, float* __restrict__ out, int V, int D, int H,
                  int W, int dch) {
@@ -286,21 +302,8 @@ warp_tile_kernel(const __grid_constant__ CUtensorMap map, const float* __restric
   const bool active = (px < W) && (py < H);
   const int p = min(py, H - 1) * W + min(px, W - 1);
   const int sub = tid % K::LPX;           // which 8-channel slice of the pixel
-  Lane L;
-  int chA, chB;                            // first channel of the lane's quad A / quad B
-  if (C == 8) {
-    L.b0 = lane & 1; L.b1 = (lane >> 1) & 1; L.b2 = (lane >> 2) & 1;
-    L.base[0] = win + (L.b0 ? 16 : 0);
-    L.base[1] = win + (L.b0 ? 0 : 16);
-    chA = L.b0 ? 4 : 0; chB = L.b0 ? 0 : 4;
-  } else {
-    // lanes 2j, 2j+1 = the two channel halves of one pixel; bits 1-2 of the lane = tap slot inside an LDS.128 phase
-    L.b0 = false; L.b1 = (lane >> 1) & 1; L.b2 = (lane >> 2) & 1;
-    const int q0 = 2 * sub + (L.b1 ? 1 : 0), q1 = 2 * sub + (L.b1 ? 0 : 1);
-    L.base[0] = win + q0 * 16;
-    L.base[1] = win + q1 * 16;
-    chA = q0 * 4; chB = q1 * 4;
-  }
+  int chA, chB;
+  const Lane L = make_lane<C>(lane, sub, win, chA, chB);
   if (tid == 0) {
     mbar_init(smem_u32(&sh.bar), 1);
     fence_barrier_init();
@@ -319,9 +322,7 @@ warp_tile_kernel(const __grid_constant__ CUtensorMap map, const float* __restric
   auto make_view = [&](int v) {
     ViewCtx<C> vc;
     vc.m = load_hom(homs + (size_t)v * 12);
-    vc.rx = __fadd_rn(fmaf(vc.m.r01, fyp, __fmul_rn(vc.m.r00, fxp)), vc.m.r02);
-    vc.ry = __fadd_rn(fmaf(vc.m.r11, fyp, __fmul_rn(vc.m.r10, fxp)), vc.m.r12);
-    vc.rz = __fadd_rn(fmaf(vc.m.r21, fyp, __fmul_rn(vc.m.r20, fxp)), vc.m.r22);
+    vc.ray = ref_ray(vc.m, fxp, fyp);
     vc.srcA = feat + (size_t)(v + 1) * HW * C + chA;
     vc.srcB = feat + (size_t)(v + 1) * HW * C + chB;
     return vc;
@@ -407,7 +408,7 @@ warp_tile_kernel(const __grid_constant__ CUtensorMap map, const float* __restric
 }
 
 // ======================================================================================================================
-// Pass A of the SPILL plan for the fine stages, as a persistent producer / consumer pipeline (the cascade's default path):
+// Pass A of the SPILL plan for the finest stage (C = 8, D = 4), as a persistent producer / consumer pipeline:
 //   out: entropy[v][pixel]  and  corr[v][d][pixel][8]   (then vis CNN, then corr_aggregate streams corr).
 // One producer warp runs ahead of eight consumer warps through a ring of NBUF window buffers:
 //   producer, per (tile, view): wait empty[buf] -> predict the window origin from 32 sample pixels of the tile (first and last
@@ -431,11 +432,33 @@ struct PsShared {
   int origin[NBUF][2];
 };
 
+// the producer's sample pixel of this lane in a tile: 4 rows x 8 columns spread over the 8 x 32 tile
+template <int C>
+__device__ __forceinline__ int2 sample_pixel(int tile, int tiles_x, int lane, int W, int H) {
+  const int sr = (lane >> 3) * 2 + 1, sc = (lane & 7) * 4 + 1;
+  return make_int2(min((tile % tiles_x) * TW + sc, W - 1), min((tile / tiles_x) * PsCfg<C>::TROWS + sr, H - 1));
+}
+// Origin of the window the producer stages for one (tile, view): the bounding box of the sample pixels' taps at the first
+// and last hypothesis (the taps of a pixel lie between them on its epipolar line), reduced over the warp.
+template <int C>
+__device__ __forceinline__ int2 predict_window(const Hom& m, const float3& ray, float d_first, float d_last, const CoordConst& cc,
+                                               int W, int H) {
+  Bbox b;
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    float ix, iy;
+    warp_coord_lean(ray, m, e ? d_last : d_first, cc, ix, iy);
+    b.add(split_coord(ix, iy, W, H));
+  }
+  b.reduce_warp();
+  return window_origin<C>(b);
+}
+
 template <int C, int D, int NBUF>
-__global__ void __launch_bounds__(PsCfg<C>::THREADS, (C == 8) ? MVSF_PS_BLOCKS8 : 1)
+__global__ void __launch_bounds__(PsCfg<C>::THREADS, kPsBlocks)
 warp_stream_entropy_store_kernel(const __grid_constant__ CUtensorMap map, const float* __restrict__ feat,
                                  const float* __restrict__ homs, const float* __restrict__ depth, float* __restrict__ entropy,
-                                 float* __restrict__ corr, int V, int H, int W, int tiles_x, int ntiles, int dbg,
+                                 float* __restrict__ corr, int V, int H, int W, int tiles_x, int ntiles,
                                  const int* __restrict__ select) {
   using K = Cfg<C>;
   using P = PsCfg<C>;
@@ -455,50 +478,22 @@ warp_stream_entropy_store_kernel(const __grid_constant__ CUtensorMap map, const 
 
   if (warp == P::NCONS / 32) {
     // ------------------------------------------------------------------------------------------------ producer warp
-    // sample pixel of this lane inside a tile: 4 rows x 8 columns spread over the 8 x 32 tile
-    const int sr = (lane >> 3) * 2 + 1, sc = (lane & 7) * 4 + 1;
     int j = 0;
     for (int t = 0; t < my_tiles; ++t) {
-      const int tile = (int)blockIdx.x + t * (int)gridDim.x;
-      const int px = min((tile % tiles_x) * TW + sc, W - 1), py = min((tile / tiles_x) * P::TROWS + sr, H - 1);
-      const int p = py * W + px;
+      const int2 sp = sample_pixel<C>((int)blockIdx.x + t * (int)gridDim.x, tiles_x, lane, W, H);
+      const int p = sp.y * W + sp.x;
       const float d_first = __ldg(depth + p), d_last = __ldg(depth + (size_t)(D - 1) * HW + p);
-      const float fxp = (float)px, fyp = (float)py;
       for (int v = 0; v < V - 1; ++v, ++j) {
         const int buf = j % NBUF;
         const Hom m = load_hom(homs + (size_t)v * 12);
-        const float rx = __fadd_rn(fmaf(m.r01, fyp, __fmul_rn(m.r00, fxp)), m.r02);
-        const float ry = __fadd_rn(fmaf(m.r11, fyp, __fmul_rn(m.r10, fxp)), m.r12);
-        const float rz = __fadd_rn(fmaf(m.r21, fyp, __fmul_rn(m.r20, fxp)), m.r22);
-        int mnx = INT_MAX, mxx = INT_MIN, mny = INT_MAX, mxy = INT_MIN;
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float ix, iy;
-          warp_coord_lean(rx, ry, rz, m, e ? d_last : d_first, cc, ix, iy);
-          const TapCoord tc = split_coord(ix, iy, W, H);
-          if (tc.inb) { mnx = min(mnx, tc.x0); mxx = max(mxx, tc.x0); mny = min(mny, tc.y0); mxy = max(mxy, tc.y0); }
-        }
-        mnx = __reduce_min_sync(0xffffffffu, mnx);
-        mxx = __reduce_max_sync(0xffffffffu, mxx);
-        mny = __reduce_min_sync(0xffffffffu, mny);
-        mxy = __reduce_max_sync(0xffffffffu, mxy);
-        int ox = 0, oy = 0;
-        if (mnx <= mxx) {
-          const int slack_x = K::WX - (mxx + 2 - mnx), slack_y = K::WY - (mxy + 2 - mny);
-          ox = mnx - (slack_x > 0 ? slack_x / 2 : 0);
-          oy = (mny - (slack_y > 0 ? slack_y / 2 : 0)) & ~1;
-        }
+        const int2 o = predict_window<C>(m, ref_ray(m, (float)sp.x, (float)sp.y), d_first, d_last, cc, W, H);
         mbar_wait_warp(smem_u32(&sh.empty[buf]), (uint32_t)(((j / NBUF) & 1) ^ 1));   // consumers released this buffer
         if (lane == 0) {
-          sh.origin[buf][0] = ox;
-          sh.origin[buf][1] = oy;
+          sh.origin[buf][0] = o.x;
+          sh.origin[buf][1] = o.y;
           const uint32_t bar = smem_u32(&sh.full[buf]);
-          if (dbg & 1) {   // measurement only: no staging, the buffer is declared full at once
-            asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
-          } else {
-            expect_tx(bar, K::BYTES);
-            tma_load_5d(win0 + (uint32_t)buf * K::BYTES, &map, 0, 0, ox, oy >> 1, v + 1, bar);
-          }
+          expect_tx(bar, K::BYTES);
+          tma_load_5d(win0 + (uint32_t)buf * K::BYTES, &map, 0, 0, o.x, o.y >> 1, v + 1, bar);
         }
         __syncwarp();
       }
@@ -508,21 +503,8 @@ warp_stream_entropy_store_kernel(const __grid_constant__ CUtensorMap map, const 
 
   // -------------------------------------------------------------------------------------------------- consumer warps
   const int pix_in_cta = tid / K::LPX, sub = tid % K::LPX;
-  Lane L;
   int chA, chB;
-  uint32_t base0, base1;
-  if (C == 8) {
-    L.b0 = lane & 1; L.b1 = (lane >> 1) & 1; L.b2 = (lane >> 2) & 1;
-    base0 = (L.b0 ? 16 : 0);
-    base1 = (L.b0 ? 0 : 16);
-    chA = L.b0 ? 4 : 0; chB = L.b0 ? 0 : 4;
-  } else {
-    L.b0 = false; L.b1 = (lane >> 1) & 1; L.b2 = (lane >> 2) & 1;
-    const int q0 = 2 * sub + (L.b1 ? 1 : 0), q1 = 2 * sub + (L.b1 ? 0 : 1);
-    base0 = q0 * 16;
-    base1 = q1 * 16;
-    chA = q0 * 4; chB = q1 * 4;
-  }
+  const Lane L0 = make_lane<C>(lane, sub, 0u, chA, chB);   // piece offsets; the ring buffer's address is added per window
   constexpr float inv_cpg = 8.0f / (float)C;
   int j = 0;
   for (int t = 0; t < my_tiles; ++t) {
@@ -538,33 +520,30 @@ warp_stream_entropy_store_kernel(const __grid_constant__ CUtensorMap map, const 
     for (int v = 0; v < V - 1; ++v, ++j) {
       const int buf = j % NBUF;
       const Hom m = load_hom(homs + (size_t)v * 12);
-      const float rx = __fadd_rn(fmaf(m.r01, fyp, __fmul_rn(m.r00, fxp)), m.r02);
-      const float ry = __fadd_rn(fmaf(m.r11, fyp, __fmul_rn(m.r10, fxp)), m.r12);
-      const float rz = __fadd_rn(fmaf(m.r21, fyp, __fmul_rn(m.r20, fxp)), m.r22);
-      const float* __restrict__ srcA = feat + (size_t)(v + 1) * HW * C + chA;
-      const float* __restrict__ srcB = feat + (size_t)(v + 1) * HW * C + chB;
+      const float3 ray = ref_ray(m, fxp, fyp);
+      const float* __restrict__ src = feat + (size_t)(v + 1) * HW * C;
       mbar_wait_warp(smem_u32(&sh.full[buf]), (uint32_t)((j / NBUF) & 1));
       const int ox = sh.origin[buf][0], oy = sh.origin[buf][1];
-      L.base[0] = win0 + (uint32_t)buf * K::BYTES + base0;
-      L.base[1] = win0 + (uint32_t)buf * K::BYTES + base1;
+      const uint32_t wbuf = win0 + (uint32_t)buf * K::BYTES;
+      const Lane L = {L0.b0, L0.b1, L0.b2, {wbuf + L0.base[0], wbuf + L0.base[1]}};
       float sims[D];
       float mx = -FLT_MAX;
 #pragma unroll
       for (int k = 0; k < D; ++k) {
         float ix, iy;
-        warp_coord_lean(rx, ry, rz, m, dv[k], cc, ix, iy);
+        warp_coord_lean(ray, m, dv[k], cc, ix, iy);
         TapCoord tc = split_coord(ix, iy, W, H);
         tc.inb = tc.inb && active;
         float4 sA = make_float4(0.f, 0.f, 0.f, 0.f), sB = sA;
         const int lx = tc.x0 - ox, ly = tc.y0 - oy;
-        const bool inwin = tc.inb && (unsigned)lx <= (unsigned)(K::WX - 2) && (unsigned)ly <= (unsigned)(K::WY - 2);
-        if (!(dbg & 2)) gather_window<C>(L, inwin ? lx : 0, inwin ? ly : 0, tc.fx, tc.fy, sA, sB);
+        const bool inwin = in_window<C>(tc.inb, lx, ly);
+        gather_window<C>(L, inwin ? lx : 0, inwin ? ly : 0, tc.fx, tc.fy, sA, sB);
         if (!inwin) {
           sA = make_float4(0.f, 0.f, 0.f, 0.f); sB = sA;
-          if (tc.inb && !(dbg & 4)) gather_global<C>(srcA, srcB, ix, iy, W, H, sA, sB);
+          if (tc.inb) gather_global<C>(src + chA, src + chB, ix, iy, W, H, sA, sB);
         }
         // per-view group correlations exactly as the aggregation pass consumes them (cost_volume.py:78-85)
-        if (active && !(dbg & 8)) {
+        if (active) {
           float* cp = corr + (((size_t)v * D + k) * HW + p) * 8;
           if (C == 8) {
             *reinterpret_cast<float4*>(cp + chA) = make_float4(rA.x * sA.x, rA.y * sA.y, rA.z * sA.z, rA.w * sA.w);
@@ -609,49 +588,26 @@ template <int C, int D>
 __global__ void __launch_bounds__(1024)
 warp_stream_select_kernel(const float* __restrict__ homs, const float* __restrict__ depth, int V, int H, int W, int tiles_x,
                           int ntiles, int max_miss_permille, int* __restrict__ select) {
-  using K = Cfg<C>;
-  using P = PsCfg<C>;
   const int lane = threadIdx.x & 31, HW = H * W;
   const CoordConst cc = make_coord_const(W, H);
-  const int sr = (lane >> 3) * 2 + 1, sc = (lane & 7) * 4 + 1;   // the producer's sample pixels
-  const int tile = (int)(((long long)blockIdx.x * ntiles) / gridDim.x);
-  const int px = min((tile % tiles_x) * TW + sc, W - 1), py = min((tile / tiles_x) * P::TROWS + sr, H - 1);
-  const int p = py * W + px;
-  const float fxp = (float)px, fyp = (float)py;
+  const int2 sp = sample_pixel<C>((int)(((long long)blockIdx.x * ntiles) / gridDim.x), tiles_x, lane, W, H);
+  const int p = sp.y * W + sp.x;
   float dv[D];
 #pragma unroll
   for (int k = 0; k < D; ++k) dv[k] = __ldg(depth + (size_t)k * HW + p);
   unsigned int tot = 0u, miss = 0u;
   for (int v = threadIdx.x >> 5; v < V - 1; v += blockDim.x >> 5) {
     const Hom m = load_hom(homs + (size_t)v * 12);
-    const float rx = __fadd_rn(fmaf(m.r01, fyp, __fmul_rn(m.r00, fxp)), m.r02);
-    const float ry = __fadd_rn(fmaf(m.r11, fyp, __fmul_rn(m.r10, fxp)), m.r12);
-    const float rz = __fadd_rn(fmaf(m.r21, fyp, __fmul_rn(m.r20, fxp)), m.r22);
-    TapCoord tc[D];
-    int mnx = INT_MAX, mxx = INT_MIN, mny = INT_MAX, mxy = INT_MIN;
+    const float3 ray = ref_ray(m, (float)sp.x, (float)sp.y);
+    const int2 o = predict_window<C>(m, ray, dv[0], dv[D - 1], cc, W, H);
 #pragma unroll
     for (int k = 0; k < D; ++k) {
       float ix, iy;
-      warp_coord_lean(rx, ry, rz, m, dv[k], cc, ix, iy);
-      tc[k] = split_coord(ix, iy, W, H);
-      if ((k == 0 || k == D - 1) && tc[k].inb) { mnx = min(mnx, tc[k].x0); mxx = max(mxx, tc[k].x0); mny = min(mny, tc[k].y0); mxy = max(mxy, tc[k].y0); }
-    }
-    mnx = __reduce_min_sync(0xffffffffu, mnx);
-    mxx = __reduce_max_sync(0xffffffffu, mxx);
-    mny = __reduce_min_sync(0xffffffffu, mny);
-    mxy = __reduce_max_sync(0xffffffffu, mxy);
-    int ox = 0, oy = 0;
-    if (mnx <= mxx) {
-      const int slack_x = K::WX - (mxx + 2 - mnx), slack_y = K::WY - (mxy + 2 - mny);
-      ox = mnx - (slack_x > 0 ? slack_x / 2 : 0);
-      oy = (mny - (slack_y > 0 ? slack_y / 2 : 0)) & ~1;
-    }
-#pragma unroll
-    for (int k = 0; k < D; ++k) {
-      if (!tc[k].inb) continue;
+      warp_coord_lean(ray, m, dv[k], cc, ix, iy);
+      const TapCoord tc = split_coord(ix, iy, W, H);
+      if (!tc.inb) continue;
       ++tot;
-      const int lx = tc[k].x0 - ox, ly = tc[k].y0 - oy;
-      if (!((unsigned)lx <= (unsigned)(K::WX - 2) && (unsigned)ly <= (unsigned)(K::WY - 2))) ++miss;
+      if (!in_window<C>(true, tc.x0 - o.x, tc.y0 - o.y)) ++miss;
     }
   }
   tot = __reduce_add_sync(0xffffffffu, tot);
@@ -742,14 +698,12 @@ static int launch_stream_store(const float* feat, const float* homs, const float
   int rc = make_window_map<C>(&map, feat, V, H, W);
   if (rc) return rc;
   const int tiles_x = cdiv(W, TW), tiles_y = cdiv(H, PsCfg<C>::TROWS), ntiles = tiles_x * tiles_y;
-  const int per_sm = (C == 8) ? MVSF_PS_BLOCKS8 : 1;
-  const int cap = device_sm_count(dev) * per_sm;
-  static const int dbg = getenv("MVSF_WT_DEBUG") ? atoi(getenv("MVSF_WT_DEBUG")) : 0;   // measurement knobs (1: no staging, 2: no
+  const int cap = device_sm_count(dev) * kPsBlocks;
   if (select) {
     const int nsample = ntiles < 96 ? ntiles : 96, warps = V - 1 < 32 ? V - 1 : 32;
     warp_stream_select_kernel<C, D><<<nsample, 32 * warps, 0, s>>>(homs, depth, V, H, W, tiles_x, ntiles, max_miss_permille, select);
   }
-  kern<<<ntiles < cap ? ntiles : cap, PsCfg<C>::THREADS, smem, s>>>(map, feat, homs, depth, entropy, corr, V, H, W, tiles_x, ntiles, dbg, select);   // window gather, 4: no fallback, 8: no store)
+  kern<<<ntiles < cap ? ntiles : cap, PsCfg<C>::THREADS, smem, s>>>(map, feat, homs, depth, entropy, corr, V, H, W, tiles_x, ntiles, select);
   return MVSF_OK;
 }
 
@@ -774,16 +728,15 @@ int warp_tile_aggregate(const float* feat, const float* homs, const float* depth
                 : wt::dispatch<16>(1, feat, homs, depth, vis, volume, V, D, H, W, s);
 }
 
-// pass A of the spill plan (entropy + per-view group correlations) for the shapes the pipeline kernel is built for
+// pass A of the spill plan (entropy + per-view group correlations) for the shape the pipeline kernel is built for
 bool warp_stream_store_supported(const float* feat, const float* corr, int C, int G, int D, int H, int W) {
-  return warp_tile_supported(feat, C, G, D, H, W) && ((C == 8 && D == 4) || (C == 16 && D == 8)) && ((uintptr_t)corr & 15) == 0;
+  return warp_tile_supported(feat, C, G, D, H, W) && C == 8 && D == 4 && ((uintptr_t)corr & 15) == 0;
 }
 // select != nullptr: five device ints (decision, miss share, three zeroed scratch counters); a small kernel decides from the geometry of THIS call whether the pipeline kernel runs
 // (select[0] = 1) or leaves the call to the L1-gather kernel the caller launches next (select[0] = 0)
 int warp_stream_entropy_store(const float* feat, const float* homs, const float* depth, float* entropy, float* corr, int V,
-                              int C, int D, int H, int W, int* select, int max_miss_permille, cudaStream_t s) {
-  if (C == 8) return wt::launch_stream_store<8, 4, MVSF_PS_NBUF8>(feat, homs, depth, entropy, corr, V, H, W, select, max_miss_permille, s);
-  return wt::launch_stream_store<16, 8, 3>(feat, homs, depth, entropy, corr, V, H, W, select, max_miss_permille, s);
+                              int H, int W, int* select, int max_miss_permille, cudaStream_t s) {
+  return wt::launch_stream_store<8, 4, wt::kPsNbuf>(feat, homs, depth, entropy, corr, V, H, W, select, max_miss_permille, s);
 }
 
 }  // namespace mvsf
