@@ -1,10 +1,10 @@
 // Softmax attention of the stage-1 transformer regulariser (models/module.py:507-600 -> attention.py:141-170) on wgmma.
 // Included by costreg_tr.cu (uses its split_f16 / ex2f helpers).
 //
-// One CTA works on one 128-query tile of one head (head dim 16).
-//   warp 8        bulk-copy producer: K / V^T tiles (pre-tiled by qkv_tile_kernel into the canonical K-major layouts, 4 KB
-//                 and 10 KB) through two mbarrier rings of NKV stages
-//   warps 0-7     two warpgroups of 64 query rows each.  Per 128-key tile: S = Q_lo K_hi + Q_hi K_lo + Q_hi K_hi (three
+// One CTA works on NWG x 64 query rows of one head (head dim 16): 192 for the shipped fp16-P kernel, 128 for the hi + lo one.
+//   warpgroup NWG   bulk-copy producer (one thread): the CTA's Q blocks, then K / V^T tiles (pre-tiled by qkv_tile_kernel
+//                   into the canonical K-major layouts, 4 KB and 10 KB) through two mbarrier rings of NKV stages
+//   warpgroups 0..NWG-1   64 query rows each.  Per 128-key tile: S = Q_lo K_hi + Q_hi K_lo + Q_hi K_hi (three
 //                 m64n128k16 MMAs, fp32 scores in registers), online softmax (a row lives in the 4 threads of a quad), P
 //                 rounded to fp16 IN REGISTERS and used directly as the A operand of the P*V MMAs against
 //                 [V_lo | V_hi | 1 | 0] (N = 40): the ones row of V makes the tensor core produce the softmax normaliser of
@@ -12,22 +12,32 @@
 //                 the running output.
 // Schedule (after FlashAttention-3): each warpgroup issues the scores of tile j+1 and P*V of tile j back to back; the
 // softmax of tile j+1 runs once the scores are complete (wgmma.wait_group 1) while P*V of tile j is still in flight, and
-// tile j is folded into the output after it.  Measured on an H100 SXM at 700 W (N = 27 648): 1.51-1.55 ms per launch
-// against 1.72-1.73 ms for a loop that waits for each product before its softmax.  Variants measured slower on the same
-// kind of card and dropped: a named-barrier ping-pong that alternates the two warpgroups' MMA issue (+4 %), and
+// tile j is folded into the output after it.  Measured on an H100 SXM at 700 W (N = 27 648, two warpgroups): 1.51-1.55 ms
+// per launch against 1.72-1.73 ms for a loop that waits for each product before its softmax.  Variants measured slower on
+// the same kind of card and dropped: a named-barrier ping-pong that alternates the two warpgroups' MMA issue (+4 %), and
 // computing 1/8 or 1/4 of the exponentials with a polynomial on the FMA pipe as FlashAttention-4 does
 // (+3 % and +9 % on top of the ping-pong loop).
+// The exp unit (MUFU.EX2, 64 per row and key tile) bounds the loop.  While a warpgroup waits for its scores or reduces
+// its row maxima it feeds no exps, so three warpgroups (three softmax warps per SM sub-partition instead of two) keep the
+// unit busier; each row still sees the same products in the same order, so the results are bit-identical to two.  A
+// 416-thread CTA (three warpgroups + one producer warp) would cap every thread at 128 registers (four of its warps share
+// one sub-partition's 16 384), below the loop's ~150: the producer is a whole warpgroup that gives its registers away
+// (setmaxnreg 32 / 160).  On an H100 SXM at a 400 W limit: 1.63-1.73 ms per launch at N = 27 648 (two warpgroups
+// 1.83-1.92), 2.44-2.48 ms at N = 32 640 (2.59-2.64), though 192-row CTAs leave a coarser last wave (DTU 576 CTAs on 132
+// SMs: 5 waves, busiest SM 960 rows against 896 with 128-row CTAs).
 #pragma once
 
 namespace fa {
 using namespace gmma;
-constexpr int NCONS = 256, THREADS = NCONS + 32, NKV = 3;
+constexpr int NKV = 3;
 constexpr uint32_t TILE = 4096;                 // one canonical 128 x 16 (Q, K) fp16 tile
-constexpr uint32_t LBO_QK = 2048, LBO_V = 640;  // k-chunk strides: Q/K 128 rows; V^T 40 rows = V_lo dims | V_hi dims | ones row + 7 zero rows
+// k-chunk strides: K 128 rows; the Q block of one warpgroup 64 rows; V^T 40 rows = V_lo dims | V_hi dims | ones row + 7 zero rows
+constexpr uint32_t LBO_QK = 2048, LBO_Q = 1024, LBO_V = 640;
 constexpr uint32_t V_TILE = 16 * LBO_V;         // 10 KB
-// Q (hi, lo) | K ring (hi, lo) | V ring | barriers
-constexpr uint32_t OFF_Q = 0, OFF_K = 2 * TILE, OFF_V = OFF_K + NKV * 2 * TILE, OFF_BAR = OFF_V + NKV * V_TILE;
-constexpr uint32_t SMEM = OFF_BAR + 8 + 32 * NKV;
+// K ring (hi, lo) | V ring | per warpgroup: Q hi, Q lo (64 rows each, 4 KB together) | barriers
+constexpr uint32_t OFF_K = 0, OFF_V = OFF_K + NKV * 2 * TILE, OFF_Q = OFF_V + NKV * V_TILE;
+constexpr int threads(int nwg) { return 128 * (nwg + 1); }   // nwg consumer warpgroups + the producer warpgroup
+constexpr uint32_t smem_bytes(int nwg) { return OFF_Q + nwg * TILE + 8 + 32 * NKV; }
 }  // namespace fa
 
 // tiled layout: planes Qh, Ql, Kh, Kl of 4 heads x ntiles x 2048 halves (tile = [2 k-chunks][128 rows][8]) and one V plane
@@ -160,33 +170,44 @@ __device__ __forceinline__ void fold_tile(float (&o)[2][4], float (&l)[2], const
 //              traffic, no lo-split arithmetic in the softmax threads.  Measured against fp64 in tests/test_gpu_parity.py.
 // (Scores keep all three products Q_lo K_hi + Q_hi K_lo + Q_hi K_hi: a one-product variant has 20x the error, 5.2e-3 vs
 //  fp64, and a stage-2 cascade probability error of 1.5e-4.)
-template <bool PLO>
-__global__ void __launch_bounds__(fa::THREADS, 1)
+template <bool PLO, int NWG>
+__global__ void __launch_bounds__(fa::threads(NWG), 1)
 attention_fa_kernel(const __half* __restrict__ tiled, float* __restrict__ out, __half* __restrict__ out2, int N, int ntiles) {
   using namespace fa;
   extern __shared__ __align__(128) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int head = blockIdx.y, qt = blockIdx.x;
+  const int head = blockIdx.y;
   const size_t plane = (size_t)4 * ntiles * 2048;
   const __half* base = tiled + (size_t)head * ntiles * 2048;       // + plane index * plane + tile * 2048
   const uint32_t sb = smem_u32(smem);
-  const uint32_t bar_q = sb + OFF_BAR, bar_kf = bar_q + 8, bar_ke = bar_kf + 8 * NKV, bar_vf = bar_ke + 8 * NKV,
+  const uint32_t bar_q = sb + OFF_Q + NWG * TILE, bar_kf = bar_q + 8, bar_ke = bar_kf + 8 * NKV, bar_vf = bar_ke + 8 * NKV,
                  bar_ve = bar_vf + 8 * NKV;
   if (tid == 0) {
     mbar_init(bar_q, 1);
-    // a K / V stage is free once both warpgroups' products that read it are complete (K and V are released at different
+    // a K / V stage is free once every warpgroup's products that read it are complete (K and V are released at different
     // points of the loop, each by one thread per warpgroup)
-    for (int i = 0; i < NKV; ++i) { mbar_init(bar_kf + 8 * i, 1); mbar_init(bar_ke + 8 * i, 2); mbar_init(bar_vf + 8 * i, 1); mbar_init(bar_ve + 8 * i, 2); }
+    for (int i = 0; i < NKV; ++i) { mbar_init(bar_kf + 8 * i, 1); mbar_init(bar_ke + 8 * i, NWG); mbar_init(bar_vf + 8 * i, 1); mbar_init(bar_ve + 8 * i, NWG); }
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp == NCONS / 32) {
+  if (warp >= 4 * NWG) {
     // ------------------------------------------------------------------------------------------ producer
-    if (lane == 0) {
-      expect_tx(bar_q, 2 * TILE);
-      bulk_load(sb + OFF_Q, base + 0 * plane + (size_t)qt * 2048, TILE, bar_q);
-      bulk_load(sb + OFF_Q + TILE, base + 1 * plane + (size_t)qt * 2048, TILE, bar_q);
+    // 512 threads start with 128 registers each, fewer than the consumers' loop needs: the producer warpgroup hands
+    // its registers to them (32 + 3 x 160 = 512 per thread slot)
+    if constexpr (NWG == 3) asm volatile("setmaxnreg.dec.sync.aligned.u32 32;");
+    if (warp == 4 * NWG && lane == 0) {
+      // Q: 64-row block NWG * blockIdx.x + w of the 128-row tiles for warpgroup w, as four 1 KB copies (hi, lo x two
+      // k-chunks).  A block past the last tile has only rows >= N, which are computed and not stored: it reads the last
+      // block instead, so that no CTA reads past the Q planes.
+      expect_tx(bar_q, NWG * TILE);
+      for (int w = 0; w < NWG; ++w) {
+        const int b = min(NWG * (int)blockIdx.x + w, 2 * ntiles - 1);
+        for (int p = 0; p < 2; ++p)
+          for (int kc = 0; kc < 2; ++kc)
+            bulk_load(sb + OFF_Q + w * TILE + p * (TILE / 2) + kc * LBO_Q,
+                      base + p * plane + (size_t)(b >> 1) * 2048 + kc * 1024 + (b & 1) * 512, LBO_Q, bar_q);
+      }
       for (int t = 0; t < ntiles; ++t) {
         const int s = t % NKV;
         const uint32_t par = (uint32_t)(((t / NKV) & 1) ^ 1);
@@ -202,11 +223,12 @@ attention_fa_kernel(const __half* __restrict__ tiled, float* __restrict__ out, _
     return;
   }
   // -------------------------------------------------------------------------------------------- MMA + softmax warpgroups
-  // thread (warpgroup wg, warp wq of it, lane): query rows 64 wg + 16 wq + lane / 4 + 8 h (h = 0, 1); score columns
-  // 8 b + 2 (lane % 4) + e of accumulator register 4 b + 2 h + e
+  if constexpr (NWG == 3) asm volatile("setmaxnreg.inc.sync.aligned.u32 160;");
+  // thread (warpgroup wg, warp wq of it, lane): query rows 64 (NWG blockIdx.x + wg) + 16 wq + lane / 4 + 8 h (h = 0, 1);
+  // score columns 8 b + 2 (lane % 4) + e of accumulator register 4 b + 2 h + e
   const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
   const bool leader = (tid & 127) == 0;
-  const uint64_t q_hi = make_desc(sb + OFF_Q + wg * 1024, LBO_QK, 128), q_lo = make_desc(sb + OFF_Q + TILE + wg * 1024, LBO_QK, 128);
+  const uint64_t q_hi = make_desc(sb + OFF_Q + wg * TILE, LBO_Q, 128), q_lo = make_desc(sb + OFF_Q + wg * TILE + TILE / 2, LBO_Q, 128);
   float o[2][4];   // per row: head dims 2q, 2q + 1, 8 + 2q, 9 + 2q
   float m[2] = {-1e30f, -1e30f}, l[2] = {0.f, 0.f};
 #pragma unroll
@@ -262,7 +284,7 @@ attention_fa_kernel(const __half* __restrict__ tiled, float* __restrict__ out, _
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int r = qt * 128 + 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
+    const int r = 64 * (NWG * (int)blockIdx.x + wg) + 16 * wq + (lane >> 2) + 8 * h;
     if (r >= N) continue;
     const float inv = __fdiv_rn(1.0f, l[h]);
 #pragma unroll

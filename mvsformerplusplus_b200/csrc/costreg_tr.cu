@@ -138,6 +138,12 @@ __global__ void unpatch_ln_prob_kernel(const float* __restrict__ u, const float*
 // 0 (default): softmax probabilities as fp16 (P_hi only); 1: fp16 hi + lo (three partial P*V products, round-1 kernel)
 static int g_attention_plo = 0;
 
+// one CTA per NWG * 64 query rows of one head
+template <bool PLO, int NWG>
+static void launch_attention(const __half* tiled, float* o, __half* o2, int N, int ntiles, cudaStream_t s) {
+  attention_fa_kernel<PLO, NWG><<<dim3(cdiv(N, 64 * NWG), 4), fa::threads(NWG), fa::smem_bytes(NWG), s>>>(tiled, o, o2, N, ntiles);
+}
+
 static int run_attention(const float* qkv, float* o, __half* o2, __half* tiled, int N, float scale_log2e, cudaStream_t s) {
   const int ntiles = cdiv(N, 128);
   qkv_tile_kernel<<<cdiv((long long)ntiles * 128 * 24, 256), 256, 0, s>>>(qkv, tiled, N, ntiles, scale_log2e);
@@ -145,16 +151,17 @@ static int run_attention(const float* qkv, float* o, __half* o2, __half* tiled, 
   static DeviceOnce once;
   const int dev = current_device();
   if (once.need(dev)) {
-    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa::SMEM));
-    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa::SMEM));
+    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa::smem_bytes(2)));
+    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa::smem_bytes(3)));
     once.done(dev);
   }
   cudaEvent_t kt = ktimer_enabled() ? ktimer_begin("attention_tc", s) : nullptr;
-  const dim3 grid(ntiles, 4);
+  // three consumer warpgroups keep three softmax warps per SM sub-partition feeding the exp unit.  The hi + lo variant
+  // keeps two: it spills at 168 registers already, more than the 160 three warpgroups leave each thread.
   if (g_attention_plo)
-    attention_fa_kernel<true><<<grid, fa::THREADS, fa::SMEM, s>>>(tiled, o, o2, N, ntiles);
+    launch_attention<true, 2>(tiled, o, o2, N, ntiles, s);
   else
-    attention_fa_kernel<false><<<grid, fa::THREADS, fa::SMEM, s>>>(tiled, o, o2, N, ntiles);
+    launch_attention<false, 3>(tiled, o, o2, N, ntiles, s);
   if (kt) ktimer_end(kt, s);
   MVSF_LAUNCH_CHECK("attention_tc");
   return MVSF_OK;
