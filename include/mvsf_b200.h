@@ -242,6 +242,26 @@ int mvsf_vit_decoder_forward(const float* x0, const float* x1, const float* x2, 
                              float* out, void* workspace, size_t workspace_bytes, int B, int V, int h, int w,
                              mvsf_stream_t stream);
 
+/* ---- V2: models/dino/dinov2.py:249-266 DinoVisionTransformer.forward_interval_features, shipped config (ViT-B/14 built
+ *      by DINOv2_mvsformer_model.py:40-41: embed 768, 12 blocks of 12 heads x 64 softmax attention (attention.py:77-101,
+ *      scale 1/8), mlp 3072 exact-erf GELU, LayerScale, LayerNorm eps 1e-6, cross_interval_layers 3).
+ * img [n][3][14 gh][14 gw] fp32 (contiguous); pos [gh gw + 1][768] = interpolate_pos_encoding(pos_embed) for the grid
+ * (dinov2.py:176-200, computed once per grid at pack time).  Outputs, cls token dropped: out0 = block 3, out1 = block 7,
+ * out2 = norm(block 11), each [n][gh gw][768] in its first n gh gw rows; out0 and out1 also hold the residual stream and
+ * need n (gh gw + 1) rows (the n cls rows come after the patch rows), out2 needs n gh gw rows.
+ * wts: the small fp32 parameters (tail of packing.pack_vit, layout in csrc/vit.cu, 141 312 floats); wts_tc =
+ * mvsf_vit_pack_tc(GEMM prefix of packing.pack_vit: 85 426 176 floats).  Bad shapes (n outside [1, 65535], gh or gw
+ * outside [1, 1024], n (gh gw + 1) > 2^21), null or misaligned pointers: -1; short workspace: -3; nothing launched. */
+int mvsf_vit_workspace_bytes(int n, int gh, int gw, size_t* bytes);
+int mvsf_vit_tc_bytes(size_t* bytes);
+int mvsf_vit_pack_tc(const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
+int mvsf_vit_forward(const float* img, const float* pos, const float* wts, const void* wts_tc, float* out0, float* out1,
+                     float* out2, void* workspace, size_t workspace_bytes, int n, int gh, int gw, mvsf_stream_t stream);
+/* The ViT's softmax attention alone: qkv [n][N][2304] fp32 (row stride ldq, [q | k | v] x 12 heads x 64) -> out
+ * [n][N][768] (row stride ldo).  workspace >= n * 12 * ceil(N / 128) * 100 352 bytes. */
+int mvsf_vit_attention_forward(const float* qkv, int ldq, float* out, int ldo, void* workspace, size_t workspace_bytes,
+                               int n, int N, mvsf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

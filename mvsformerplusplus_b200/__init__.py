@@ -3,13 +3,14 @@ cost regularisation -> soft-argmax, 4-stage cascade) behind the reference's Pyth
 from .config import default_args, load_args, validate_args  # noqa: F401
 
 __all__ = ["default_args", "load_args", "validate_args", "StageNet", "FMT_with_pathway", "HotPathNet", "install",
-           "cascade_forward", "homo_warping_3D_with_mask", "FPNEncoder", "FPNDecoder", "CrossVITDecoder"]
+           "cascade_forward", "homo_warping_3D_with_mask", "FPNEncoder", "FPNDecoder", "CrossVITDecoder",
+           "DinoVisionTransformer", "vit_base"]
 
 
 def __getattr__(name):  # hotpath imports torch + ctypes; keep `import mvsformerplusplus_b200` light
     if name in ("StageNet", "FMT_with_pathway", "HotPathNet", "install", "cascade_forward", "to_nhwc", "to_nchw",
                 "homo_warping_3D_with_mask", "FPNEncoder", "FPNDecoder",
-                "CrossVITDecoder"):
+                "CrossVITDecoder", "DinoVisionTransformer", "vit_base"):
         from . import hotpath
         return getattr(hotpath, name)
     raise AttributeError(name)

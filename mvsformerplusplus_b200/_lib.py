@@ -59,6 +59,11 @@ SIGNATURES = {
     "mvsf_vit_decoder_tc_bytes": ([ctypes.POINTER(Z)], I),
     "mvsf_vit_decoder_pack_tc": ([P, P, Z, P], I),
     "mvsf_vit_decoder_forward": ([P] * 7 + [Z, I, I, I, I, P], I),
+    "mvsf_vit_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
+    "mvsf_vit_tc_bytes": ([ctypes.POINTER(Z)], I),
+    "mvsf_vit_pack_tc": ([P, P, Z, P], I),
+    "mvsf_vit_forward": ([P] * 8 + [Z, I, I, I, P], I),
+    "mvsf_vit_attention_forward": ([P, I, P, I, P, Z, I, I, P], I),
 }
 
 

@@ -93,11 +93,7 @@ __device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
   hi = __float2half_rn(x);
   lo = __float2half_rn(x - __half2float(hi));
 }
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
+using gmma::ex2f;
 
 #include "attention_fa.cuh"   // attention kernel (inside namespace mvsf)
 

@@ -36,6 +36,15 @@ struct TcsArgs : TcLinArgs {
   int sy, sx, py, px;
 };
 void tcs_token_rows(TcsArgs& a);   // one tap (0, 0) on a 1 x 1 grid: plain rows of A, stored in place
+// token linear of M rows: A rows [hi(K) | lo(K)] of stride lda, weights [N][K] at Bh / Bl (rows of stride K)
+inline TcsArgs tcs_rows(const __half* A, int lda, int K, const __half* Bh, const __half* Bl, int N, int M) {
+  TcsArgs a{};
+  a.Ah = A; a.Al = A + K; a.lda = lda;
+  a.Bh = Bh; a.Bl = Bl; a.ldb = K;
+  a.M = M; a.N = N; a.K = K;
+  tcs_token_rows(a);
+  return a;
+}
 int launch_linear_tcs(const TcsArgs& a, int epi, cudaStream_t s);
 // out row m = [hi(0..K) | lo(0..K)] (ldo >= 2K)
 int launch_split_f16(const float* x, int ldx, __half* out, int ldo, int M, int K, cudaStream_t s);

@@ -64,12 +64,7 @@ struct Ws {
 };
 
 static TcsArgs gemm(const Ws& ws, const __half* A, int lda, int K, size_t woff, int N, int M) {
-  TcsArgs a{};
-  a.Ah = A; a.Al = A + K; a.lda = lda;
-  a.Bh = ws.wh + woff; a.Bl = ws.wl + woff; a.ldb = K;
-  a.M = M; a.N = N; a.K = K;
-  tcs_token_rows(a);
-  return a;
+  return tcs_rows(A, lda, K, ws.wh + woff, ws.wl + woff, N, M);
 }
 
 // K / V summary of a cross layer from the raw reference tokens r [L][D] (pre_norm_query: no norm1)

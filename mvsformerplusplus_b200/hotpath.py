@@ -9,6 +9,8 @@ enqueue libmvsf_b200 kernels.  PyTorch is used for device memory, streams and mo
   install(model, feature_pyramid=True)  also rebinds model.encoder / model.decoder
   CrossVITDecoder.forward(x, Fmats=None, vit_shape=None)                          <- models/module.py:273-364
   install(model, vit_decoder=True)  also rebinds model.decoder_vit
+  DinoVisionTransformer.forward_interval_features(x, masks=None)                  <- models/dino/dinov2.py:249-266
+  install(model, vit=True)  also rebinds model.vit (vit_base(...), DINOv2_mvsformer_model.py:40-41)
 
 Tensors crossing the seams keep the reference's logical shapes ([B,V,C,H,W] features, [B,D,H,W] volumes).  Feature
 maps produced by FMT_with_pathway are channels-last in memory (a permuted view), which StageNet consumes
@@ -22,7 +24,7 @@ import torch.nn as nn
 
 from . import _lib, packing
 from .config import load_args, stage_list, validate_args
-from .params import build_fmt, build_fpn_decoder, build_fpn_encoder, build_stage, build_vit_decoder
+from .params import build_fmt, build_fpn_decoder, build_fpn_encoder, build_stage, build_vit, build_vit_decoder
 
 
 def _ptr(t):
@@ -630,12 +632,121 @@ class CrossVITDecoder(_PackedMixin, nn.Module):
 
 
 # =====================================================================================================
-def install(model, args=None, feature_pyramid=False, vit_decoder=False):
+def _check_vit_config(img_size, patch_size, in_chans, embed_dim, depth, num_heads, mlp_ratio, qkv_bias, ffn_bias,
+                      proj_bias, init_values, act_layer, ffn_layer, block_chunks, kwargs):
+    shipped = dict(img_size=(img_size, 518), patch_size=(patch_size, 14), in_chans=(in_chans, 3),
+                   embed_dim=(embed_dim, 768), depth=(depth, 12), num_heads=(num_heads, 12), mlp_ratio=(mlp_ratio, 4),
+                   qkv_bias=(qkv_bias, True), ffn_bias=(ffn_bias, True), proj_bias=(proj_bias, True),
+                   act_layer=(act_layer, nn.GELU), ffn_layer=(ffn_layer, "mlp"), block_chunks=(block_chunks, 0),
+                   cross_interval_layers=(kwargs.get("cross_interval_layers"), 3),
+                   softmax_scale=(kwargs.get("softmax_scale"), None), dino_layer_idxs=(kwargs.get("dino_layer_idxs"), None))
+    for k, (got, want) in shipped.items():
+        if got != want:
+            raise NotImplementedError(f"DinoVisionTransformer: only the shipped ViT-B/14 is implemented ({k} = {want!r}), "
+                                      f"got {k} = {got!r}")
+    if not init_values:
+        raise NotImplementedError(f"DinoVisionTransformer: init_values must be set (LayerScale), got {init_values!r}")
+
+
+class DinoVisionTransformer(_PackedMixin, nn.Module):
+    """Drop-in for the reference DinoVisionTransformer (models/dino/dinov2.py:43-266) as DINOv2_mvsformer_model.py:40-41
+    builds it (vit_base, img_size 518, patch 14, LayerScale, block_chunks 0, mlp ffn, cross_interval_layers 3), eval mode:
+    same parameter names (load_state_dict(strict=True) of the reference's vit.* keys), embed_dim, patch_size and
+    forward_interval_features(x, masks=None).  x [n,3,14 gh,14 gw] in any float dtype and strides; returns the outputs of
+    blocks 3 and 7 and norm(x) after block 11 without the cls token, each fp32 [n, gh gw, 768], contiguous.
+    use_flash2_dino selects the same math in the reference and is accepted either way."""
+
+    def __init__(self, img_size=224, patch_size=16, in_chans=3, embed_dim=768, depth=12, num_heads=12, mlp_ratio=4.0,
+                 qkv_bias=True, ffn_bias=True, proj_bias=True, drop_path_rate=0.0, drop_path_uniform=False,
+                 init_values=None, act_layer=nn.GELU, ffn_layer="mlp", block_chunks=1, **kwargs):
+        super().__init__()
+        _check_vit_config(img_size, patch_size, in_chans, embed_dim, depth, num_heads, mlp_ratio, qkv_bias, ffn_bias,
+                          proj_bias, init_values, act_layer, ffn_layer, block_chunks, kwargs)
+        self.num_features = self.embed_dim = embed_dim
+        self.num_tokens = 1
+        self.n_blocks = depth
+        self.num_heads = num_heads
+        self.patch_size = patch_size
+        self.cross_interval_layers = kwargs["cross_interval_layers"]
+        self.dino_layer_idxs = None
+        build_vit(self, init_values=float(init_values))
+        for prm in self.parameters():   # frozen, as in the reference (dinov2.py:164-165)
+            prm.requires_grad = False
+        self._init_packing()
+
+    def _pack(self, device):
+        if self._packed is None or self._packed["device"] != device:
+            L = _lib.lib()
+            blob = packing.pack_vit(self.state_dict()).to(device)
+            need = ctypes.c_size_t(0)
+            _lib.check(L.mvsf_vit_tc_bytes(ctypes.byref(need)), "vit_tc_bytes")
+            tc = torch.empty(need.value // 2, device=device, dtype=torch.float16)
+            _lib.check(L.mvsf_vit_pack_tc(_ptr(blob), _ptr(tc), ctypes.c_size_t(need.value), _stream()), "vit_pack_tc")
+            # keep the fp16 hi / lo GEMM weights and the small fp32 parameters, not the fp32 GEMM weights
+            w = blob[packing.VIT_GEMM_WTS:].clone()
+            del blob
+            self._packed = {"device": device, "w": w, "tc": tc, "pos": {}}
+        return self._packed
+
+    def _pos(self, pk, gh, gw):
+        """interpolated pos_embed of the grid (a weight transform), cached with the packed weights"""
+        if (gh, gw) not in pk["pos"]:
+            pk["pos"][(gh, gw)] = packing.vit_pos_embed(self.pos_embed, gh, gw).to(pk["device"])
+        return pk["pos"][(gh, gw)]
+
+    @torch.no_grad()
+    def forward_interval_features(self, x, masks=None):
+        if isinstance(x, list):
+            raise NotImplementedError("DinoVisionTransformer: list inputs (forward_features_list) are not implemented")
+        if masks is not None:
+            raise NotImplementedError("DinoVisionTransformer: masks are not implemented")
+        if self.training:
+            raise NotImplementedError("the ViT implements the eval-mode forward; call .eval()")
+        n, c, H, W = x.shape
+        ps = self.patch_size
+        assert H % ps == 0, f"Input image height {H} is not a multiple of patch height {ps}"
+        assert W % ps == 0, f"Input image width {W} is not a multiple of patch width: {ps}"
+        if c != 3:
+            raise AssertionError(f"DinoVisionTransformer expects [n,3,H,W] images, got {tuple(x.shape)}")
+        _require_cuda(x, "DinoVisionTransformer.forward_interval_features(x)")
+        gh, gw = H // ps, W // ps
+        L = _lib.lib()
+        x = _f32c(x)
+        if x.data_ptr() % 16:
+            x = x.clone()
+        pk = self._pack(x.device)
+        pos = self._pos(pk, gh, gw)
+        f32 = dict(device=x.device, dtype=torch.float32)
+        P = gh * gw
+        # out0 / out1 also carry the residual stream: the n cls rows follow the n * P patch rows
+        outs = [torch.empty((n * (P + 1), 768), **f32), torch.empty((n * (P + 1), 768), **f32),
+                torch.empty((n * P, 768), **f32)]
+        need = ctypes.c_size_t(0)
+        _lib.check(L.mvsf_vit_workspace_bytes(n, gh, gw, ctypes.byref(need)), "vit_workspace_bytes")
+        ws = torch.empty(need.value // 4 + 4, **f32)
+        _lib.check(L.mvsf_vit_forward(_ptr(x), _ptr(pos), _ptr(pk["w"]), _ptr(pk["tc"]), *[_ptr(o) for o in outs],
+                                      _ptr(ws), ctypes.c_size_t(ws.numel() * 4), n, gh, gw, _stream()), "vit_forward")
+        return [o[:n * P].view(n, P, 768) for o in outs]
+
+
+def vit_base(patch_size=16, **kwargs):
+    """models/dino/dinov2.py:388-398: the ViT-B DinoVisionTransformer (embed 768, depth 12, 12 heads, mlp_ratio 4)."""
+    return DinoVisionTransformer(patch_size=patch_size, embed_dim=768, depth=12, num_heads=12, mlp_ratio=4, **kwargs)
+
+
+# =====================================================================================================
+def install(model, args=None, feature_pyramid=False, vit_decoder=False, vit=False):
     """Rebinds the hot-path seams of a reference-constructed DINOv2MVSNet (models/networks/DINOv2_mvsformer_model.py)
     to the CUDA path: model.FMT_module and model.fusions[i] are replaced by this package's modules carrying the
     same weights (state_dict round trip, strict).  With feature_pyramid=True model.encoder and model.decoder (the FPN,
-    DINOv2_mvsformer_model.py:34-35,87-89) are replaced as well, and with vit_decoder=True model.decoder_vit
-    (CrossVITDecoder, DINOv2_mvsformer_model.py:43,64).  The ViT itself stays untouched.  Returns model."""
+    DINOv2_mvsformer_model.py:34-35,87-89) are replaced as well, with vit_decoder=True model.decoder_vit
+    (CrossVITDecoder, DINOv2_mvsformer_model.py:43,64), and with vit=True model.vit (the DINOv2 ViT-B backbone,
+    DINOv2_mvsformer_model.py:40-41,55-59).  The bicubic image resize in front of the ViT stays PyTorch.  Returns model."""
+    if vit:
+        dino_cfg = (getattr(model, "vit_args", model.args) if args is None else load_args(args)).get("dino_cfg", {})
+        v = vit_base(img_size=518, patch_size=14, init_values=1.0, block_chunks=0, ffn_layer="mlp", **dino_cfg)
+        v.load_state_dict(model.vit.state_dict(), strict=True)
+        model.vit = v.to(next(model.vit.parameters()).device).eval()
     if vit_decoder:
         dec = CrossVITDecoder(getattr(model, "vit_args", model.args) if args is None else load_args(args))
         dec.load_state_dict(model.decoder_vit.state_dict(), strict=True)

@@ -183,3 +183,51 @@ def pack_vit_decoder(sd, p=""):
     out = _cat(g + small + biases, pad_to=8)
     assert out.numel() == VIT_DECODER_WTS, out.numel()
     return out
+
+
+VIT_GEMM_WTS = 85426176   # floats of the GEMM prefix of pack_vit (csrc/vit.cu NG)
+VIT_SMALL_WTS = 141312    # floats of its small-parameter tail (csrc/vit.cu NS)
+
+
+def pack_vit(sd, p=""):
+    """models/dino/dinov2.py (ViT-B/14) -> the fp32 blob of mvsf_vit_forward (layout in csrc/vit.cu): the GEMM prefix
+    patch_embed.proj [768][640] (k = c * 196 + ky * 14 + kx, zero from 588), then per block qkv [2304][768], proj, fc1,
+    fc2 as [N][K] rows; then the small parameters, per block norm1 w, b, qkv bias, proj bias, ls1, norm2 w, b, fc1 bias,
+    fc2 bias, ls2, and patch bias, cls token, norm w, b.  The two parts are split at VIT_GEMM_WTS."""
+    pw = _d(sd[p + "patch_embed.proj.weight"]).reshape(768, 588)
+    g = [torch.cat([pw, torch.zeros(768, 640 - 588, dtype=torch.float64)], 1)]
+    small = []
+    for i in range(12):
+        q = f"{p}blocks.{i}."
+        g += [_d(sd[q + k]) for k in ("attn.qkv.weight", "attn.proj.weight", "mlp.fc1.weight", "mlp.fc2.weight")]
+        small += [_d(sd[q + k]) for k in ("norm1.weight", "norm1.bias", "attn.qkv.bias", "attn.proj.bias", "ls1.gamma",
+                                          "norm2.weight", "norm2.bias", "mlp.fc1.bias", "mlp.fc2.bias", "ls2.gamma")]
+    small += [_d(sd[p + "patch_embed.proj.bias"]), _d(sd[p + "cls_token"]), _d(sd[p + "norm.weight"]),
+              _d(sd[p + "norm.bias"])]
+    out = _cat(g + small, pad_to=8)
+    assert out.numel() == VIT_GEMM_WTS + VIT_SMALL_WTS, out.numel()
+    return out
+
+
+def vit_pos_embed(pos_embed, gh, gw):
+    """DinoVisionTransformer.interpolate_pos_encoding (dinov2.py:176-200) for a gh x gw patch grid (image 14 gh x 14 gw),
+    with the reference's own F.interpolate call on the fp32 parameter, so the result is bit-identical on the same device:
+    pos_embed [1, 1370, 768] -> fp32 [gh * gw + 1, 768] (row 0 = cls).  Unchanged when the grid is the 37 x 37 one the
+    parameter was trained at (npatch == 1369 and image H == W); otherwise bicubic with scale_factor
+    ((gh + 0.1) / 37, (gw + 0.1) / 37) - not the size ratio, which gives different values."""
+    import math
+    import torch.nn.functional as F
+    pos = pos_embed.detach()
+    npatch, N = gh * gw, pos.shape[1] - 1
+    if npatch == N and gh == gw:
+        return pos.float().reshape(N + 1, -1).contiguous()
+    pos = pos.float()
+    dim = pos.shape[-1]
+    s = int(math.sqrt(N))
+    w0, h0 = gh + 0.1, gw + 0.1   # the reference calls the image height w and the width h
+    with torch.autocast(pos.device.type, enabled=False):
+        patch = F.interpolate(pos[:, 1:].reshape(1, s, s, dim).permute(0, 3, 1, 2),
+                              scale_factor=(w0 / math.sqrt(N), h0 / math.sqrt(N)), mode="bicubic")
+    assert patch.shape[-2:] == (gh, gw), patch.shape
+    patch = patch.permute(0, 2, 3, 1).reshape(-1, dim)
+    return torch.cat([pos[0, :1], patch], 0).contiguous()

@@ -203,6 +203,40 @@ def build_vit_decoder(m, init_values=1.0, prev_values=0.5):
     return m
 
 
+VIT_DEPTH, VIT_DIM, VIT_PATCH, VIT_GRID = 12, 768, 14, 37   # ViT-B/14 at img_size 518: a 37 x 37 pos_embed grid
+
+
+def build_vit(m, init_values=1.0):
+    """models/dino/dinov2.py:43-165 at the shipped vit_base(img_size=518, patch_size=14, block_chunks=0, ffn_layer="mlp"):
+    cls_token, pos_embed [1, 1370, 768], mask_token, patch_embed.proj (14 x 14 conv), blocks.{0..11} (norm1, attn.qkv
+    with bias, attn.proj, ls1.gamma, norm2, mlp.fc1 / fc2, ls2.gamma; LayerNorm eps 1e-6) and norm."""
+    d = VIT_DIM
+    m.cls_token = nn.Parameter(torch.zeros(1, 1, d))
+    m.pos_embed = nn.Parameter(torch.zeros(1, VIT_GRID * VIT_GRID + 1, d))
+    m.patch_embed = Bag()
+    m.patch_embed.proj = nn.Conv2d(3, d, VIT_PATCH, stride=VIT_PATCH)
+    blocks = []
+    for _ in range(VIT_DEPTH):
+        b = Bag()
+        b.norm1 = nn.LayerNorm(d, eps=1e-6)
+        b.attn = Bag()
+        b.attn.qkv = nn.Linear(d, 3 * d)
+        b.attn.proj = nn.Linear(d, d)
+        b.ls1 = Bag()
+        b.ls1.gamma = nn.Parameter(init_values * torch.ones(d))
+        b.norm2 = nn.LayerNorm(d, eps=1e-6)
+        b.mlp = Bag()
+        b.mlp.fc1 = nn.Linear(d, 4 * d)
+        b.mlp.fc2 = nn.Linear(4 * d, d)
+        b.ls2 = Bag()
+        b.ls2.gamma = nn.Parameter(init_values * torch.ones(d))
+        blocks.append(b)
+    m.blocks = nn.ModuleList(blocks)
+    m.norm = nn.LayerNorm(d, eps=1e-6)
+    m.mask_token = nn.Parameter(torch.zeros(1, d))
+    return m
+
+
 def build_hotpath_params(args):
     root = Bag()
     root.FMT_module = build_fmt(args["FMT_config"])
