@@ -216,6 +216,13 @@ int mvsf_fmt_forward(const float* f1, const float* f2, const float* f3, const fl
 int mvsf_fpn_encoder_workspace_bytes(int N, int H, int W, size_t* bytes);
 int mvsf_fpn_encoder_forward(const float* x, const float* wts, const void* wts_tc, float* c01, float* c11, float* c21,
                              float* c31, void* workspace, size_t workspace_bytes, int N, int H, int W, mvsf_stream_t stream);
+/* The encoder as DINOv2MVSNet.forward uses it (DINOv2_mvsformer_model.py:85-88): c31 receives LeakyReLU(conv31) +
+ * vit_feat[n % V] (one fp32 add in the last layer's epilogue), vit_feat [V][H/8][W/8][64] (NHWC, what
+ * mvsf_vit_decoder_forward writes for one batch item).  Image n = b V + v thus gets view v of batch item 0's ViT
+ * features, as the reference's eval forward adds vit_feat[vi] for every batch item. */
+int mvsf_fpn_encoder_vit_forward(const float* x, const float* vit_feat, int V, const float* wts, const void* wts_tc,
+                                 float* c01, float* c11, float* c21, float* c31, void* workspace, size_t workspace_bytes,
+                                 int N, int H, int W, mvsf_stream_t stream);
 /* ---- P2: models/module.py:242-270 FPNDecoder.forward (F.interpolate bilinear, align_corners=True; BN folded).
  * c01..c31 as the encoder writes them (NHWC, full-resolution H x W) -> o0 [N][64][H/8][W/8], o1 [N][32][H/4][W/4],
  * o2 [N][16][H/2][W/2], o3 [N][8][H][W] (NCHW: the layout mvsf_fmt_forward reads, DINOv2_mvsformer_model.py:95-98).
@@ -257,6 +264,12 @@ int mvsf_vit_tc_bytes(size_t* bytes);
 int mvsf_vit_pack_tc(const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
 int mvsf_vit_forward(const float* img, const float* pos, const float* wts, const void* wts_tc, float* out0, float* out1,
                      float* out2, void* workspace, size_t workspace_bytes, int n, int gh, int gw, mvsf_stream_t stream);
+/* The same forward on images of any size: img [n][3][H][W] fp32 (contiguous) is resized to 14 gh x 14 gw as
+ * F.interpolate(mode="bicubic", align_corners=False) does (DINOv2_mvsformer_model.py:76-77) inside the patch im2col; the
+ * resized image is never stored.  H, W >= 1 and H W < 2^30. */
+int mvsf_vit_forward_image(const float* img, int H, int W, const float* pos, const float* wts, const void* wts_tc,
+                           float* out0, float* out1, float* out2, void* workspace, size_t workspace_bytes, int n, int gh,
+                           int gw, mvsf_stream_t stream);
 /* The ViT's softmax attention alone: qkv [n][N][2304] fp32 (row stride ldq, [q | k | v] x 12 heads x 64) -> out
  * [n][N][768] (row stride ldo).  workspace >= n * 12 * ceil(N / 128) * 100 352 bytes. */
 int mvsf_vit_attention_forward(const float* qkv, int ldq, float* out, int ldo, void* workspace, size_t workspace_bytes,

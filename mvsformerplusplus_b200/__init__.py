@@ -4,13 +4,13 @@ from .config import default_args, load_args, validate_args  # noqa: F401
 
 __all__ = ["default_args", "load_args", "validate_args", "StageNet", "FMT_with_pathway", "HotPathNet", "install",
            "cascade_forward", "homo_warping_3D_with_mask", "FPNEncoder", "FPNDecoder", "CrossVITDecoder",
-           "DinoVisionTransformer", "vit_base"]
+           "DinoVisionTransformer", "vit_base", "DINOv2MVSNet"]
 
 
 def __getattr__(name):  # hotpath imports torch + ctypes; keep `import mvsformerplusplus_b200` light
     if name in ("StageNet", "FMT_with_pathway", "HotPathNet", "install", "cascade_forward", "to_nhwc", "to_nchw",
                 "homo_warping_3D_with_mask", "FPNEncoder", "FPNDecoder",
-                "CrossVITDecoder", "DinoVisionTransformer", "vit_base"):
+                "CrossVITDecoder", "DinoVisionTransformer", "vit_base", "DINOv2MVSNet"):
         from . import hotpath
         return getattr(hotpath, name)
     raise AttributeError(name)

@@ -50,6 +50,7 @@ SIGNATURES = {
     "mvsf_fmt_forward": ([P] * 7 + [Z] + [P] * 5 + [Z, I, I, I, P], I),
     "mvsf_fpn_encoder_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
     "mvsf_fpn_encoder_forward": ([P] * 8 + [Z, I, I, I, P], I),
+    "mvsf_fpn_encoder_vit_forward": ([P, P, I] + [P] * 7 + [Z, I, I, I, P], I),
     "mvsf_fpn_decoder_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
     "mvsf_fpn_decoder_forward": ([P] * 11 + [Z, I, I, I, P], I),
     "mvsf_fpn_tc_bytes": ([I, ctypes.POINTER(Z)], I),
@@ -63,6 +64,7 @@ SIGNATURES = {
     "mvsf_vit_tc_bytes": ([ctypes.POINTER(Z)], I),
     "mvsf_vit_pack_tc": ([P, P, Z, P], I),
     "mvsf_vit_forward": ([P] * 8 + [Z, I, I, I, P], I),
+    "mvsf_vit_forward_image": ([P, I, I] + [P] * 7 + [Z, I, I, I, P], I),
     "mvsf_vit_attention_forward": ([P, I, P, I, P, Z, I, I, P], I),
 }
 

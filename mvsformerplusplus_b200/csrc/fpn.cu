@@ -164,6 +164,20 @@ struct NhwcLeaky {   // encoder: LeakyReLU(0.1), [N][OH][OW][CO]
     *reinterpret_cast<float2*>(out + (((size_t)n * OH + y) * OW + x) * CO + ch) = make_float2(a, b);
   }
 };
+template <int CO>
+struct NhwcLeakyAddVit {   // last encoder layer of the model: LeakyReLU(0.1), then + vit[n % V] (conv31 + vit_feat)
+  float* out;
+  const float* vit;   // [V][OH][OW][CO]
+  int V;
+  static constexpr bool BIAS = true;
+  __device__ void store(int n, int OH, int OW, int y, int x, int ch, float a, float b) const {
+    a = a > 0.f ? a : __fmul_rn(0.1f, a);   // rounded on its own, as the reference's two separate ops round it
+    b = b > 0.f ? b : __fmul_rn(0.1f, b);
+    const float2 v = *reinterpret_cast<const float2*>(vit + (((size_t)(n % V) * OH + y) * OW + x) * CO + ch);
+    *reinterpret_cast<float2*>(out + (((size_t)n * OH + y) * OW + x) * CO + ch) = make_float2(__fadd_rn(a, v.x),
+                                                                                              __fadd_rn(b, v.y));
+  }
+};
 __device__ __forceinline__ float swish(float v) { return v / (1.0f + expf(-v)); }
 template <int CO>
 struct NchwSwish {   // decoder: Swish, [N][CO][OH][OW]
@@ -245,6 +259,16 @@ static int dec_level(const float* prev, const float* lat, const float* wts, cons
                         NchwSwish<L::CO>{out}, wtc + dec_tc_off(K), wts + conv + (size_t)9 * 64 * L::CO, N, 2 * h, 2 * w, s);
 }
 
+// conv31: the last encoder layer, optionally with the model's + vit_feat in its epilogue
+static int enc_last(const float* in, float* out, const float* vit, int V, const float* wts, const unsigned char* wtc,
+                    int N, int IH, int IW, cudaStream_t s) {
+  if (vit == nullptr) return enc_layer<10>(in, out, wts, wtc, N, IH, IW, s);
+  using L = EncL<10>;
+  const float* bias = wts + enc_off(10) + (size_t)L::KS * L::KS * L::CI * L::CO;
+  return launch_conv<L>(NhwcSrc<L>{in, IH, IW}, NhwcLeakyAddVit<L::CO>{out, vit, V}, wtc + enc_tc_off(10), bias, N, IH,
+                        IW, s);
+}
+
 static bool shape_ok(int N, int H, int W) {
   return N > 0 && N <= 65535 && H >= 8 && W >= 8 && H % 8 == 0 && W % 8 == 0 && (long long)H * W < (1ll << 28);
 }
@@ -283,9 +307,9 @@ extern "C" int mvsf_fpn_encoder_workspace_bytes(int N, int H, int W, size_t* byt
   return MVSF_OK;
 }
 
-extern "C" int mvsf_fpn_encoder_forward(const float* x, const float* wts, const void* wts_tc, float* c01, float* c11,
-                                        float* c21, float* c31, void* workspace, size_t workspace_bytes, int N, int H,
-                                        int W, mvsf_stream_t stream) {
+static int encoder_forward(const float* x, const float* vit, int V, const float* wts, const void* wts_tc, float* c01,
+                           float* c11, float* c21, float* c31, void* workspace, size_t workspace_bytes, int N, int H,
+                           int W, mvsf_stream_t stream) {
   size_t need = 0;
   if (mvsf_fpn_encoder_workspace_bytes(N, H, W, &need) != MVSF_OK) return MVSF_ERR_INVALID;
   MVSF_REQUIRE(x && wts && wts_tc && c01 && c11 && c21 && c31 && workspace, "fpn_encoder_forward: null pointer");
@@ -306,7 +330,22 @@ extern "C" int mvsf_fpn_encoder_forward(const float* x, const float* wts, const 
   if ((rc = enc_layer<7>(t1, c21, wts, wtc, N, H / 4, W / 4, s))) return rc;
   if ((rc = enc_layer<8>(c21, t0, wts, wtc, N, H / 4, W / 4, s))) return rc;
   if ((rc = enc_layer<9>(t0, t1, wts, wtc, N, H / 8, W / 8, s))) return rc;
-  return enc_layer<10>(t1, c31, wts, wtc, N, H / 8, W / 8, s);
+  return enc_last(t1, c31, vit, V, wts, wtc, N, H / 8, W / 8, s);
+}
+
+extern "C" int mvsf_fpn_encoder_forward(const float* x, const float* wts, const void* wts_tc, float* c01, float* c11,
+                                        float* c21, float* c31, void* workspace, size_t workspace_bytes, int N, int H,
+                                        int W, mvsf_stream_t stream) {
+  return encoder_forward(x, nullptr, 1, wts, wts_tc, c01, c11, c21, c31, workspace, workspace_bytes, N, H, W, stream);
+}
+
+extern "C" int mvsf_fpn_encoder_vit_forward(const float* x, const float* vit_feat, int V, const float* wts,
+                                            const void* wts_tc, float* c01, float* c11, float* c21, float* c31,
+                                            void* workspace, size_t workspace_bytes, int N, int H, int W,
+                                            mvsf_stream_t stream) {
+  MVSF_REQUIRE(vit_feat && ((uintptr_t)vit_feat & 7) == 0 && V >= 1, "fpn_encoder_vit_forward: need an 8-byte aligned "
+               "vit_feat and V >= 1 (got V=%d)", V);
+  return encoder_forward(x, vit_feat, V, wts, wts_tc, c01, c11, c21, c31, workspace, workspace_bytes, N, H, W, stream);
 }
 
 extern "C" int mvsf_fpn_decoder_workspace_bytes(int N, int H, int W, size_t* bytes) {

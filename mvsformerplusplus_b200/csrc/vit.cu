@@ -58,6 +58,60 @@ __global__ void patch_im2col_kernel(const float* __restrict__ img, __half* __res
   split_store8(dst, dst + KPAD, v);
 }
 
+// ATen upsample_bicubic2d (UpSample.h get_cubic_upsample_coefficients, A = -0.75)
+__device__ __forceinline__ void cubic_coeffs(float t, float c[4]) {
+  constexpr float A = -0.75f;
+  const float x1 = t + 1.f, x2 = 1.f - t, x3 = x2 + 1.f;
+  c[0] = ((A * x1 - 5.f * A) * x1 + 8.f * A) * x1 - 4.f * A;
+  c[1] = ((A + 2.f) * t - (A + 3.f)) * t * t + 1.f;
+  c[2] = ((A + 2.f) * x2 - (A + 3.f)) * x2 * x2 + 1.f;
+  c[3] = ((A * x3 - 5.f * A) * x3 + 8.f * A) * x3 - 4.f * A;
+}
+
+// patch_im2col_kernel on the image resized from H x W to 14 gh x 14 gw the way F.interpolate(mode="bicubic",
+// align_corners=False) does it (ATen upsample_bicubic2d: scale in / out, source index scale (dst + 0.5) - 0.5, the four
+// taps clamped to the border, each row interpolated along x first, then the four rows along y).  The resized image never
+// reaches memory: each im2col element is evaluated from its 16 source pixels.
+__global__ void patch_im2col_bicubic_kernel(const float* __restrict__ img, __half* __restrict__ rows, int n, int gh,
+                                            int gw, int H, int W) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int P = gh * gw, oct = (int)(i % (KPAD / 8));
+  const long long row = i / (KPAD / 8);
+  if (row >= (long long)n * P) return;
+  const int b = (int)(row / P), p = (int)(row % P), py = p / gw, px = p % gw;
+  const float sy = (float)H / (float)(gh * PATCH), sx = (float)W / (float)(gw * PATCH);
+  float v[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const int k = oct * 8 + e;
+    v[e] = 0.f;
+    if (k < KP) {
+      const int c = k / 196, r = k % 196, ky = r / PATCH, kx = r % PATCH;
+      const float ry = sy * ((float)(py * PATCH + ky) + 0.5f) - 0.5f, rx = sx * ((float)(px * PATCH + kx) + 0.5f) - 0.5f;
+      const float fy = floorf(ry), fx = floorf(rx);
+      const int iy = (int)fy, ix = (int)fx;
+      float cy[4], cx[4];
+      cubic_coeffs(ry - fy, cy);
+      cubic_coeffs(rx - fx, cx);
+      int xs[4];
+#pragma unroll
+      for (int t = 0; t < 4; ++t) xs[t] = min(max(ix - 1 + t, 0), W - 1);
+      const float* plane = img + ((size_t)b * 3 + c) * H * W;
+      float acc = 0.f;
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const float* src = plane + (size_t)min(max(iy - 1 + t, 0), H - 1) * W;
+        const float rowv = __ldg(src + xs[0]) * cx[0] + __ldg(src + xs[1]) * cx[1] + __ldg(src + xs[2]) * cx[2] +
+                           __ldg(src + xs[3]) * cx[3];
+        acc = t == 0 ? rowv * cy[0] : acc + rowv * cy[t];
+      }
+      v[e] = acc;
+    }
+  }
+  __half* dst = rows + (size_t)row * 2 * KPAD + oct * 8;
+  split_store8(dst, dst + KPAD, v);
+}
+
 // x rows [0, n P): patch embedding (conv output with bias) += pos[1 + p]; rows n P + b: cls + pos[0]
 // (prepare_tokens_with_masks: cat(cls, patches) + pos).  Then xn2 <- split(norm1_0(x)).  One warp per row.
 __global__ void __launch_bounds__(256)
@@ -176,9 +230,10 @@ extern "C" int mvsf_vit_attention_forward(const float* qkv, int ldq, float* out,
   return vit::attention(qkv, ldq, out, ldo, nullptr, static_cast<__half*>(workspace), n, N, false, (cudaStream_t)stream);
 }
 
-extern "C" int mvsf_vit_forward(const float* img, const float* pos, const float* wts, const void* wts_tc, float* out0,
-                                float* out1, float* out2, void* workspace, size_t workspace_bytes, int n, int gh, int gw,
-                                mvsf_stream_t stream) {
+// the forward of both entry points: img [n][3][H][W], resized to 14 gh x 14 gw inside the patch im2col when `resize`
+static int vit_forward(const float* img, int H, int W, bool resize, const float* pos, const float* wts,
+                       const void* wts_tc, float* out0, float* out1, float* out2, void* workspace, size_t workspace_bytes,
+                       int n, int gh, int gw, mvsf_stream_t stream) {
   size_t need = 0;
   if (mvsf_vit_workspace_bytes(n, gh, gw, &need) != MVSF_OK) return MVSF_ERR_INVALID;
   MVSF_REQUIRE(img && pos && wts && wts_tc && out0 && out1 && out2 && workspace, "vit_forward: null pointer");
@@ -200,8 +255,14 @@ extern "C" int mvsf_vit_forward(const float* img, const float* pos, const float*
   const int P = gh * gw, N = P + 1, M = n * N;
   int rc;
   // patch embedding straight into the patch rows of the stream, then the tokens and block 0's norm1
-  patch_im2col_kernel<<<cdiv((long long)n * P * (KPAD / 8), 256), 256, 0, s>>>(img, hid2, n, gh, gw);
-  MVSF_LAUNCH_CHECK("vit_patch_im2col");
+  const long long im2col_threads = (long long)n * P * (KPAD / 8);
+  if (resize) {
+    patch_im2col_bicubic_kernel<<<cdiv(im2col_threads, 256), 256, 0, s>>>(img, hid2, n, gh, gw, H, W);
+    MVSF_LAUNCH_CHECK("vit_patch_im2col_bicubic");
+  } else {
+    patch_im2col_kernel<<<cdiv(im2col_threads, 256), 256, 0, s>>>(img, hid2, n, gh, gw);
+    MVSF_LAUNCH_CHECK("vit_patch_im2col");
+  }
   {
     TcsArgs a = tcs_rows(hid2, 2 * KPAD, KPAD, wh + G_PATCH, wl + G_PATCH, D, n * P);
     a.bias = wts + P_PATCHB; a.C = out0; a.ldc = D;
@@ -239,4 +300,19 @@ extern "C" int mvsf_vit_forward(const float* img, const float* pos, const float*
   final_norm_kernel<<<cdiv(n * P, 8), 256, 0, s>>>(x, wts + P_NW, wts + P_NB, out2, n * P);
   MVSF_LAUNCH_CHECK("vit_final_norm");
   return MVSF_OK;
+}
+
+extern "C" int mvsf_vit_forward(const float* img, const float* pos, const float* wts, const void* wts_tc, float* out0,
+                                float* out1, float* out2, void* workspace, size_t workspace_bytes, int n, int gh, int gw,
+                                mvsf_stream_t stream) {
+  return vit_forward(img, PATCH * gh, PATCH * gw, false, pos, wts, wts_tc, out0, out1, out2, workspace, workspace_bytes, n,
+                     gh, gw, stream);
+}
+
+extern "C" int mvsf_vit_forward_image(const float* img, int H, int W, const float* pos, const float* wts,
+                                      const void* wts_tc, float* out0, float* out1, float* out2, void* workspace,
+                                      size_t workspace_bytes, int n, int gh, int gw, mvsf_stream_t stream) {
+  MVSF_REQUIRE(H >= 1 && W >= 1 && (long long)H * W < (1ll << 30),
+               "vit_forward_image: need 1 <= H, W and H W < 2^30 (got H=%d W=%d)", H, W);
+  return vit_forward(img, H, W, true, pos, wts, wts_tc, out0, out1, out2, workspace, workspace_bytes, n, gh, gw, stream);
 }

@@ -11,6 +11,7 @@ enqueue libmvsf_b200 kernels.  PyTorch is used for device memory, streams and mo
   install(model, vit_decoder=True)  also rebinds model.decoder_vit
   DinoVisionTransformer.forward_interval_features(x, masks=None)                  <- models/dino/dinov2.py:249-266
   install(model, vit=True)  also rebinds model.vit (vit_base(...), DINOv2_mvsformer_model.py:40-41)
+  DINOv2MVSNet(args).forward(imgs, proj_matrices, depth_values, tmp)              <- DINOv2_mvsformer_model.py:68-179
 
 Tensors crossing the seams keep the reference's logical shapes ([B,V,C,H,W] features, [B,D,H,W] volumes).  Feature
 maps produced by FMT_with_pathway are channels-last in memory (a permuted view), which StageNet consumes
@@ -489,7 +490,9 @@ class FPNEncoder(_PackedMixin, nn.Module):
         return self._packed
 
     @torch.no_grad()
-    def forward(self, x):
+    def forward(self, x, vit_feat=None):
+        """vit_feat [V,64,H/8,W/8] (DINOv2MVSNet): conv31 is returned as conv31 + vit_feat[n % V], added in the last
+        layer's epilogue"""
         if self.training:
             raise NotImplementedError("the FPN hot path implements the eval-mode forward; call .eval()")
         N, C, H, W = x.shape
@@ -505,8 +508,19 @@ class FPNEncoder(_PackedMixin, nn.Module):
         need = ctypes.c_size_t(0)
         _lib.check(L.mvsf_fpn_encoder_workspace_bytes(N, H, W, ctypes.byref(need)), "fpn_encoder_workspace_bytes")
         ws = torch.empty(need.value // 4 + 4, **f32)
-        _lib.check(L.mvsf_fpn_encoder_forward(_ptr(x), _ptr(pk["w"]), _ptr(pk["tc"]), *[_ptr(o) for o in outs], _ptr(ws),
-                                              ctypes.c_size_t(ws.numel() * 4), N, H, W, _stream()), "fpn_encoder_forward")
+        if vit_feat is None:
+            _lib.check(L.mvsf_fpn_encoder_forward(_ptr(x), _ptr(pk["w"]), _ptr(pk["tc"]), *[_ptr(o) for o in outs],
+                                                  _ptr(ws), ctypes.c_size_t(ws.numel() * 4), N, H, W, _stream()),
+                       "fpn_encoder_forward")
+        else:
+            V = vit_feat.shape[0]
+            if tuple(vit_feat.shape) != (V, 64, H // 8, W // 8):
+                raise AssertionError(f"FPNEncoder: vit_feat must be [V,64,{H // 8},{W // 8}], got {tuple(vit_feat.shape)}")
+            _require_cuda(vit_feat, "FPNEncoder.forward(vit_feat)")
+            vit = to_nhwc(vit_feat)
+            _lib.check(L.mvsf_fpn_encoder_vit_forward(_ptr(x), _ptr(vit), V, _ptr(pk["w"]), _ptr(pk["tc"]),
+                                                      *[_ptr(o) for o in outs], _ptr(ws), ctypes.c_size_t(ws.numel() * 4),
+                                                      N, H, W, _stream()), "fpn_encoder_vit_forward")
         return [o.permute(0, 3, 1, 2) for o in outs]
 
 
@@ -700,16 +714,30 @@ class DinoVisionTransformer(_PackedMixin, nn.Module):
             raise NotImplementedError("DinoVisionTransformer: list inputs (forward_features_list) are not implemented")
         if masks is not None:
             raise NotImplementedError("DinoVisionTransformer: masks are not implemented")
-        if self.training:
-            raise NotImplementedError("the ViT implements the eval-mode forward; call .eval()")
-        n, c, H, W = x.shape
+        H, W = x.shape[-2:]
         ps = self.patch_size
         assert H % ps == 0, f"Input image height {H} is not a multiple of patch height {ps}"
         assert W % ps == 0, f"Input image width {W} is not a multiple of patch width: {ps}"
+        return self._interval_features(x, H // ps, W // ps, resize=False)
+
+    @torch.no_grad()
+    def forward_interval_features_resized(self, x, size):
+        """forward_interval_features(F.interpolate(x, size, mode="bicubic", align_corners=False)) with the resize done
+        inside the patch embedding (DINOv2_mvsformer_model.py:76-78): the resized images are never stored.  size =
+        (vit_h, vit_w), multiples of the patch size."""
+        vh, vw = size
+        ps = self.patch_size
+        if vh % ps or vw % ps or vh < ps or vw < ps:
+            raise ValueError(f"DinoVisionTransformer: the resized size must be positive multiples of {ps}, got {vh}x{vw}")
+        return self._interval_features(x, vh // ps, vw // ps, resize=True)
+
+    def _interval_features(self, x, gh, gw, resize):
+        if self.training:
+            raise NotImplementedError("the ViT implements the eval-mode forward; call .eval()")
+        n, c, H, W = x.shape
         if c != 3:
             raise AssertionError(f"DinoVisionTransformer expects [n,3,H,W] images, got {tuple(x.shape)}")
         _require_cuda(x, "DinoVisionTransformer.forward_interval_features(x)")
-        gh, gw = H // ps, W // ps
         L = _lib.lib()
         x = _f32c(x)
         if x.data_ptr() % 16:
@@ -724,14 +752,88 @@ class DinoVisionTransformer(_PackedMixin, nn.Module):
         need = ctypes.c_size_t(0)
         _lib.check(L.mvsf_vit_workspace_bytes(n, gh, gw, ctypes.byref(need)), "vit_workspace_bytes")
         ws = torch.empty(need.value // 4 + 4, **f32)
-        _lib.check(L.mvsf_vit_forward(_ptr(x), _ptr(pos), _ptr(pk["w"]), _ptr(pk["tc"]), *[_ptr(o) for o in outs],
-                                      _ptr(ws), ctypes.c_size_t(ws.numel() * 4), n, gh, gw, _stream()), "vit_forward")
+        if resize:
+            _lib.check(L.mvsf_vit_forward_image(_ptr(x), H, W, _ptr(pos), _ptr(pk["w"]), _ptr(pk["tc"]),
+                                                *[_ptr(o) for o in outs], _ptr(ws), ctypes.c_size_t(ws.numel() * 4), n, gh,
+                                                gw, _stream()), "vit_forward_image")
+        else:
+            _lib.check(L.mvsf_vit_forward(_ptr(x), _ptr(pos), _ptr(pk["w"]), _ptr(pk["tc"]), *[_ptr(o) for o in outs],
+                                          _ptr(ws), ctypes.c_size_t(ws.numel() * 4), n, gh, gw, _stream()), "vit_forward")
         return [o[:n * P].view(n, P, 768) for o in outs]
 
 
 def vit_base(patch_size=16, **kwargs):
     """models/dino/dinov2.py:388-398: the ViT-B DinoVisionTransformer (embed 768, depth 12, 12 heads, mlp_ratio 4)."""
     return DinoVisionTransformer(patch_size=patch_size, embed_dim=768, depth=12, num_heads=12, mlp_ratio=4, **kwargs)
+
+
+# =====================================================================================================
+class DINOv2MVSNet(nn.Module):
+    """Drop-in for the reference DINOv2MVSNet (models/networks/DINOv2_mvsformer_model.py:22-179), eval mode: same
+    constructor argument (config["arch"]["args"]), sub-module and parameter names (a reference checkpoint loads with
+    load_state_dict(strict=True)) and forward(imgs, proj_matrices, depth_values, tmp) -> the reference's output dict.
+    The whole forward, images to depth maps, runs on this package's kernels on the current stream:
+      ViT on the full-resolution images with the bicubic resize fused into its patch embedding -> ViT decoder ->
+      FPN encoder over all B V images with + vit_feat in conv31's epilogue -> FPN decoder over all B V images, whose NCHW
+      outputs are the [B,V,C,h,w] stage features as views -> FMT + cascade (cascade_forward).
+    As in the reference's eval forward (:88), image (b, v) receives batch item 0's vit_feat[v]: the ViT and its decoder run
+    on batch item 0's V images only.  vit_path is not read (a checkpoint carries the vit.* keys).  Images may be any float
+    dtype and strides; bf16 autocast does not change the arithmetic."""
+
+    def __init__(self, args):
+        super().__init__()
+        self.args = validate_args(load_args(args))
+        a = self.args
+        self.ndepths = a["ndepths"]
+        self.depth_interals_ratio = a["depth_interals_ratio"]
+        self.inverse_depth = a.get("inverse_depth", False)
+        self.use_pe3d = a.get("use_pe3d", False)
+        self.cost_reg_type = a.get("cost_reg_type", ["Normal"] * 4)
+        self.encoder = FPNEncoder(feat_chs=a["feat_chs"])
+        self.decoder = FPNDecoder(feat_chs=a["feat_chs"])
+        self.vit_args = a
+        self.freeze_vit = a.get("freeze_vit", True)
+        self.vit = vit_base(img_size=518, patch_size=14, init_values=1.0, block_chunks=0, ffn_layer="mlp",
+                            **a.get("dino_cfg", {}))
+        self.decoder_vit = CrossVITDecoder(a)
+        self.FMT_module = FMT_with_pathway(**a["FMT_config"])
+        self.fusions = nn.ModuleList([StageNet(a, self.ndepths[i], i) for i in range(len(self.ndepths))])
+
+    def vit_grid(self, H, W):
+        """the ViT's patch grid for H x W images: vit_h = int(H * rescale // 14 * 14) (DINOv2_mvsformer_model.py:72)"""
+        rescale = self.vit_args["rescale"]
+        return int(H * rescale // 14 * 14) // 14, int(W * rescale // 14 * 14) // 14
+
+    @torch.no_grad()
+    def extract_features(self, imgs):
+        """DINOv2_mvsformer_model.py:70-98: imgs [B,V,3,H,W] -> the FPN pyramid {stage1..4: [B,V,C,h,w]} (NCHW views)"""
+        if self.training:
+            raise NotImplementedError("DINOv2MVSNet implements the eval-mode forward (test.py); call .eval()")
+        B, V, C, H, W = imgs.shape
+        if C != 3:
+            raise AssertionError(f"DINOv2MVSNet expects [B,V,3,H,W] images, got {tuple(imgs.shape)}")
+        if H % 32 or W % 32 or H < 32 or W < 32:
+            raise ValueError(f"DINOv2MVSNet: image height and width must be positive multiples of 32 (the stage-1 "
+                             f"regulariser downsamples H/8 x W/8 by 4), got {H}x{W}")
+        gh, gw = self.vit_grid(H, W)
+        if 4 * gh != H // 8 or 4 * gw != W // 8:
+            raise NotImplementedError(f"DINOv2MVSNet: the ViT grid {gh}x{gw} (rescale {self.vit_args['rescale']}) must give "
+                                      f"vit_feat at H/8 x W/8 = {H // 8}x{W // 8}; the bilinear vit_feat resize of "
+                                      "DINOv2_mvsformer_model.py:80-82 is not implemented")
+        _require_cuda(imgs, "DINOv2MVSNet.forward(imgs)")
+        imgs = _f32c(imgs)
+        if imgs.data_ptr() % 16:
+            imgs = imgs.clone()
+        vit_out = self.vit.forward_interval_features_resized(imgs[0], (14 * gh, 14 * gw))
+        vit_feat = self.decoder_vit.forward([o.view(1, V, gh * gw, 768) for o in vit_out], vit_shape=(1, V, gh, gw, 768))
+        conv = self.encoder.forward(imgs.view(B * V, 3, H, W), vit_feat=vit_feat)
+        outs = self.decoder.forward(*conv)
+        return {f"stage{k + 1}": o.view(B, V, *o.shape[1:]) for k, o in enumerate(outs)}
+
+    @torch.no_grad()
+    def forward(self, imgs, proj_matrices, depth_values, tmp=(5.0, 5.0, 5.0, 1.0)):
+        features = self.extract_features(imgs)
+        return cascade_forward(self.FMT_module, self.fusions, self.args, features, proj_matrices, depth_values, tmp)
 
 
 # =====================================================================================================

@@ -26,15 +26,20 @@ class PrefetchingRunner:
                       for _ in range(slots)]
         self._next = 0
 
-    # a batch is (features: dict[str, Tensor], proj_matrices: dict[str, Tensor], depth_values: Tensor), pinned host tensors
+    # a batch is (features: dict[str, Tensor], proj_matrices: dict[str, Tensor], depth_values: Tensor), pinned host tensors,
+    # run by net.forward_features; or (imgs: Tensor [B,V,3,H,W], proj_matrices, depth_values), run by net.forward (a
+    # DINOv2MVSNet: images to depth maps, what the reference's test loop uploads)
     @staticmethod
     def _flat(batch):
         f, p, d = batch
-        return [f[k] for k in sorted(f)] + [p[k] for k in sorted(p)] + [d]
+        f = [f] if isinstance(f, torch.Tensor) else [f[k] for k in sorted(f)]
+        return f + [p[k] for k in sorted(p)] + [d]
 
     @staticmethod
     def _unflat(batch, flat):
         f, p, _ = batch
+        if isinstance(f, torch.Tensor):
+            return flat[0], {k: flat[1 + i] for i, k in enumerate(sorted(p))}, flat[-1]
         kf, kp = sorted(f), sorted(p)
         return ({k: flat[i] for i, k in enumerate(kf)}, {k: flat[len(kf) + i] for i, k in enumerate(kp)}, flat[-1])
 
@@ -83,7 +88,7 @@ class PrefetchingRunner:
         f, p, d = self._unflat(batch, cur["bufs"])
         with torch.cuda.stream(compute):
             compute.wait_event(cur["ready"])
-            out = self.net.forward_features(f, p, d, tmp)
+            out = (self.net.forward if isinstance(f, torch.Tensor) else self.net.forward_features)(f, p, d, tmp)
             cur["free"].record(compute)
         cur["tag"] = cur["batch"] = None                   # consumed: the same host batch is uploaded again next time
         if self.lanes:
