@@ -153,11 +153,6 @@ int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, c
 /* install-time helper: fp32 weight blob (n floats, n % 8 == 0) -> out16 = [n fp16 hi parts | n fp16 lo parts] (4n bytes) */
 int mvsf_split_weights_f16(const float* wts, void* out16, size_t n, mvsf_stream_t stream);
 
-/* ---- precision of the softmax probabilities inside the attention kernel: 0 (default) = fp16 P (one P*V product per
- * V half; the same rounded P feeds numerator and normaliser), 1 = fp16 hi + lo P (three partial products, fp32-class).
- * Both are held to the fp64 softmax attention in tests/test_gpu_parity.py; full-size cascade parity decides the default. */
-int mvsf_attention_set_precision(int p_lo);
-
 /* softmax attention of R1 alone: models/dino/layers/attention.py:141-170 (FlashAttention2.forward after the qkv linear).
  * qkv [N][3][4][16] fp32 -> out [N][64]; workspace >= (N+128)*896 bytes.  wgmma tensor cores, 3-term split-fp16 operands,
  * fp32 accumulation in registers; |q*scale|, |k|, |v| must be < 65504. */

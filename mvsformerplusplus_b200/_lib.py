@@ -40,7 +40,6 @@ SIGNATURES = {
     "mvsf_costreg_tr_workspace_bytes": ([I, I, I, I, ctypes.POINTER(Z)], I),
     "mvsf_costreg_tr_forward": ([P, P, P, P, Z, P, P, Z, I, I, I, I, I, F, P], I),
     "mvsf_split_weights_f16": ([P, P, Z, P], I),
-    "mvsf_attention_set_precision": ([I], I),
     "mvsf_attention_forward": ([P, P, P, Z, I, F, P], I),
     "mvsf_linear_tc_forward": ([P, P, P, P, P, Z, I, I, I, I, P], I),
     "mvsf_linear_tc_epilogue": ([I, P, I, P, P, P, I, P, P, P, F, I, P, I, P, I, P, I, P, Z, I, I, I, P], I),
@@ -82,8 +81,6 @@ def lib():
             fn = getattr(L, name)  # AttributeError if the symbol is not exported
             fn.argtypes = argt
             fn.restype = rest
-        if os.environ.get("MVSF_ATTENTION_PLO", "0") == "1":   # A-B measurements: round-1 three-product attention
-            L.mvsf_attention_set_precision(1)
         if os.environ.get("MVSF_VIS_XLO") in ("0", "1"):   # A-B measurements of the vis-CNN activation precision
             L.mvsf_vis_cnn_set_precision(int(os.environ["MVSF_VIS_XLO"]))
         if os.environ.get("MVSF_WARP_TILE", "1") in ("0", "2"):   # A-B measurements: 0 force the L1-gather kernels, 2 force the window kernels
@@ -122,8 +119,7 @@ class profile_calls:
             if name.endswith("_workspace_bytes") or name in ("mvsf_abi_version", "mvsf_launch_count", "mvsf_ktimer_enable",
                                                              "mvsf_ktimer_read", "mvsf_warp_corr_plan",
                                                              "mvsf_warp_corr_set_tile_path", "mvsf_warp_corr_set_max_window_miss", "mvsf_set_prefer_shared_carveout",
-                                                             "mvsf_warp_corr_last_selection", "mvsf_attention_set_precision",
-                                                             "mvsf_vis_cnn_set_precision"):
+                                                             "mvsf_warp_corr_last_selection", "mvsf_vis_cnn_set_precision"):
                 continue
             fn = getattr(L, name)
             self._orig[name] = fn

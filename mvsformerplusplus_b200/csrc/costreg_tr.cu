@@ -10,6 +10,7 @@
 #include <cuda_fp16.h>
 #include <float.h>
 
+#include "attention_fa.cuh"
 #include "linear_tc.cuh"
 #include "wgmma.cuh"
 
@@ -80,23 +81,6 @@ __global__ void patch_gather_kernel(const float* __restrict__ vol, __half* __res
   split_store8(row, row + 256, v);
 }
 
-__device__ __forceinline__ uint32_t pack_f16x2(float lo_elem, float hi_elem) {
-  uint32_t r;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
-  return r;
-}
-__device__ __forceinline__ float2 unpack_f16x2(uint32_t u) {
-  __half2 h = *reinterpret_cast<__half2*>(&u);
-  return __half22float2(h);  // .x = low half, .y = high half
-}
-__device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
-  hi = __float2half_rn(x);
-  lo = __float2half_rn(x - __half2float(hi));
-}
-using gmma::ex2f;
-
-#include "attention_fa.cuh"   // attention kernel (inside namespace mvsf)
-
 // un-patchify epilogue: u [N][256] (n = vox*8+co) -> LayerNorm3D over the 8 channels of each voxel (eps 1e-6)
 // -> prob 1x1x1 (8 -> 1) + bias -> logits [D][H][W]
 __global__ void unpatch_ln_prob_kernel(const float* __restrict__ u, const float* __restrict__ tail,
@@ -131,33 +115,22 @@ __global__ void unpatch_ln_prob_kernel(const float* __restrict__ u, const float*
 }
 
 
-// 0 (default): softmax probabilities as fp16 (P_hi only); 1: fp16 hi + lo (three partial P*V products, round-1 kernel)
-static int g_attention_plo = 0;
-
-// one CTA per NWG * 64 query rows of one head
-template <bool PLO, int NWG>
-static void launch_attention(const __half* tiled, float* o, __half* o2, int N, int ntiles, cudaStream_t s) {
-  attention_fa_kernel<PLO, NWG><<<dim3(cdiv(N, 64 * NWG), 4), fa::threads(NWG), fa::smem_bytes(NWG), s>>>(tiled, o, o2, N, ntiles);
-}
-
 static int run_attention(const float* qkv, float* o, __half* o2, __half* tiled, int N, float scale_log2e, cudaStream_t s) {
+  // three consumer warpgroups keep three softmax warps per SM sub-partition feeding the exp unit
+  constexpr int NWG = 3;
+  using A = fa::Layout<NWG>;
   const int ntiles = cdiv(N, 128);
   qkv_tile_kernel<<<cdiv((long long)ntiles * 128 * 24, 256), 256, 0, s>>>(qkv, tiled, N, ntiles, scale_log2e);
   MVSF_LAUNCH_CHECK("qkv_tile");
   static DeviceOnce once;
   const int dev = current_device();
   if (once.need(dev)) {
-    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa::smem_bytes(2)));
-    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fa::smem_bytes(3)));
+    MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)A::SMEM));
     once.done(dev);
   }
   cudaEvent_t kt = ktimer_enabled() ? ktimer_begin("attention_tc", s) : nullptr;
-  // three consumer warpgroups keep three softmax warps per SM sub-partition feeding the exp unit.  The hi + lo variant
-  // keeps two: it spills at 168 registers already, more than the 160 three warpgroups leave each thread.
-  if (g_attention_plo)
-    launch_attention<true, 2>(tiled, o, o2, N, ntiles, s);
-  else
-    launch_attention<false, 3>(tiled, o, o2, N, ntiles, s);
+  // one CTA per NWG * 64 query rows of one head
+  attention_fa_kernel<NWG><<<dim3(cdiv(N, 64 * NWG), 4), A::THREADS, A::SMEM, s>>>(tiled, o, o2, N, ntiles);
   if (kt) ktimer_end(kt, s);
   MVSF_LAUNCH_CHECK("attention_tc");
   return MVSF_OK;
@@ -254,12 +227,7 @@ int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, c
   return MVSF_OK;
 }
 
-/* Softmax attention alone (attention.py:141-170): qkv [N][3][4][16] fp32 -> out [N][64].  workspace >= N*768 bytes. */
-int mvsf_attention_set_precision(int p_lo) {
-  g_attention_plo = p_lo != 0;   // 0: fp16 P (default) | 1: fp16 hi+lo P (round 1)
-  return MVSF_OK;
-}
-
+/* Softmax attention alone (attention.py:141-170): qkv [N][3][4][16] fp32 -> out [N][64].  workspace >= (N+128)*896 bytes. */
 int mvsf_attention_forward(const float* qkv, float* out, void* workspace, size_t workspace_bytes, int N,
                            float softmax_scale, mvsf_stream_t stream) {
   MVSF_REQUIRE(qkv && out && workspace && N > 0, "attention_forward: bad arguments");

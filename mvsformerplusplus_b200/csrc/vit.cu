@@ -161,12 +161,12 @@ static int attention(const float* qkv, int ldq, float* out, int ldo, __half* out
   static DeviceOnce once;
   const int dev = current_device();
   if (once.need(dev)) {
-    MVSF_CUDA_OK(cudaFuncSetAttribute(vit_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vfa::SMEM));
+    MVSF_CUDA_OK(cudaFuncSetAttribute(vit_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vfa::Layout::SMEM));
     once.done(dev);
   }
   cudaEvent_t kt = ktimer_enabled() ? ktimer_begin("vit_attention", s) : nullptr;
-  vit_attention_kernel<<<dim3(cdiv(N, 128), vfa::NH, n), vfa::THREADS, vfa::SMEM, s>>>(tiled, out, ldo, out2, n, N, nt,
-                                                                                         cls_last);
+  vit_attention_kernel<<<dim3(cdiv(N, 128), vfa::NH, n), vfa::Layout::THREADS, vfa::Layout::SMEM, s>>>(tiled, out, ldo, out2,
+                                                                                                         n, N, nt, cls_last);
   if (kt) ktimer_end(kt, s);
   MVSF_LAUNCH_CHECK("vit_attention");
   return MVSF_OK;

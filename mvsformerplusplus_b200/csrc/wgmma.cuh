@@ -160,13 +160,6 @@ __device__ __forceinline__ void mma_ss_n256(float* d, uint64_t a, uint64_t b, ui
       : "l"(a), "l"(b), "r"(acc));
 }
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, A from registers (4 fp16x2 per thread, laid out like an m64n16 accumulator)
-__device__ __forceinline__ void mma_rs_n24(float* d, const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %17, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n24k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, %16, p, 1, 1, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
-}
 __device__ __forceinline__ void mma_rs_n40(float* d, const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %25, 0;\n\t"
@@ -235,6 +228,11 @@ __device__ __forceinline__ void fill_tile(uint32_t tile_smem, const __half* g, s
 __device__ __forceinline__ uint32_t pack_half2(float lo_elem, float hi_elem) {
   const __half2 h = __floats2half2_rn(lo_elem, hi_elem);
   return *reinterpret_cast<const uint32_t*>(&h);
+}
+// fp16 hi | lo split of one value
+__device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
+  hi = __float2half_rn(x);
+  lo = __float2half_rn(x - __half2float(hi));
 }
 // fp16 hi | lo split of two consecutive values, stored as one half2 each
 __device__ __forceinline__ void split_store2(__half* hi_dst, __half* lo_dst, float a, float b) {
