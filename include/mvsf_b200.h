@@ -159,6 +159,11 @@ int mvsf_split_weights_f16(const float* wts, void* out16, size_t n, mvsf_stream_
 int mvsf_attention_forward(const float* qkv, float* out, void* workspace, size_t workspace_bytes, int N,
                            float softmax_scale, mvsf_stream_t stream);
 
+/* how mvsf_attention_forward (and each layer of mvsf_costreg_tr_forward) covers num_sms SMs at N tokens: the last
+ * *split_items (head, 192-query) items of the grid run as *parts key ranges each, merged by a second kernel; 0 and 1
+ * when every item runs whole.  Host only. */
+int mvsf_attention_split_plan(int N, int num_sms, int* split_items, int* parts);
+
 /* token-wise linear layer alone (nn.Linear, e.g. models/module.py:520-522 FFN.linear1): C[M,N] = act(A[M,K] W[N,K]^T + bias)
  * on the wgmma tensor cores with fp16 hi/lo split operands (fp32-class accuracy).  N in {16, 64, 128, 192, 256}, K % 64 == 0.
  * workspace >= (M+N)*2K*2 + 256 bytes.  gelu != 0 applies the exact-erf GELU. */

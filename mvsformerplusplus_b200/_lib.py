@@ -41,6 +41,7 @@ SIGNATURES = {
     "mvsf_costreg_tr_forward": ([P, P, P, P, Z, P, P, Z, I, I, I, I, I, F, P], I),
     "mvsf_split_weights_f16": ([P, P, Z, P], I),
     "mvsf_attention_forward": ([P, P, P, Z, I, F, P], I),
+    "mvsf_attention_split_plan": ([I, I, ctypes.POINTER(I), ctypes.POINTER(I)], I),
     "mvsf_linear_tc_forward": ([P, P, P, P, P, Z, I, I, I, I, P], I),
     "mvsf_linear_tc_epilogue": ([I, P, I, P, P, P, I, P, P, P, F, I, P, I, P, I, P, I, P, Z, I, I, I, P], I),
     "mvsf_softargmax": ([P, P, F, P, P, P, I, I, I, P], I),
@@ -117,7 +118,7 @@ class profile_calls:
         self._orig = {}
         for name in SIGNATURES:
             if name.endswith("_workspace_bytes") or name in ("mvsf_abi_version", "mvsf_launch_count", "mvsf_ktimer_enable",
-                                                             "mvsf_ktimer_read", "mvsf_warp_corr_plan",
+                                                             "mvsf_ktimer_read", "mvsf_warp_corr_plan", "mvsf_attention_split_plan",
                                                              "mvsf_warp_corr_set_tile_path", "mvsf_warp_corr_set_max_window_miss", "mvsf_set_prefer_shared_carveout",
                                                              "mvsf_warp_corr_last_selection", "mvsf_vis_cnn_set_precision"):
                 continue

@@ -11,10 +11,16 @@
 // 416-thread CTA (three warpgroups + one producer warp) would cap every thread at 128 registers (four of its warps share
 // one sub-partition's 16 384), below the loop's ~150: the producer is a whole warpgroup that gives its registers away
 // (setmaxnreg 32 / 160).  On an H100 SXM at a 400 W limit: 1.63-1.73 ms per launch at N = 27 648 (two warpgroups
-// 1.83-1.92), 2.44-2.48 ms at N = 32 640 (2.59-2.64), though 192-row CTAs leave a coarser last wave (DTU 576 CTAs on 132
-// SMs: 5 waves, busiest SM 960 rows against 896 with 128-row CTAs).
+// 1.83-1.92), 2.44-2.48 ms at N = 32 640 (2.59-2.64).
+// One CTA per SM runs in waves, and time follows the waves, not the work: on an H100 SXM (132 SMs, 700 W) N = 27 648
+// (576 items: 4 full waves + 48) takes 1.33x the time of N = 25 344 (528: exactly 4 waves) for 1.19x the work.  So the
+// items of a partial last wave are split over key ranges (fa::split_plan) that run on the otherwise idle SMs, and
+// attention_merge_kernel merges their partials: DTU 48 items x 2 parts, T&T (680 items) 20 x 6.  Same card, merge
+// included: 1.23-1.26 ms per call at N = 27 648 (1.37-1.39 without the split), 1.67-1.69 ms at N = 32 640 (1.91-1.96).
 #pragma once
 #include <cuda_fp16.h>
+
+#include <algorithm>
 
 #include "linear_tc.cuh"
 #include "softmax_attention.cuh"
@@ -82,10 +88,15 @@ struct Layout {
   static constexpr uint32_t OFF_K = 0, OFF_V = OFF_K + NKV * 2 * K_TILE, OFF_Q = OFF_V + NKV * V_TILE,
                             OFF_BAR = OFF_Q + NWG * Q_BLOCK, SMEM = OFF_BAR + 8 + 32 * NKV;
   static constexpr int THREADS = 128 * (NWG + 1);   // NWG consumer warpgroups + the producer warpgroup
+  // an item is one head's group of ROWS query rows; the partial of a key range of it: per row o (HD), m, l
+  static constexpr bool SPLIT = true;
+  static constexpr int ROWS = 64 * NWG, PART_FLOATS = ROWS * (HD + 2);
 
   const __half* tiled;
   const __half* base;         // this head in the Q and K planes: + plane index * plane + tile * 2048
   size_t plane, head_tiles;   // head_tiles = head * ntiles
+  int head, group, t0, t1;    // the CTA's item and key tiles [t0, t1)
+  float* part;                // null for a whole item, else the partial slot of the key range
 
   // descriptors of the warpgroup's Q block at q (hi, lo)
   struct QOperand { uint64_t hi, lo; };
@@ -133,14 +144,87 @@ struct Layout {
 };
 }  // namespace fa
 
+namespace fa {
+// bytes of the tiled planes per 128-key tile: Q hi, Q lo, K hi, K lo (4 heads x 2048 halves each) and V^T (4 x 5120)
+constexpr size_t TILE_BYTES = (4 * 4 * 2048 + 4 * 5120) * sizeof(__half);
+// shortest key range worth a CTA of its own: a split item costs a second launch (a few us) and every part refills the
+// K / V ring, while a key tile takes ~1.3 us (H100 SXM, 700 W)
+constexpr int MIN_PART_TILES = 16;
+
+// How one attention call covers the SMs.  The 4 ceil(N / ROWS) items of ntiles key tiles run one CTA per SM; when the
+// last wave is partial, its `split` items (the last ones) are each cut into `parts` contiguous key ranges whose lengths
+// differ by at most one tile, so that the wave runs on up to `sms` SMs instead of `split`.  The parts' partials take
+// the workspace beyond the tiled planes (`region_bytes` in all).  split = 0, parts = 1: every item runs whole.
+struct SplitPlan { int items, split, parts; };
+template <int NWG>
+inline SplitPlan split_plan(int N, int sms, size_t region_bytes) {
+  using A = Layout<NWG>;
+  const int ntiles = (N + 127) / 128, items = 4 * ((N + A::ROWS - 1) / A::ROWS), r = items % sms;
+  const size_t planes = (size_t)ntiles * TILE_BYTES;
+  const size_t slots = region_bytes > planes ? (region_bytes - planes) / (A::PART_FLOATS * sizeof(float)) : 0;
+  const int k = r ? (int)std::min({(size_t)(sms / r), slots / r, (size_t)(ntiles / MIN_PART_TILES)}) : 0;
+  return k >= 2 ? SplitPlan{items, r, k} : SplitPlan{items, 0, 1};
+}
+}  // namespace fa
+
 // out: fp32 rows [N][64] and / or out2: fp16 hi|lo rows [N][hi(64) | lo(64)].  NWG (3 shipped) is in the kernel's name.
+// 1-D grid of fa::split_plan: the whole items first, then the `parts` key ranges of each of the last `split` items (the
+// block scheduler starts the short ranges last), which write their partials to `partials` for attention_merge_kernel.
 template <int NWG>
 __global__ void __launch_bounds__(fa::Layout<NWG>::THREADS, 1)
-attention_fa_kernel(const __half* __restrict__ tiled, float* __restrict__ out, __half* __restrict__ out2, int N, int ntiles) {
-  const int head = blockIdx.y;
+attention_fa_kernel(const __half* __restrict__ tiled, float* __restrict__ out, __half* __restrict__ out2, int N, int ntiles,
+                    int split, int parts, float* __restrict__ partials) {
+  using A = fa::Layout<NWG>;
+  const int groups = (N + A::ROWS - 1) / A::ROWS, whole = 4 * groups - split;
+  int item = blockIdx.x, t0 = 0, t1 = ntiles;
+  float* part = nullptr;
+  if (item >= whole) {
+    const int b = item - whole, p = b % parts;
+    item = whole + b / parts;
+    t0 = p * ntiles / parts;
+    t1 = (p + 1) * ntiles / parts;
+    part = partials + (size_t)b * A::PART_FLOATS;
+  }
+  const int head = item / groups;
   const size_t head_tiles = (size_t)head * ntiles;
-  const fa::Layout<NWG> lay{tiled, tiled + head_tiles * 2048, (size_t)4 * ntiles * 2048, head_tiles};
+  const A lay{tiled, tiled + head_tiles * 2048, (size_t)4 * ntiles * 2048, head_tiles, head, item % groups, t0, t1, part};
   attn::softmax_attention(lay, out, 64, out2, N, ntiles);
+}
+
+// The outputs of the split items: per row, the `parts` partials (o, m, l) merged in part order, m* = max m, o and l
+// weighted by 2^(m - m*), then the epilogue of softmax_attention.  One thread per (split item, row); no CTA of the
+// attention kernel waits for another.
+template <int NWG>
+__global__ void attention_merge_kernel(const float* __restrict__ partials, float* __restrict__ out, __half* __restrict__ out2,
+                                       int N, int split, int parts) {
+  using A = fa::Layout<NWG>;
+  constexpr int HD = A::HD, W = A::NH * A::HD, ROWS = A::ROWS;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= split * ROWS) return;
+  const int groups = (N + ROWS - 1) / ROWS, s = i / ROWS, rr = i % ROWS, item = 4 * groups - split + s;
+  const int head = item / groups, t = (item % groups) * ROWS + rr;
+  if (t >= N) return;
+  const float* p0 = partials + (size_t)s * parts * A::PART_FLOATS + (size_t)rr * (HD + 2);
+  float mx = -1e30f;
+  for (int p = 0; p < parts; ++p) mx = fmaxf(mx, p0[(size_t)p * A::PART_FLOATS + HD]);
+  float o[HD], l = 0.f;
+#pragma unroll
+  for (int d = 0; d < HD; ++d) o[d] = 0.f;
+  for (int p = 0; p < parts; ++p) {
+    const float* pp = p0 + (size_t)p * A::PART_FLOATS;
+    const float w = gmma::ex2f(pp[HD] - mx);
+    l = fmaf(pp[HD + 1], w, l);
+#pragma unroll
+    for (int d = 0; d < HD; ++d) o[d] = fmaf(pp[d], w, o[d]);
+  }
+  const float inv = __fdiv_rn(1.0f, l);
+#pragma unroll
+  for (int d = 0; d < HD; d += 2) {
+    const int col = head * HD + d;
+    const float r0 = o[d] * inv, r1 = o[d + 1] * inv;
+    if (out) *reinterpret_cast<float2*>(out + (size_t)t * W + col) = make_float2(r0, r1);
+    if (out2) gmma::split_store2(out2 + (size_t)t * (2 * W) + col, out2 + (size_t)t * (2 * W) + W + col, r0, r1);
+  }
 }
 
 }  // namespace mvsf

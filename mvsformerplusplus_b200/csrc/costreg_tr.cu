@@ -115,9 +115,13 @@ __global__ void unpatch_ln_prob_kernel(const float* __restrict__ u, const float*
 }
 
 
+// three consumer warpgroups keep three softmax warps per SM sub-partition feeding the exp unit
+constexpr int ATT_NWG = 3;
+// the operand workspace of one attention call: the tiled planes, then the partials of the split plan
+static size_t attention_workspace_bytes(int N) { return (size_t)(N + 128) * 896; }
+
 static int run_attention(const float* qkv, float* o, __half* o2, __half* tiled, int N, float scale_log2e, cudaStream_t s) {
-  // three consumer warpgroups keep three softmax warps per SM sub-partition feeding the exp unit
-  constexpr int NWG = 3;
+  constexpr int NWG = ATT_NWG;
   using A = fa::Layout<NWG>;
   const int ntiles = cdiv(N, 128);
   qkv_tile_kernel<<<cdiv((long long)ntiles * 128 * 24, 256), 256, 0, s>>>(qkv, tiled, N, ntiles, scale_log2e);
@@ -128,11 +132,19 @@ static int run_attention(const float* qkv, float* o, __half* o2, __half* tiled, 
     MVSF_CUDA_OK(cudaFuncSetAttribute(attention_fa_kernel<NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)A::SMEM));
     once.done(dev);
   }
+  const fa::SplitPlan plan = fa::split_plan<NWG>(N, device_sm_count(dev), attention_workspace_bytes(N));
+  float* partials = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(tiled) + (size_t)ntiles * fa::TILE_BYTES);
+  // one timed call: the attention and the merge of its split items
   cudaEvent_t kt = ktimer_enabled() ? ktimer_begin("attention_tc", s) : nullptr;
-  // one CTA per NWG * 64 query rows of one head
-  attention_fa_kernel<NWG><<<dim3(cdiv(N, 64 * NWG), 4), A::THREADS, A::SMEM, s>>>(tiled, o, o2, N, ntiles);
-  if (kt) ktimer_end(kt, s);
+  attention_fa_kernel<NWG><<<plan.items - plan.split + plan.split * plan.parts, A::THREADS, A::SMEM, s>>>(
+      tiled, o, o2, N, ntiles, plan.split, plan.parts, partials);
   MVSF_LAUNCH_CHECK("attention_tc");
+  if (plan.split) {
+    attention_merge_kernel<NWG><<<cdiv((long long)plan.split * A::ROWS, 128), 128, 0, s>>>(partials, o, o2, N, plan.split,
+                                                                                            plan.parts);
+    MVSF_LAUNCH_CHECK("attention_merge");
+  }
+  if (kt) ktimer_end(kt, s);
   return MVSF_OK;
 }
 
@@ -231,7 +243,16 @@ int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, c
 int mvsf_attention_forward(const float* qkv, float* out, void* workspace, size_t workspace_bytes, int N,
                            float softmax_scale, mvsf_stream_t stream) {
   MVSF_REQUIRE(qkv && out && workspace && N > 0, "attention_forward: bad arguments");
-  if (workspace_bytes < (size_t)(N + 128) * 896) return fail(MVSF_ERR_WORKSPACE, "attention_forward: workspace %zu < %zu bytes", workspace_bytes, (size_t)(N + 128) * 896);
+  if (workspace_bytes < attention_workspace_bytes(N)) return fail(MVSF_ERR_WORKSPACE, "attention_forward: workspace %zu < %zu bytes", workspace_bytes, attention_workspace_bytes(N));
   return run_attention(qkv, out, nullptr, reinterpret_cast<__half*>(workspace), N, softmax_scale * 1.4426950408889634f, (cudaStream_t)stream);
+}
+
+/* the split plan mvsf_attention_forward and mvsf_costreg_tr_forward run for N tokens on num_sms SMs */
+int mvsf_attention_split_plan(int N, int num_sms, int* split_items, int* parts) {
+  MVSF_REQUIRE(N > 0 && num_sms > 0 && split_items && parts, "attention_split_plan: bad arguments");
+  const fa::SplitPlan p = fa::split_plan<ATT_NWG>(N, num_sms, attention_workspace_bytes(N));
+  *split_items = p.split;
+  *parts = p.parts;
+  return MVSF_OK;
 }
 }

@@ -3,7 +3,8 @@
 // warpgroup and stage counts, register split, tile sizes, the Q / K / V source addresses, the products and the output
 // row map.
 //
-// One CTA works on L::NWG x 64 query rows (grid x) of one head (grid y):
+// One CTA works on L::NWG x 64 query rows (grid x) of one head (grid y), over all keys, or (L::SPLIT) on the query
+// group, head and key-tile range the layout gives it:
 //   warpgroup NWG   bulk-copy producer (one thread): the CTA's Q blocks, then K (hi, lo) and V^T tiles of 128 keys,
 //                   pre-tiled into the canonical K-major layouts, through two mbarrier rings of L::NKV stages
 //   warpgroups 0..NWG-1   64 query rows each.  Per 128-key tile: S = Q_lo K_hi + Q_hi K_lo + Q_hi K_hi (fp32 scores in
@@ -37,6 +38,10 @@
 //                                    last one instead)
 //   k_tile(t, p), v_tile(t)          global source of K tile t (p = 0 hi, 1 lo) and V^T tile t
 //   row(t)                           output row of query t
+//   SPLIT                            false: grid (query group, head), all key tiles.  true: members head, group (query
+//                                    group of L::NWG x 64 rows), key tiles [t0, t1) and part: null, or the CTA's
+//                                    partial slot, which gets per row the unnormalised output (HD), m and l instead
+//                                    of the output rows
 #pragma once
 #include <cuda_fp16.h>
 
@@ -81,6 +86,16 @@ __device__ __forceinline__ void pack_p(const float (&S)[64], uint32_t (&ph)[8][4
     for (int r = 0; r < 4; ++r) ph[i][r] = pack_half2(S[8 * i + 2 * r], S[8 * i + 2 * r + 1]);
 }
 
+// the CTA's head and query group (of L::NWG x 64 rows)
+template <class L>
+__device__ __forceinline__ int item_head(const L& lay) {
+  if constexpr (L::SPLIT) return lay.head; else return blockIdx.y;
+}
+template <class L>
+__device__ __forceinline__ int item_group(const L& lay) {
+  if constexpr (L::SPLIT) return lay.group; else return blockIdx.x;
+}
+
 // out: fp32 rows (row stride ldo) and / or out2: fp16 hi|lo rows [hi(NH HD) | lo(NH HD)], rows from lay.row
 template <class L>
 __device__ __forceinline__ void softmax_attention(const L& lay, float* __restrict__ out, int ldo, __half* __restrict__ out2,
@@ -89,7 +104,12 @@ __device__ __forceinline__ void softmax_attention(const L& lay, float* __restric
   static_assert(128 * (L::REGS_PRODUCER + NWG * L::REGS_CONSUMER) <= 65536, "setmaxnreg exceeds the register file");
   extern __shared__ __align__(128) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int head = blockIdx.y;
+  const int head = item_head(lay);
+  int t0 = 0, nt = ntiles;                 // key tiles t0 .. t0 + nt - 1
+  float* part = nullptr;
+  if constexpr (L::SPLIT) {
+    t0 = lay.t0; nt = lay.t1 - lay.t0; part = lay.part;
+  }
   const uint32_t sb = smem_u32(smem);
   const uint32_t bar_q = sb + L::OFF_BAR, bar_kf = bar_q + 8, bar_ke = bar_kf + 8 * NKV, bar_vf = bar_ke + 8 * NKV,
                  bar_ve = bar_vf + 8 * NKV;
@@ -110,24 +130,24 @@ __device__ __forceinline__ void softmax_attention(const L& lay, float* __restric
     if (warp == 4 * NWG && lane == 0) {
       const int nqb = L::q_blocks(N, ntiles);
       expect_tx(bar_q, NWG * L::Q_BLOCK);
-      for (int w = 0; w < NWG; ++w) lay.load_q(sb + L::OFF_Q + w * L::Q_BLOCK, min(NWG * (int)blockIdx.x + w, nqb - 1), bar_q);
-      for (int t = 0; t < ntiles; ++t) {
+      for (int w = 0; w < NWG; ++w) lay.load_q(sb + L::OFF_Q + w * L::Q_BLOCK, min(NWG * item_group(lay) + w, nqb - 1), bar_q);
+      for (int t = 0; t < nt; ++t) {
         const int s = t % NKV;
         const uint32_t par = (uint32_t)(((t / NKV) & 1) ^ 1);
         mbar_wait(bar_ke + 8 * s, par);
         expect_tx(bar_kf + 8 * s, 2 * L::K_TILE);
-        bulk_load(sb + L::OFF_K + (2 * s) * L::K_TILE, lay.k_tile(t, 0), L::K_TILE, bar_kf + 8 * s);
-        bulk_load(sb + L::OFF_K + (2 * s + 1) * L::K_TILE, lay.k_tile(t, 1), L::K_TILE, bar_kf + 8 * s);
+        bulk_load(sb + L::OFF_K + (2 * s) * L::K_TILE, lay.k_tile(t0 + t, 0), L::K_TILE, bar_kf + 8 * s);
+        bulk_load(sb + L::OFF_K + (2 * s + 1) * L::K_TILE, lay.k_tile(t0 + t, 1), L::K_TILE, bar_kf + 8 * s);
         mbar_wait(bar_ve + 8 * s, par);
         expect_tx(bar_vf + 8 * s, L::V_TILE);
-        bulk_load(sb + L::OFF_V + s * L::V_TILE, lay.v_tile(t), L::V_TILE, bar_vf + 8 * s);
+        bulk_load(sb + L::OFF_V + s * L::V_TILE, lay.v_tile(t0 + t), L::V_TILE, bar_vf + 8 * s);
       }
     }
     return;
   }
   // -------------------------------------------------------------------------------------------- MMA + softmax warpgroups
   asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(L::REGS_CONSUMER));
-  // thread (warpgroup wg, warp wq of it, lane): query rows 64 (NWG blockIdx.x + wg) + 16 wq + lane / 4 + 8 h (h = 0, 1);
+  // thread (warpgroup wg, warp wq of it, lane): query rows 64 (NWG group + wg) + 16 wq + lane / 4 + 8 h (h = 0, 1);
   // score / output columns 8 b + 2 (lane % 4) + e of accumulator register 4 b + 2 h + e
   const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
   const bool leader = (tid & 127) == 0;
@@ -147,14 +167,14 @@ __device__ __forceinline__ void softmax_attention(const L& lay, float* __restric
   wg_wait<0>();
   fence_regs<64>(S);
   if (leader) mbar_arrive(bar_ke);
-  softmax_tile(S, m, corr, 0, N, q);
+  softmax_tile(S, m, corr, t0, N, q);
   pack_p(S, ph);
-  if (ntiles > 1) {                            // operands of iteration 0
+  if (nt > 1) {                                // operands of iteration 0
     mbar_wait(bar_kf + 8, 0u);
     mbar_wait(bar_vf, 0u);
   }
   // iteration j: scores of tile j + 1 and P*V of tile j; the softmax of tile j + 1 overlaps P*V of tile j
-  for (int j = 0; j + 1 < ntiles; ++j) {
+  for (int j = 0; j + 1 < nt; ++j) {
     const int s = j % NKV, s1 = (j + 1) % NKV, s2 = (j + 2) % NKV;
     wg_fence();
     L::issue_scores(S, qs, sb + L::OFF_K + (2 * s1) * L::K_TILE);
@@ -163,10 +183,10 @@ __device__ __forceinline__ void softmax_attention(const L& lay, float* __restric
     fence_regs<64>(S);
     if (leader) mbar_arrive(bar_ke + 8 * s1);
     float corr1[2];
-    softmax_tile(S, m, corr1, j + 1, N, q);
+    softmax_tile(S, m, corr1, t0 + j + 1, N, q);
     // operands of the next iteration.  Waiting for them here, between the softmax and the wait for P*V, also keeps ptxas
     // from hoisting that wait above the softmax: it does not move it across the polling loop.
-    if (j + 2 < ntiles) mbar_wait(bar_kf + 8 * s2, (uint32_t)(((j + 2) / NKV) & 1));
+    if (j + 2 < nt) mbar_wait(bar_kf + 8 * s2, (uint32_t)(((j + 2) / NKV) & 1));
     mbar_wait(bar_vf + 8 * s1, (uint32_t)(((j + 1) / NKV) & 1));
     wg_wait<0>();
     fence_regs<L::O_REGS>(O);
@@ -177,7 +197,7 @@ __device__ __forceinline__ void softmax_attention(const L& lay, float* __restric
     corr[1] = corr1[1];
   }
   {                                            // P*V of the last tile
-    const int j = ntiles - 1, s = j % NKV;
+    const int j = nt - 1, s = j % NKV;
     mbar_wait(bar_vf + 8 * s, (uint32_t)((j / NKV) & 1));
     wg_fence();
     L::issue_pv(O, ph, sb + L::OFF_V + s * L::V_TILE);
@@ -185,10 +205,23 @@ __device__ __forceinline__ void softmax_attention(const L& lay, float* __restric
     fence_regs<L::O_REGS>(O);
     L::fold_tile(o, l, O, corr, lane);
   }
+  if constexpr (L::SPLIT) {
+    if (part) {                                // a key range of the item: its partial, rows >= N included
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float* pr = part + (size_t)(64 * wg + 16 * wq + (lane >> 2) + 8 * h) * (L::HD + 2);
+#pragma unroll
+        for (int b = 0; b < L::HD / 8; ++b)
+          *reinterpret_cast<float2*>(pr + 8 * b + 2 * q) = make_float2(o[h][2 * b], o[h][2 * b + 1]);
+        if (q == 0) *reinterpret_cast<float2*>(pr + L::HD) = make_float2(m[h], l[h]);
+      }
+      return;
+    }
+  }
   constexpr int W = L::NH * L::HD;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int t = 64 * (NWG * (int)blockIdx.x + wg) + 16 * wq + (lane >> 2) + 8 * h;
+    const int t = 64 * (NWG * item_group(lay) + wg) + 16 * wq + (lane >> 2) + 8 * h;
     if (t >= N) continue;
     const size_t r = lay.row(t);
     const float inv = __fdiv_rn(1.0f, l[h]);

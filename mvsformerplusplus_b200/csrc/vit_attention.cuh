@@ -102,6 +102,7 @@ struct Layout {
   static constexpr uint32_t OFF_K = 0, OFF_V = OFF_K + NKV * 2 * K_TILE, OFF_Q = OFF_V + NKV * V_TILE,
                             OFF_BAR = OFF_Q + NWG * Q_BLOCK, SMEM = OFF_BAR + 8 + 32 * NKV;
   static constexpr int THREADS = 128 * (NWG + 1);
+  static constexpr bool SPLIT = false;   // grid (query tiles, heads, images), every CTA over all keys
 
   const __half* qbase;   // this (image, head) in the Q hi, K hi and V^T planes
   const __half* kbase;
