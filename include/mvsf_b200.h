@@ -181,6 +181,22 @@ int mvsf_linear_tc_epilogue(int epi, const float* A, int lda, const float* W, co
                             int ldres, const float* gamma, const float* ln_w, const float* ln_b, float ln_eps,
                             int elu_cols, float* C, int ldc, float* Cpre, int ldcpre, void* C2, int ldc2,
                             void* workspace, size_t workspace_bytes, int M, int N, int K, mvsf_stream_t stream);
+/* test seam: the token MLP of an FMT block or a transformer-regulariser layer in the one kernel they run it on: proj,
+ * its residual + LayerNorm epilogue, FFN1 (GELU), FFN2 and its residual epilogue.  With p = A proj_w^T + proj_b and
+ * f(z) = gelu(z f1_w^T + f1_b) f2_w^T + f2_b:
+ *   form 0 (pre-norm block): x = res + gamma1 p; x += gamma2 f(LN_mid(x)); C = x, C2 = split(LN_out(x))
+ *   form 1 (last pre-norm block): the same, C = x only (C2, out_w, out_b unused)
+ *   form 2 (post-norm layer): y = LN_mid(res + gamma1 p); C = LN_out(y + gamma2 f(y)), C2 = split(C)
+ * LN_mid / LN_out: LayerNorm over the row with mid_w, mid_b, mid_eps / out_w, out_b, out_eps.  Dense fp32 rows: A, res
+ * and C [M][64] (C may alias res); C2 [M][128] fp16 = [hi(64) | lo(64)].  Weights fp32 in nn.Linear layout: proj_w
+ * [64][64], f1_w [256][64], f2_w [64][256]; A and the weights are split into fp16 hi/lo parts inside the call.  The
+ * outputs equal those of the three mvsf_linear_tc_epilogue calls (proj: epilogue 4, FFN1: epilogue 1, FFN2: epilogue 4
+ * or 3) bit for bit.  Operands and outputs 16-byte aligned.  workspace >= (M*128 + 73728)*2 bytes. */
+int mvsf_token_mlp_forward(int form, const float* A, const float* res, const float* proj_w, const float* proj_b,
+                           const float* gamma1, const float* mid_w, const float* mid_b, float mid_eps, const float* f1_w,
+                           const float* f1_b, const float* f2_w, const float* f2_b, const float* gamma2,
+                           const float* out_w, const float* out_b, float out_eps, float* C, void* C2, void* workspace,
+                           size_t workspace_bytes, int M, mvsf_stream_t stream);
 /* test seam: the streamed-weight GEMM the ViT decoder runs on (models/module.py:273-364: its q/k/v, proj, fc1, fc2
  * linears and conv head), for token rows.  Weights stream through the pipeline with A, so N and K are limited only by
  * N % 64 == 0 and K % 64 == 0.  epi: 0 bias, 1 gelu, 2 elu+1 on columns < elu_cols, 3 C = res + gamma * (acc + bias),

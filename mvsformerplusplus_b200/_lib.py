@@ -55,6 +55,7 @@ SIGNATURES = {
     "mvsf_fpn_decoder_forward": ([P] * 11 + [Z, I, I, I, P], I),
     "mvsf_fpn_tc_bytes": ([I, ctypes.POINTER(Z)], I),
     "mvsf_fpn_pack_tc": ([I, P, P, Z, P], I),
+    "mvsf_token_mlp_forward": ([I, P, P, P, P, P, P, P, F, P, P, P, P, P, P, P, F, P, P, P, Z, I, P], I),
     "mvsf_linear_tc_streamed_epilogue": ([I, P, I, P, P, P, I, P, I, P, I, P, I, P, Z, I, I, I, P], I),
     "mvsf_vit_decoder_workspace_bytes": ([I, I, I, I, ctypes.POINTER(Z)], I),
     "mvsf_vit_decoder_tc_bytes": ([ctypes.POINTER(Z)], I),

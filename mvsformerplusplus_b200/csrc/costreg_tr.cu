@@ -159,9 +159,8 @@ int mvsf_costreg_tr_workspace_bytes(int C, int D, int H, int W, size_t* bytes) {
   MVSF_REQUIRE(D % 2 == 0 && H % 4 == 0 && W % 4 == 0 && D > 0 && H > 0 && W > 0,
                "costreg_tr: D %% 2, H %% 4, W %% 4 must be 0 (down_rate (2,4,4))");
   size_t N = (size_t)(D / 2) * (H / 4) * (W / 4);
-  // per token (in floats): big 256 (patches2 / ffn hidden split / un-patchify out), x 64, y 64, x2 64, y2 64, o2 64,
-  // qkv 192, attention operand split 192
-  *bytes = (N * (256 + 64 + 64 + 64 + 64 + 64 + 192) + (N + 128) * 224) * sizeof(float);
+  // per token (in floats): big 256 (patches2 / un-patchify out), x 64, x2 64, o2 64, qkv 192, attention operand split 192
+  *bytes = (N * (256 + 64 + 64 + 64 + 192) + (N + 128) * 224) * sizeof(float);
   return MVSF_OK;
 }
 
@@ -185,10 +184,8 @@ int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, c
   float* big = (float*)workspace;                             // [N][256] floats
   __half* big2 = reinterpret_cast<__half*>(big);             // [N][512] halves: row = [hi(256) | lo(256)]
   float* x = big + (size_t)N * 256;                           // [N][64]
-  float* y = x + (size_t)N * 64;                              // [N][64]
-  __half* x2 = reinterpret_cast<__half*>(y + (size_t)N * 64);    // [N][128] = [hi(64) | lo(64)]
-  __half* y2 = x2 + (size_t)N * 128;
-  __half* o2 = y2 + (size_t)N * 128;
+  __half* x2 = reinterpret_cast<__half*>(x + (size_t)N * 64);    // [N][128] = [hi(64) | lo(64)]
+  __half* o2 = x2 + (size_t)N * 128;
   float* qkv = reinterpret_cast<float*>(o2 + (size_t)N * 128);   // [N][192]
   __half* split = reinterpret_cast<__half*>(qkv + (size_t)N * 192);  // [6][4][N][16] fp16
 
@@ -214,20 +211,14 @@ int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, c
     q.M = N; q.N = 192; q.K = 64; q.C = qkv; q.ldc = 192;
     if ((rc = launch_linear_tc(q, LIN_BIAS, s))) return rc;
     if ((rc = run_attention(qkv, nullptr, o2, split, N, scale_log2e, s))) return rc;
-    TcLinArgs p{};
-    p.Ah = o2; p.Al = o2 + 64; p.lda = 128; p.Bh = wh + lo + L_PROJ_W; p.Bl = wl + lo + L_PROJ_W; p.ldb = 64;
-    p.M = N; p.N = 64; p.K = 64; p.bias = lw + L_PROJ_B; p.res = x; p.ldres = 64; p.gamma = lw + L_G1;
-    p.ln_w = lw + L_N1W; p.ln_b = lw + L_N1B; p.ln_eps = 1e-5f; p.C = y; p.ldc = 64; p.C2 = y2; p.ldc2 = 128;
-    if ((rc = launch_linear_tc(p, LIN_RES_LN, s))) return rc;
-    TcLinArgs f1{};
-    f1.Ah = y2; f1.Al = y2 + 64; f1.lda = 128; f1.Bh = wh + lo + L_F1W; f1.Bl = wl + lo + L_F1W; f1.ldb = 64;
-    f1.M = N; f1.N = 256; f1.K = 64; f1.bias = lw + L_F1B; f1.C2 = big2; f1.ldc2 = 512;
-    if ((rc = launch_linear_tc(f1, LIN_GELU, s))) return rc;
-    TcLinArgs f2{};
-    f2.Ah = big2; f2.Al = big2 + 256; f2.lda = 512; f2.Bh = wh + lo + L_F2W; f2.Bl = wl + lo + L_F2W; f2.ldb = 256;
-    f2.M = N; f2.N = 64; f2.K = 256; f2.bias = lw + L_F2B; f2.res = y; f2.ldres = 64; f2.gamma = lw + L_G2;
-    f2.ln_w = lw + L_N2W; f2.ln_b = lw + L_N2B; f2.ln_eps = 1e-5f; f2.C = x; f2.ldc = 64; f2.C2 = x2; f2.ldc2 = 128;
-    if ((rc = launch_linear_tc(f2, LIN_RES_LN, s))) return rc;
+    // y = norm1(x + gamma1 * proj(o)); x = norm2(y + gamma2 * ffn(y)); x2 = split(x)
+    TokenMlpArgs p{};
+    p.A = o2; p.res = x; p.C = x; p.C2 = x2; p.M = N;
+    p.pw_h = wh + lo + L_PROJ_W; p.pw_l = wl + lo + L_PROJ_W; p.f1w_h = wh + lo + L_F1W; p.f1w_l = wl + lo + L_F1W;
+    p.f2w_h = wh + lo + L_F2W; p.f2w_l = wl + lo + L_F2W;
+    p.proj_b = lw + L_PROJ_B; p.gamma1 = lw + L_G1; p.f1_b = lw + L_F1B; p.f2_b = lw + L_F2B; p.gamma2 = lw + L_G2;
+    p.mid_w = lw + L_N1W; p.mid_b = lw + L_N1B; p.mid_eps = 1e-5f; p.out_w = lw + L_N2W; p.out_b = lw + L_N2B; p.out_eps = 1e-5f;
+    if ((rc = launch_token_mlp(p, MLP_POST_NORM, s))) return rc;
   }
   const size_t uo = (size_t)TR_LAYER0 + (size_t)layers * TR_LAYER;
   TcLinArgs u{};

@@ -42,7 +42,7 @@ __global__ void tokens_add_pe_kernel(const float* __restrict__ f, const float* _
 }
 
 struct FmtWs {
-  __half *xn2, *att2, *hid2;   // fp16 hi|lo split activations: [M][128], [M][128], [M][512]
+  __half *xn2, *att2;          // fp16 hi|lo split activations: [M][128], [M][128]
   float *qkv, *ref0, *kvpart, *kvfin, *kvc;
   const __half *wh, *wl;       // fp16 hi / lo parts of the packed weight blob (same indexing as the fp32 blob)
 };
@@ -87,26 +87,15 @@ static int run_block(float* x, int nviews, int L, const float* bw, size_t boff, 
       MVSF_LAUNCH_CHECK("fmt_linattn_apply");
     }
   }
-  TcLinArgs p{};
-  p.Ah = ws.att2; p.Al = ws.att2 + 64; p.lda = 128; p.Bh = ws.wh + boff + B_PW; p.Bl = ws.wl + boff + B_PW; p.ldb = 64;
-  p.M = M; p.N = 64; p.K = 64; p.bias = bw + B_PB; p.res = x; p.ldres = 64; p.gamma = bw + B_G1;
-  p.Cpre = x; p.ldcpre = 64; p.ln_w = bw + B_N2W; p.ln_b = bw + B_N2B; p.ln_eps = 1e-5f; p.C2 = ws.xn2; p.ldc2 = 128;
-  if ((rc = launch_linear_tc(p, LIN_RES_LN, s))) return rc;   // x += gamma1 * proj(...), xn2 = split(norm2(x))
-  TcLinArgs f1{};
-  f1.Ah = ws.xn2; f1.Al = ws.xn2 + 64; f1.lda = 128; f1.Bh = ws.wh + boff + B_F1W; f1.Bl = ws.wl + boff + B_F1W; f1.ldb = 64;
-  f1.M = M; f1.N = 256; f1.K = 64; f1.bias = bw + B_F1B; f1.C2 = ws.hid2; f1.ldc2 = 512;
-  if ((rc = launch_linear_tc(f1, LIN_GELU, s))) return rc;
-  TcLinArgs f2{};
-  f2.Ah = ws.hid2; f2.Al = ws.hid2 + 256; f2.lda = 512; f2.Bh = ws.wh + boff + B_F2W; f2.Bl = ws.wl + boff + B_F2W; f2.ldb = 256;
-  f2.M = M; f2.N = 64; f2.K = 256; f2.bias = bw + B_F2B; f2.res = x; f2.ldres = 64; f2.gamma = bw + B_G2;
-  if (next_bw) {   // x += gamma2 * ffn(...), xn2 = split(norm1_next(x))
-    f2.Cpre = x; f2.ldcpre = 64; f2.ln_w = next_bw + B_N1W; f2.ln_b = next_bw + B_N1B; f2.ln_eps = 1e-5f; f2.C2 = ws.xn2; f2.ldc2 = 128;
-    if ((rc = launch_linear_tc(f2, LIN_RES_LN, s))) return rc;
-  } else {
-    f2.C = x; f2.ldc = 64;
-    if ((rc = launch_linear_tc(f2, LIN_RES, s))) return rc;
-  }
-  return MVSF_OK;
+  // x += gamma1 * proj(...); x += gamma2 * ffn(norm2(x)); xn2 = split(norm1_next(x))
+  TokenMlpArgs p{};
+  p.A = ws.att2; p.res = x; p.C = x; p.C2 = next_bw ? ws.xn2 : nullptr; p.M = M;
+  p.pw_h = ws.wh + boff + B_PW; p.pw_l = ws.wl + boff + B_PW; p.f1w_h = ws.wh + boff + B_F1W; p.f1w_l = ws.wl + boff + B_F1W;
+  p.f2w_h = ws.wh + boff + B_F2W; p.f2w_l = ws.wl + boff + B_F2W;
+  p.proj_b = bw + B_PB; p.gamma1 = bw + B_G1; p.f1_b = bw + B_F1B; p.f2_b = bw + B_F2B; p.gamma2 = bw + B_G2;
+  p.mid_w = bw + B_N2W; p.mid_b = bw + B_N2B; p.mid_eps = 1e-5f;
+  if (next_bw) { p.out_w = next_bw + B_N1W; p.out_b = next_bw + B_N1B; p.out_eps = 1e-5f; }
+  return launch_token_mlp(p, next_bw ? MLP_PRE_NORM : MLP_PRE_NORM_LAST, s);
 }
 
 // K/V summary of a cross layer: key = value = norm1_layer(ref_feature)   (block.py:341-343, FMT.py:121-125)
@@ -245,7 +234,7 @@ int mvsf_fmt_workspace_bytes(int V, int H1, int W1, size_t* bytes) {
   MVSF_REQUIRE(bytes && V >= 2 && H1 > 0 && W1 > 0, "fmt: bad arguments");
   size_t L = (size_t)H1 * W1, VL = (size_t)V * L;
   size_t nblk = (L + KV_CHUNK - 1) / KV_CHUNK;
-  size_t n = 640 * VL + 64 * L + (size_t)V * nblk * KVSZ + (size_t)(V + 2) * KVSZ + 64;
+  size_t n = 320 * VL + 64 * L + (size_t)V * nblk * KVSZ + (size_t)(V + 2) * KVSZ + 64;
   *bytes = n * sizeof(float) + SM_TC;
   return MVSF_OK;
 }
@@ -267,11 +256,10 @@ int mvsf_fmt_forward(const float* f1, const float* f2, const float* f3, const fl
   FmtWs ws;
   ws.xn2 = reinterpret_cast<__half*>(base);                  // [V*L][128] halves (= 64 floats / token)
   ws.qkv = base + 64 * VL;                                   // [V*L][192]
-  ws.att2 = reinterpret_cast<__half*>(ws.qkv + 192 * VL);    // [V*L][128] halves
-  ws.hid2 = ws.att2 + 128 * VL;                              // [V*L][512] halves  (576 VL floats in total; the pathway reuses the first 128 VL)
+  ws.att2 = reinterpret_cast<__half*>(ws.qkv + 192 * VL);    // [V*L][128] halves  (320 VL floats in total; the pathway reuses the first 128 VL)
   ws.wh = reinterpret_cast<const __half*>(wts16);
   ws.wl = ws.wh + n_wts;
-  ws.ref0 = base + 640 * VL;          // [L][64]
+  ws.ref0 = base + 320 * VL;          // [L][64]
   const size_t nblk = (L + KV_CHUNK - 1) / KV_CHUNK;
   ws.kvpart = ws.ref0 + 64 * (size_t)L;
   ws.kvfin = ws.kvpart + (size_t)V * nblk * KVSZ;

@@ -70,6 +70,27 @@ __device__ __forceinline__ void epi_store2(float* crow, __half* c2row, int lo_of
   if (c2row) split_store2(c2row + col, c2row + lo_off + col, t[0], t[1]);
 }
 
+// LayerNorm of a 64-wide row whose values sit in the accumulator layout: 16 per thread (columns 8b + 2q + e, b < 8,
+// e < 2, q = lane & 3), the row spread over the 4 threads of a quad.  Shared by every LayerNorm epilogue, so the fused
+// token MLP and the single GEMMs round alike.
+__device__ __forceinline__ void ln64_stats(const float (&x)[16], float eps, float& mean, float& sd) {
+  float s = 0.f;
+#pragma unroll
+  for (int b = 0; b < 8; ++b) s += x[2 * b] + x[2 * b + 1];
+  s += __shfl_xor_sync(0xffffffffu, s, 1);
+  s += __shfl_xor_sync(0xffffffffu, s, 2);
+  mean = s * (1.0f / 64.0f);
+  float v = 0.f;
+#pragma unroll
+  for (int e = 0; e < 16; ++e) { const float d = x[e] - mean; v = fmaf(d, d, v); }
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  sd = sqrtf(v * (1.0f / 64.0f) + eps);
+}
+__device__ __forceinline__ float ln64_apply(float x, float mean, float sd, const float* w, const float* b, int col) {
+  return __fdiv_rn(x - mean, sd) * __ldg(w + col) + __ldg(b + col);
+}
+
 template <int N, int EPI>
 __device__ __forceinline__ void tc_epilogue(const TcLinArgs& a, const float (&acc)[N / 2], int row0, int lane) {
   const int q = lane & 3;
@@ -82,7 +103,6 @@ __device__ __forceinline__ void tc_epilogue(const TcLinArgs& a, const float (&ac
     __half* c2row = a.C2 ? a.C2 + (size_t)(mvalid ? m : 0) * a.ldc2 : nullptr;
     if constexpr (EPI == LIN_RES_LN || EPI == LIN_LN) {   // N == 64: a row is spread over the 4 threads of a quad
       float x[16];
-      float s = 0.f;
 #pragma unroll
       for (int b = 0; b < 8; ++b) {
         const int col = 8 * b + 2 * q;
@@ -94,28 +114,20 @@ __device__ __forceinline__ void tc_epilogue(const TcLinArgs& a, const float (&ac
           t0 = r2.x + g2.x * t0; t1 = r2.y + g2.y * t1;
         }
         x[2 * b] = t0; x[2 * b + 1] = t1;
-        s += t0 + t1;
       }
       if (a.Cpre && mvalid) {
         float* prow = a.Cpre + (size_t)m * a.ldcpre;
 #pragma unroll
         for (int b = 0; b < 8; ++b) *reinterpret_cast<float2*>(prow + 8 * b + 2 * q) = make_float2(x[2 * b], x[2 * b + 1]);
       }
-      s += __shfl_xor_sync(0xffffffffu, s, 1);
-      s += __shfl_xor_sync(0xffffffffu, s, 2);
-      const float mean = s * (1.0f / 64.0f);
-      float v = 0.f;
-#pragma unroll
-      for (int e = 0; e < 16; ++e) { const float d = x[e] - mean; v = fmaf(d, d, v); }
-      v += __shfl_xor_sync(0xffffffffu, v, 1);
-      v += __shfl_xor_sync(0xffffffffu, v, 2);
-      const float sd = sqrtf(v * (1.0f / 64.0f) + a.ln_eps);
+      float mean, sd;
+      ln64_stats(x, a.ln_eps, mean, sd);
       if (mvalid) {
 #pragma unroll
         for (int b = 0; b < 8; ++b) {
           const int col = 8 * b + 2 * q;
-          const float o0 = __fdiv_rn(x[2 * b] - mean, sd) * __ldg(a.ln_w + col) + __ldg(a.ln_b + col);
-          const float o1 = __fdiv_rn(x[2 * b + 1] - mean, sd) * __ldg(a.ln_w + col + 1) + __ldg(a.ln_b + col + 1);
+          const float o0 = ln64_apply(x[2 * b], mean, sd, a.ln_w, a.ln_b, col);
+          const float o1 = ln64_apply(x[2 * b + 1], mean, sd, a.ln_w, a.ln_b, col + 1);
           if (crow) *reinterpret_cast<float2*>(crow + col) = make_float2(o0, o1);
           if (c2row) split_store2(c2row + col, c2row + N + col, o0, o1);
         }
@@ -312,6 +324,260 @@ int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s) {
     case 128: return launch_tc_n<128>(a, epi, smem, grid, s);
     case 192: return launch_tc_n<192>(a, epi, smem, grid, s);
     default: return launch_tc_n<256>(a, epi, smem, grid, s);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Fused token MLP (launch_token_mlp, TokenMlpArgs in linear_tc.cuh): proj (64 -> 64) + its epilogue, FFN1 (64 -> 256,
+// GELU) and FFN2 (256 -> 64) + its epilogue in one kernel, so neither the LayerNorm split that feeds FFN1 nor the 256-wide
+// hidden layer goes through memory.  Same roles as linear_tc_kernel: one CTA per SM, 128-row tiles, a producer warpgroup
+// streaming the attention output (the A of proj) through a 2-stage cp.async ring, two MMA warpgroups of 64 rows each.
+// All three weight matrices stay resident (hi and lo: 16.3 + 64.3 + 65 KB).  Per warpgroup and tile:
+//   proj from shared memory -> epilogue in registers: the residual of FFN2 stays there, the FFN1 input becomes fp16 hi|lo
+//   register A fragments (an m64n16 accumulator slice is the A fragment of a k16 step, as the attention feeds P);
+//   FFN1 in 4 chunks of 64 hidden columns, each -> bias + GELU -> hi|lo A fragments of FFN2's K-block of that chunk,
+//   accumulated into the one N = 64 FFN2 accumulator; chunk c + 1's FFN1 products run during chunk c's GELU.
+// Every product is the one the three single GEMMs issue, in the same order (lo*hi, hi*lo, hi*hi per k16 step, FFN2
+// K-blocks 0..3 into one accumulator), and every epilogue runs the same arithmetic, so the outputs match those of the
+// three launches bit for bit.
+constexpr int MLP_RING = 2;
+constexpr uint32_t MLP_T64 = tile_bytes(64), MLP_T256 = tile_bytes(256), MLP_TA = tile_bytes(TC_BM);
+constexpr uint32_t MLP_OFF_F1 = 2 * MLP_T64, MLP_OFF_F2 = MLP_OFF_F1 + 2 * MLP_T256, MLP_OFF_A = MLP_OFF_F2 + 8 * MLP_T64,
+                   MLP_OFF_BAR = MLP_OFF_A + MLP_RING * 2 * MLP_TA, MLP_SMEM = MLP_OFF_BAR + 16 * MLP_RING;
+static_assert(MLP_SMEM <= 227 * 1024, "token MLP: resident weights + ring exceed shared memory");
+
+// hi|lo split of the pair (a, b) as two fp16x2 registers, rounded as split_store2 rounds
+__device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __half2 h = __floats2half2_rn(a, b);
+  const float2 hf = __half22float2(h);
+  const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+// D (+)= A * B^T over K = 64 with the three split products per k16 step; A = register fragments [k16 step][4],
+// B = hi tile at b (lo tile b_lo bytes after it), leading byte offset lbo
+__device__ __forceinline__ void mlp_mma_rs(float (&d)[32], const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t b,
+                                           uint32_t b_lo, uint32_t lbo, bool accumulate) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint64_t bh = make_desc(b + 2 * i * lbo, lbo, 128), bl = make_desc(b + b_lo + 2 * i * lbo, lbo, 128);
+    mma_rs_n64(d, al[i], bh, (accumulate || i > 0) ? 1u : 0u);
+    mma_rs_n64(d, ah[i], bl, 1u);
+    mma_rs_n64(d, ah[i], bh, 1u);
+  }
+}
+
+template <int FORM>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+token_mlp_kernel(TokenMlpArgs a) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const uint32_t sP = smem_u32(smem);     // proj W [64][64]: hi tile | lo tile
+  const uint32_t sF1 = sP + MLP_OFF_F1;   // FFN1 W [256][64]: hi tile | lo tile
+  const uint32_t sF2 = sP + MLP_OFF_F2;   // FFN2 W [64][256]: 4 K-blocks x (hi tile | lo tile)
+  const uint32_t sA = sP + MLP_OFF_A;     // ring [MLP_RING][hi tile | lo tile] of the attention output
+  const uint32_t bar_full = sP + MLP_OFF_BAR, bar_empty = bar_full + 8 * MLP_RING;
+
+  if (tid == 0) {
+    for (int i = 0; i < MLP_RING; ++i) { mbar_init(bar_full + 8 * i, TC_NPROD); mbar_init(bar_empty + 8 * i, 2); }
+    fence_barrier_init();
+  }
+  fill_tile<TC_THREADS>(sP, a.pw_h, 64, 64, 64, tid);
+  fill_tile<TC_THREADS>(sP + MLP_T64, a.pw_l, 64, 64, 64, tid);
+  fill_tile<TC_THREADS>(sF1, a.f1w_h, 64, 256, 256, tid);
+  fill_tile<TC_THREADS>(sF1 + MLP_T256, a.f1w_l, 64, 256, 256, tid);
+  for (int kb = 0; kb < 4; ++kb) {
+    fill_tile<TC_THREADS>(sF2 + 2 * kb * MLP_T64, a.f2w_h + kb * TC_BK, 256, 64, 64, tid);
+    fill_tile<TC_THREADS>(sF2 + (2 * kb + 1) * MLP_T64, a.f2w_l + kb * TC_BK, 256, 64, 64, tid);
+  }
+  cp_async_commit_group();
+  cp_async_wait_group<0>();
+  fence_proxy_async();
+  __syncthreads();
+
+  const int ntiles = (a.M + TC_BM - 1) / TC_BM;
+  const int my_tiles = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+
+  if (wg == 0) {
+    // ------------------------------------------------------------------ producer: tile t into stage t % MLP_RING
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    for (int t_it = 0; t_it < my_tiles; ++t_it) {
+      const int m0 = ((int)blockIdx.x + t_it * (int)gridDim.x) * TC_BM, st = t_it % MLP_RING;
+      mbar_wait(bar_empty + 8 * st, (uint32_t)(((t_it / MLP_RING) & 1) ^ 1));   // stage free (first use passes)
+      const uint32_t s0 = sA + st * 2 * MLP_TA;
+      fill_tile<TC_NPROD>(s0, a.A + (size_t)m0 * 128, 128, TC_BM, min(TC_BM, a.M - m0), tid);
+      fill_tile<TC_NPROD>(s0 + MLP_TA, a.A + (size_t)m0 * 128 + 64, 128, TC_BM, min(TC_BM, a.M - m0), tid);
+      cp_async_commit_group();
+      cp_async_wait_group<0>();   // the MMA warpgroups spend a whole tile's MLP on the other stage meanwhile
+      fence_proxy_async();
+      mbar_arrive(bar_full + 8 * st);
+    }
+  } else {
+    // ------------------------------------------------------------------ MMA + epilogue warpgroups
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int half = wg - 1;
+    const int t128 = tid & 127, lane = tid & 31, q = lane & 3;
+    const int row_in_tile = 64 * half + 16 * (t128 >> 5) + (lane >> 2);
+    constexpr uint32_t lbo_a = tile_lbo(TC_BM), lbo64 = tile_lbo(64), lbo256 = tile_lbo(256);
+    for (int t_it = 0; t_it < my_tiles; ++t_it) {
+      const int m0 = ((int)blockIdx.x + t_it * (int)gridDim.x) * TC_BM, st = t_it % MLP_RING;
+      // ---- proj
+      float acc[32];
+      mbar_wait(bar_full + 8 * st, (uint32_t)((t_it / MLP_RING) & 1));
+      const uint32_t sa = sA + st * 2 * MLP_TA + (uint32_t)half * 1024u;
+      wg_fence();
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint64_t ah = make_desc(sa + 2 * i * lbo_a, lbo_a, 128), al = make_desc(sa + MLP_TA + 2 * i * lbo_a, lbo_a, 128);
+        const uint64_t bh = make_desc(sP + 2 * i * lbo64, lbo64, 128), bl = make_desc(sP + MLP_T64 + 2 * i * lbo64, lbo64, 128);
+        mma_ss<64>(acc, al, bh, i > 0 ? 1u : 0u);
+        mma_ss<64>(acc, ah, bl, 1u);
+        mma_ss<64>(acc, ah, bh, 1u);
+      }
+      wg_commit();
+      wg_wait<0>();
+      fence_regs<32>(acc);
+      if (t128 == 0) mbar_arrive(bar_empty + 8 * st);
+      // ---- proj epilogue: r = FFN2's residual (pre-norm: x + gamma1 proj; post-norm: LN_mid of it), the FFN1 input
+      //      (pre-norm: LN_mid(x + gamma1 proj); post-norm: r) as hi|lo A fragments: k16 step b / 2, register 2 (b % 2) + h
+      float r[2][16];
+      uint32_t xh[4][4], xl[4][4];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + row_in_tile + 8 * h;
+        const bool mvalid = m < a.M;
+        const float* resrow = a.res + (size_t)(mvalid ? m : 0) * 64;
+        float x[16];
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+          const int col = 8 * b + 2 * q;
+          const float2 b2 = *reinterpret_cast<const float2*>(a.proj_b + col);
+          const float2 g2 = *reinterpret_cast<const float2*>(a.gamma1 + col);
+          const float2 r2 = mvalid ? *reinterpret_cast<const float2*>(resrow + col) : make_float2(0.f, 0.f);
+          float t0 = acc[4 * b + 2 * h] + b2.x, t1 = acc[4 * b + 2 * h + 1] + b2.y;
+          t0 = r2.x + g2.x * t0; t1 = r2.y + g2.y * t1;
+          x[2 * b] = t0; x[2 * b + 1] = t1;
+        }
+        float mean, sd;
+        ln64_stats(x, a.mid_eps, mean, sd);
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+          const int col = 8 * b + 2 * q;
+          const float o0 = ln64_apply(x[2 * b], mean, sd, a.mid_w, a.mid_b, col);
+          const float o1 = ln64_apply(x[2 * b + 1], mean, sd, a.mid_w, a.mid_b, col + 1);
+          r[h][2 * b] = FORM == MLP_POST_NORM ? o0 : x[2 * b];
+          r[h][2 * b + 1] = FORM == MLP_POST_NORM ? o1 : x[2 * b + 1];
+          split_pack2(o0, o1, xh[b >> 1][2 * (b & 1) + h], xl[b >> 1][2 * (b & 1) + h]);
+        }
+      }
+      // ---- FFN1 chunk c (hidden columns [64c, 64c + 64)) -> GELU -> A fragments of FFN2's K-block c
+      float hid[2][32], acc2[32];
+      uint32_t gh[4][4], gl[4][4];
+      wg_fence();
+      mlp_mma_rs(hid[0], xh, xl, sF1, MLP_T256, lbo256, false);
+      wg_commit();
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        if (c + 1 < 4) {
+          wg_fence();
+          mlp_mma_rs(hid[(c + 1) & 1], xh, xl, sF1 + (c + 1) * 1024u, MLP_T256, lbo256, false);
+          wg_commit();
+          wg_wait<1>();   // FFN1 chunk c and FFN2 K-block c - 1 (whose A fragments are overwritten next) are done
+        } else {
+          wg_wait<0>();
+        }
+        fence_regs<32>(hid[c & 1]);
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+          const float2 b2 = *reinterpret_cast<const float2*>(a.f1_b + 64 * c + 8 * b + 2 * q);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float t0 = hid[c & 1][4 * b + 2 * h] + b2.x, t1 = hid[c & 1][4 * b + 2 * h + 1] + b2.y;
+            t0 = gelu_erf_lean(t0); t1 = gelu_erf_lean(t1);
+            split_pack2(t0, t1, gh[b >> 1][2 * (b & 1) + h], gl[b >> 1][2 * (b & 1) + h]);
+          }
+        }
+        wg_fence();
+        mlp_mma_rs(acc2, gh, gl, sF2 + 2 * c * MLP_T64, MLP_T64, lbo64, c > 0);
+        wg_commit();
+      }
+      wg_wait<0>();
+      fence_regs<32>(acc2);
+      // ---- FFN2 epilogue: x = r + gamma2 (ffn + bias) -> C, and C2 = split(LN_out(x)) (post-norm: C = LN_out(x) too)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + row_in_tile + 8 * h;
+        const bool mvalid = m < a.M;
+        float* crow = a.C + (size_t)(mvalid ? m : 0) * 64;
+        __half* c2row = a.C2 ? a.C2 + (size_t)(mvalid ? m : 0) * 128 : nullptr;
+        float x[16];
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+          const int col = 8 * b + 2 * q;
+          const float2 b2 = *reinterpret_cast<const float2*>(a.f2_b + col);
+          const float2 g2 = *reinterpret_cast<const float2*>(a.gamma2 + col);
+          float t0 = acc2[4 * b + 2 * h] + b2.x, t1 = acc2[4 * b + 2 * h + 1] + b2.y;
+          t0 = r[h][2 * b] + g2.x * t0; t1 = r[h][2 * b + 1] + g2.y * t1;
+          x[2 * b] = t0; x[2 * b + 1] = t1;
+        }
+        if (FORM != MLP_POST_NORM && mvalid) {
+#pragma unroll
+          for (int b = 0; b < 8; ++b) *reinterpret_cast<float2*>(crow + 8 * b + 2 * q) = make_float2(x[2 * b], x[2 * b + 1]);
+        }
+        if constexpr (FORM != MLP_PRE_NORM_LAST) {
+          float mean, sd;
+          ln64_stats(x, a.out_eps, mean, sd);
+          if (mvalid) {
+#pragma unroll
+            for (int b = 0; b < 8; ++b) {
+              const int col = 8 * b + 2 * q;
+              const float o0 = ln64_apply(x[2 * b], mean, sd, a.out_w, a.out_b, col);
+              const float o1 = ln64_apply(x[2 * b + 1], mean, sd, a.out_w, a.out_b, col + 1);
+              if (FORM == MLP_POST_NORM) *reinterpret_cast<float2*>(crow + col) = make_float2(o0, o1);
+              split_store2(c2row + col, c2row + 64 + col, o0, o1);
+            }
+          }
+        }
+      }
+    }
+  }
+}
+
+template <int FORM>
+static int launch_mlp(const TokenMlpArgs& a, int grid, cudaStream_t s) {
+  static DeviceOnce once;
+  const int dev = current_device();
+  if (once.need(dev)) {
+    MVSF_CUDA_OK(cudaFuncSetAttribute(token_mlp_kernel<FORM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MLP_SMEM));
+    once.done(dev);
+  }
+  token_mlp_kernel<FORM><<<grid, TC_THREADS, MLP_SMEM, s>>>(a);
+  MVSF_LAUNCH_CHECK("token_mlp");
+  return MVSF_OK;
+}
+
+// host-side argument checks of launch_token_mlp; touch no device state
+static int check_token_mlp(const TokenMlpArgs& a, int form) {
+  MVSF_REQUIRE(form == MLP_PRE_NORM || form == MLP_PRE_NORM_LAST || form == MLP_POST_NORM, "token_mlp: unknown form %d", form);
+  MVSF_REQUIRE(a.M > 0 && a.A && a.res && a.C && a.pw_h && a.pw_l && a.f1w_h && a.f1w_l && a.f2w_h && a.f2w_l && a.proj_b &&
+                   a.gamma1 && a.mid_w && a.mid_b && a.f1_b && a.f2_b && a.gamma2,
+               "token_mlp: bad arguments");
+  if (form != MLP_PRE_NORM_LAST) MVSF_REQUIRE(a.C2 && a.out_w && a.out_b, "token_mlp: the output LayerNorm needs C2, out_w, out_b");
+  const void* ptrs16[] = {a.A, a.res, a.C, a.C2, a.pw_h, a.pw_l, a.f1w_h, a.f1w_l, a.f2w_h, a.f2w_l,
+                          a.proj_b, a.gamma1, a.f1_b, a.f2_b, a.gamma2};
+  for (const void* p : ptrs16) MVSF_REQUIRE(((uintptr_t)p & 15) == 0, "token_mlp: operands must be 16-byte aligned");
+  return MVSF_OK;
+}
+
+int launch_token_mlp(const TokenMlpArgs& a, int form, cudaStream_t s) {
+  int rc;
+  if ((rc = check_token_mlp(a, form))) return rc;
+  const int ntiles = cdiv(a.M, TC_BM), num_sms = device_sm_count(current_device());
+  const int grid = ntiles < num_sms ? ntiles : num_sms;
+  switch (form) {
+    case MLP_PRE_NORM: return launch_mlp<MLP_PRE_NORM>(a, grid, s);
+    case MLP_PRE_NORM_LAST: return launch_mlp<MLP_PRE_NORM_LAST>(a, grid, s);
+    default: return launch_mlp<MLP_POST_NORM>(a, grid, s);
   }
 }
 
@@ -621,6 +887,35 @@ extern "C" int mvsf_linear_tc_epilogue(int epi, const float* A, int lda, const f
   if ((rc = launch_split_f16(A, lda, A2, 2 * K, M, K, s))) return rc;
   if ((rc = launch_split_f16(W, K, B2, 2 * K, N, K, s))) return rc;
   return launch_linear_tc(a, epi, s);
+}
+
+extern "C" int mvsf_token_mlp_forward(int form, const float* A, const float* res, const float* proj_w, const float* proj_b,
+                                      const float* gamma1, const float* mid_w, const float* mid_b, float mid_eps,
+                                      const float* f1_w, const float* f1_b, const float* f2_w, const float* f2_b,
+                                      const float* gamma2, const float* out_w, const float* out_b, float out_eps, float* C,
+                                      void* C2, void* workspace, size_t workspace_bytes, int M, mvsf_stream_t stream) {
+  MVSF_REQUIRE(A && proj_w && f1_w && f2_w && workspace && M > 0, "token_mlp_forward: null pointer or empty shape");
+  MVSF_REQUIRE(((uintptr_t)A & 15) == 0 && ((uintptr_t)workspace & 15) == 0, "token_mlp_forward: A and workspace must be 16-byte aligned");
+  constexpr size_t NP = 64 * 64, NF = 256 * 64;   // weights of proj, of FFN1 (and of FFN2)
+  const size_t need = ((size_t)M * 128 + 2 * (NP + 2 * NF)) * sizeof(__half);
+  if (workspace_bytes < need) return fail(MVSF_ERR_WORKSPACE, "token_mlp_forward: workspace %zu < %zu bytes", workspace_bytes, need);
+  __half* A2 = reinterpret_cast<__half*>(workspace);
+  __half* wp = A2 + (size_t)M * 128;   // hi | lo of each weight matrix, same indexing as the fp32 matrix
+  __half* w1 = wp + 2 * NP;
+  __half* w2 = w1 + 2 * NF;
+  TokenMlpArgs a{};
+  a.A = A2; a.res = res; a.C = C; a.C2 = reinterpret_cast<__half*>(C2); a.M = M;
+  a.pw_h = wp; a.pw_l = wp + NP; a.f1w_h = w1; a.f1w_l = w1 + NF; a.f2w_h = w2; a.f2w_l = w2 + NF;
+  a.proj_b = proj_b; a.gamma1 = gamma1; a.f1_b = f1_b; a.f2_b = f2_b; a.gamma2 = gamma2;
+  a.mid_w = mid_w; a.mid_b = mid_b; a.mid_eps = mid_eps; a.out_w = out_w; a.out_b = out_b; a.out_eps = out_eps;
+  int rc;
+  if ((rc = check_token_mlp(a, form))) return rc;   // every rejection happens before the first launch
+  cudaStream_t s = (cudaStream_t)stream;
+  if ((rc = launch_split_f16(A, 64, A2, 128, M, 64, s))) return rc;
+  if ((rc = launch_split_blob_f16(proj_w, wp, wp + NP, NP, s))) return rc;
+  if ((rc = launch_split_blob_f16(f1_w, w1, w1 + NF, NF, s))) return rc;
+  if ((rc = launch_split_blob_f16(f2_w, w2, w2 + NF, NF, s))) return rc;
+  return launch_token_mlp(a, form, s);
 }
 
 extern "C" int mvsf_linear_tc_streamed_epilogue(int epi, const float* A, int lda, const float* W, const float* bias,

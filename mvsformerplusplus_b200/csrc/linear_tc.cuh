@@ -23,6 +23,28 @@ struct TcLinArgs {
 
 int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s);
 
+// Token MLP of a transformer block in one kernel: proj (64 -> 64) and its residual + LayerNorm epilogue, FFN1
+// (64 -> 256, GELU), FFN2 (256 -> 64) and its residual epilogue.  With p = proj(A) + proj_b, f = FFN(input):
+//   MLP_PRE_NORM       (FMT block, block.py:344-345):  x = res + gamma1 p;  x += gamma2 f(LN_mid(x));  C = x, C2 = split(LN_out(x))
+//   MLP_PRE_NORM_LAST  (last FMT block):               the same, C = x only
+//   MLP_POST_NORM      (transformer layer, module.py:575-576):  y = LN_mid(res + gamma1 p);  C = LN_out(y + gamma2 f(y)),
+//                                                               C2 = split(C)
+// Rows are dense: A [M][hi(64) | lo(64)] fp16, res and C [M][64] fp32 (C may alias res), C2 [M][hi(64) | lo(64)].
+// Weights (nn.Linear layout, hi and lo parts with rows of stride K): proj [64][64], FFN1 [256][64], FFN2 [64][256].
+enum MlpForm { MLP_PRE_NORM = 0, MLP_PRE_NORM_LAST = 1, MLP_POST_NORM = 2 };
+struct TokenMlpArgs {
+  const __half* A;
+  const float* res;
+  float* C;
+  __half* C2;
+  const __half *pw_h, *pw_l, *f1w_h, *f1w_l, *f2w_h, *f2w_l;
+  const float *proj_b, *gamma1, *f1_b, *f2_b, *gamma2;
+  const float *mid_w, *mid_b, *out_w, *out_b;   // LN_mid, LN_out (out_* unused by MLP_PRE_NORM_LAST)
+  float mid_eps, out_eps;
+  int M;
+};
+int launch_token_mlp(const TokenMlpArgs& a, int form, cudaStream_t s);
+
 // Streamed-weight GEMM (weights too large to stay resident: N, K in the thousands).  N % 64 == 0, K = taps * cin.
 // Row m of A is an implicit-GEMM row: m = (img * H + y) * W + x enumerates an H x W grid per image, and K-block kb reads
 // channels [c, c + 64) of tap t = kb / (cin / 64) at input pixel (y + dy_t, x + dx_t) of the same grid, zero outside it:
