@@ -291,6 +291,32 @@ int mvsf_vit_forward_image(const float* img, int H, int W, const float* pos, con
 int mvsf_vit_attention_forward(const float* qkv, int ldq, float* out, int ldo, void* workspace, size_t workspace_bytes,
                                int n, int N, mvsf_stream_t stream);
 
+/* ---- P1: depth-map fusion, test.py:387-517 (filter_depth / dynamic_filter_depth) over misc/fusion.py:79-165, per
+ *      reference view.  The scene is depths [N][H][W], confs [N][H][W] (fp32, contiguous) and cams [N][2][4][4] (slot 0
+ *      extrinsic, slot 1 [:3][:3] intrinsic); the source views of a reference view are an index list into them.
+ * workspace: (ceil(H W / 256) + 1) ints per reference view; mvsf_fusion_filter leaves in it the exclusive scan of the
+ * survivor counts of the 256-pixel blocks and, in its last int, the view's survivor count, which mvsf_fusion_extract reads.
+ * Bad arguments (null pointer, H W outside [1, 2^31), V outside [1, 16], a view index outside [0, N), method not 0 / 1):
+ * -1; short workspace: -3; nothing launched. */
+int mvsf_fusion_workspace_bytes(int H, int W, size_t* bytes);
+/* The inverses the un-projections need (idx_img2cam / idx_cam2world, fusion.py:23-34, invert per call): cams_inv
+ * [N][2][4][4], slot 0 = E^-1, slot 1 = K^-1 (4x4 with K in its [:3][:3]), fp64 rounded once; NaN if singular. */
+int mvsf_fusion_prepare_cameras(const float* cams, int N, float* cams_inv, mvsf_stream_t stream);
+/* method 0 = pcd: the source-confidence masking of test.py:397-400, get_reproj, vis_filter, ave_fusion (fusion.py:79-112)
+ * and the masks of test.py:402-408 (uses conf, thres_view, thres_disp).  method 1 = dpcd: get_reproj_dynamic,
+ * vis_filter_dynamic (fusion.py:114-165) and the voting of test.py:471-480 (uses conf, dist_base, rel_diff_base).
+ * src: V view indices in HOST memory.  -> mask u8 [H][W] (0 / 1), depth_avg [H][W], workspace as above. */
+int mvsf_fusion_filter(int method, const float* depths, const float* confs, const float* cams, const float* cams_inv, int N,
+                       int ref, const int* src, int V, int H, int W, float conf, float thres_view, float thres_disp,
+                       float dist_base, float rel_diff_base, unsigned char* mask, float* depth_avg, void* workspace,
+                       size_t workspace_bytes, mvsf_stream_t stream);
+/* test.py:410-424 (484-497): the world points of the averaged depth (idx_img2cam + idx_cam2world) and uint8(image * 255)
+ * of the masked pixels, in row-major pixel order.  cam_inv: the reference view's [2][4][4] of cams_inv; image [3][H][W]
+ * fp32 in [0, 1]; xyz [capacity][3], rgb [capacity][3]; survivors beyond capacity are not written. */
+int mvsf_fusion_extract(const unsigned char* mask, const float* depth_avg, const void* workspace, size_t workspace_bytes,
+                        const float* cam_inv, const float* image, float* xyz, unsigned char* rgb, long long capacity, int H,
+                        int W, mvsf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

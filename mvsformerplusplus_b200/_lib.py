@@ -67,6 +67,10 @@ SIGNATURES = {
     "mvsf_vit_forward": ([P] * 8 + [Z, I, I, I, P], I),
     "mvsf_vit_forward_image": ([P, I, I] + [P] * 7 + [Z, I, I, I, P], I),
     "mvsf_vit_attention_forward": ([P, I, P, I, P, Z, I, I, P], I),
+    "mvsf_fusion_workspace_bytes": ([I, I, ctypes.POINTER(Z)], I),
+    "mvsf_fusion_prepare_cameras": ([P, I, P, P], I),
+    "mvsf_fusion_filter": ([I, P, P, P, P, I, I, ctypes.POINTER(I), I, I, I, F, F, F, F, F, P, P, P, Z, P], I),
+    "mvsf_fusion_extract": ([P, P, P, Z, P, P, P, P, ctypes.c_longlong, I, I, P], I),
 }
 
 

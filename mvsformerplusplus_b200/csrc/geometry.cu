@@ -23,34 +23,6 @@ __device__ void compose_P(const float* pm, double P[16]) {
       P[r * 4 + c] = s;
     }
 }
-__device__ bool invert4(const double A[16], double inv[16]) {
-  double a[4][8];
-  for (int r = 0; r < 4; ++r)
-    for (int c = 0; c < 4; ++c) {
-      a[r][c] = A[r * 4 + c];
-      a[r][c + 4] = (r == c) ? 1.0 : 0.0;
-    }
-  for (int col = 0; col < 4; ++col) {
-    int piv = col;
-    double best = fabs(a[col][col]);
-    for (int r = col + 1; r < 4; ++r)
-      if (fabs(a[r][col]) > best) { best = fabs(a[r][col]); piv = r; }
-    if (best == 0.0) return false;
-    if (piv != col)
-      for (int c = 0; c < 8; ++c) { double t = a[col][c]; a[col][c] = a[piv][c]; a[piv][c] = t; }
-    double ip = 1.0 / a[col][col];
-    for (int c = 0; c < 8; ++c) a[col][c] *= ip;
-    for (int r = 0; r < 4; ++r)
-      if (r != col) {
-        double f = a[r][col];
-        if (f != 0.0)
-          for (int c = 0; c < 8; ++c) a[r][c] -= f * a[col][c];
-      }
-  }
-  for (int r = 0; r < 4; ++r)
-    for (int c = 0; c < 4; ++c) inv[r * 4 + c] = a[r][c + 4];
-  return true;
-}
 __global__ void compose_geometry_kernel(const float* __restrict__ proj, int V, float* __restrict__ homs,
                                         float* __restrict__ kinv) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;  // 0 .. V-1 ; thread 0 also writes kinv

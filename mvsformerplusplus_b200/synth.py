@@ -83,6 +83,68 @@ def make_images(V, H, W, seed=2024):
     return (x / x.std(dim=(2, 3), keepdim=True)).contiguous()
 
 
+def _smooth_field(g, H, W, passes):
+    """seeded [H,W] field, binomial low-pass `passes` times, zero mean and unit variance"""
+    x = torch.randn(1, 1, H, W, generator=g, dtype=torch.float64)
+    k = torch.tensor([1.0, 4.0, 6.0, 4.0, 1.0], dtype=torch.float64) / 16.0
+    for _ in range(passes):
+        x = F.conv2d(F.pad(x, (2, 2, 0, 0), mode="replicate"), k.view(1, 1, 1, 5))
+        x = F.conv2d(F.pad(x, (0, 0, 2, 2), mode="replicate"), k.view(1, 1, 5, 1))
+    x = x[0, 0] - x.mean()
+    return x / x.std().clamp_min(1e-12)
+
+
+def make_fusion_scene(N, H, W, seed=77, n_src=4, theta_step=0.12, radius=650.0):
+    """A scene for depth-map fusion (test.py:387-517): N cameras of the look-at ring, the true depth of an analytic
+    surface (a tilted plane with a sphere in front of it) ray-cast per view, then seeded damage so that every decision
+    of the filters goes both ways: smooth depth noise whose amplitude varies from nothing to a few thresholds, blobs of
+    gross outliers, low-confidence regions, zero-depth holes, and a last camera with 1.6 x the focal length, which sees a
+    part of what the others see, so that reprojections leave its image.
+    -> dict(depths [N,H,W], confs [N,H,W], cams [N,2,4,4], images [N,3,H,W] in [0,1] on the k/255 grid, pairs
+    [(ref, [src, ...]), ...] with the n_src nearest views of the ring first, depth_true [N,H,W]); float32, CPU."""
+    g = torch.Generator().manual_seed(seed)
+    order = [VIEW_ORDER[i % len(VIEW_ORDER)] + (i // len(VIEW_ORDER)) * 0.37 for i in range(N)]
+    cams = torch.zeros(N, 2, 4, 4, dtype=torch.float64)
+    depth_true = torch.zeros(N, H, W, dtype=torch.float64)
+    normal = torch.tensor([0.25, 0.12, -1.0], dtype=torch.float64)
+    normal = normal / normal.norm()
+    on_plane = torch.tensor([0.0, 0.0, radius + 30.0], dtype=torch.float64)
+    centre, rad = torch.tensor([25.0, -15.0, radius], dtype=torch.float64), 0.18 * radius * W / 1536.0 * 1536.0 / 2776.6
+    ys, xs = torch.meshgrid(torch.arange(H, dtype=torch.float64) + 0.5, torch.arange(W, dtype=torch.float64) + 0.5, indexing="ij")
+    pix = torch.stack([xs, ys, torch.ones_like(xs)], -1)
+    for i in range(N):
+        E, K = lookat_camera(order[i], H, W, radius=radius, theta_step=theta_step,
+                             focal_full=2776.6 * (1.6 if i == N - 1 and N > 2 else 1.0))
+        cams[i, 0], cams[i, 1, :3, :3], cams[i, 1, 3, 3] = E, K, 1.0
+        R, t = E[:3, :3], E[:3, 3]
+        C = -R.T @ t
+        d = (pix @ torch.linalg.inv(K).T) @ R            # world direction of unit camera depth
+        plane = ((on_plane - C) @ normal) / (d @ normal)
+        oc = C - centre
+        a, b, c = (d * d).sum(-1), 2.0 * (d @ oc), oc @ oc - rad * rad
+        disc = b * b - 4.0 * a * c
+        sphere = torch.where(disc > 0, (-b - disc.clamp_min(0).sqrt()) / (2.0 * a), torch.full_like(a, float("inf")))
+        sphere = torch.where(sphere > 0, sphere, torch.full_like(a, float("inf")))
+        depth_true[i] = torch.minimum(plane, sphere)
+    depths, confs = depth_true.clone(), torch.zeros(N, H, W, dtype=torch.float64)
+    images = torch.zeros(N, 3, H, W, dtype=torch.float64)
+    for i in range(N):
+        amp = (0.006 * (_smooth_field(g, H, W, 6) + 0.6)).clamp_min(0.0)          # relative; thresholds are 0.0015 .. 0.01
+        depths[i] *= 1.0 + amp * _smooth_field(g, H, W, 2)
+        blobs = _smooth_field(g, H, W, 5) > 1.5
+        depths[i] = torch.where(blobs, depths[i] * (1.0 + 0.08 * _smooth_field(g, H, W, 3)), depths[i])
+        confs[i] = (0.72 + 0.3 * _smooth_field(g, H, W, 4) + 0.05 * torch.randn(H, W, generator=g, dtype=torch.float64)).clamp(0.0, 1.0)
+        depths[i] = torch.where(_smooth_field(g, H, W, 4) > 1.9, torch.zeros_like(depths[i]), depths[i])
+        for c in range(3):
+            images[i, c] = torch.round((0.5 + 0.25 * _smooth_field(g, H, W, 3)).clamp(0.0, 1.0) * 255.0)
+    pairs = []
+    for i in range(N):
+        others = sorted((j for j in range(N) if j != i), key=lambda j: (abs(order[j] - order[i]), j))
+        pairs.append((i, others[:n_src]))
+    return dict(depths=depths.float(), confs=confs.float(), cams=cams.float(), images=(images.float() / 255.0), pairs=pairs,
+                depth_true=depth_true.float())
+
+
 def randomize_state_dict(module, seed=7, prob_gain=1.0):
     """Seeded re-initialisation of a parameter container (params.build_hotpath_params or the
     reference modules themselves - same key names): seeded normal weights (1/sqrt(fan_in)), randomised BatchNorm
