@@ -81,20 +81,16 @@ int mvsf_position3d(const float* kinv_ref, const float* depth, const float* dept
 int mvsf_homo_warp(const float* src_nhwc, const float* hom, const float* depth, float* warped, uint8_t* mask, int C,
                    int D, int H, int W, mvsf_stream_t stream);
 
-/* ---- test / measurement hooks: the cost-volume passes have two organisations computing the same function - L1 gathers
+/* ---- test seam: the cost-volume passes have two organisations computing the same function - L1 gathers
  * from global memory (warp_corr.cu, any C in 8/16/32/64) and TMA-staged shared-memory windows (warp_tile.cu, C = 8/16, even H).
- * mode 0: force the L1 organisation everywhere; 1 (default): adaptive - the window kernels of the two-gather plan where they
- * apply, and for mvsf_warp_corr_entropy_store at C = 8, D = 4 a per-call choice made ON THE DEVICE from the call's own
- * geometry (share of sampled taps that miss the pipeline kernel's predicted windows <= max_window_miss per mille ->
- * pipeline kernel, else L1 kernel; both are launched, the one not chosen returns at once); 2: force the window / pipeline
- * kernels wherever they exist.  mvsf_warp_corr_last_selection reads the most recent decision back (synchronises). */
+ * mode 0: force the L1 organisation everywhere (the tests' same-input reference); 1 (default): adaptive - the window kernels
+ * of the two-gather plan where they apply, and for mvsf_warp_corr_entropy_store at C = 8, D = 4 a per-call choice made ON
+ * THE DEVICE from the call's own geometry (share of sampled taps that miss the pipeline kernel's predicted windows <= 60 per
+ * mille -> pipeline kernel, else L1 kernel; both are launched, the one not chosen returns at once); 2: force the window /
+ * pipeline kernels wherever they exist (the only way a wide-baseline call reaches the pipeline kernel's out-of-window
+ * fallback).  mvsf_warp_corr_last_selection reads the most recent decision back (synchronises). */
 int mvsf_warp_corr_set_tile_path(int mode);
-int mvsf_warp_corr_set_max_window_miss(int permille);
 int mvsf_warp_corr_last_selection(int* used_pipeline, int* miss_permille);
-
-/* ---- measurement hook: 1 = prefer the largest shared-memory carve-out for every kernel of the context (cudaDeviceSetCacheConfig),
- * 0 = driver default. */
-int mvsf_set_prefer_shared_carveout(int on);
 
 /* ---- which of the two cost-volume plans to run for a stage shape: 1 = two gathers (mvsf_warp_corr_entropy, mvsf_vis_cnn,
  * mvsf_warp_corr_aggregate; no intermediate buffer), 0 = spill plan (mvsf_warp_corr_entropy_store, mvsf_vis_cnn,
@@ -106,10 +102,6 @@ int mvsf_warp_corr_plan(int C, int G, int D, int H, int W, int V, size_t spill_b
  * -> entropy [(V-1)][H][W].   The (V-1,C,D,H,W) warped volume is never written. */
 int mvsf_warp_corr_entropy(const float* feat, const float* homs, const float* depth, float* entropy, int V, int C,
                            int G, int D, int H, int W, mvsf_stream_t stream);
-/* ---- precision of the layer-2/3 activations inside the visibility CNN: 1 (default) = fp16 hi + lo (fp32-class),
- * 0 = fp16 (half the tensor-core instructions; measured against the oracle in tests/test_gpu_parity.py). */
-int mvsf_vis_cnn_set_precision(int x_lo);
-
 /* ---- W4 visibility CNN: models/cost_volume.py:37,93.  entropy [N][H][W] -> vis [N][H][W].
  * wts: packed, BN folded: w1[9][16] b1[16] w2[16 ic][9][16 oc] b2[16] w3[16 ic][9][8 oc] b3[8] w4[8] b4[1] (=3649 floats) */
 int mvsf_vis_cnn(const float* entropy, const float* wts, float* vis, int N, int H, int W, mvsf_stream_t stream);
@@ -164,16 +156,15 @@ int mvsf_attention_forward(const float* qkv, float* out, void* workspace, size_t
  * when every item runs whole.  Host only. */
 int mvsf_attention_split_plan(int N, int num_sms, int* split_items, int* parts);
 
-/* token-wise linear layer alone (nn.Linear, e.g. models/module.py:520-522 FFN.linear1): C[M,N] = act(A[M,K] W[N,K]^T + bias)
- * on the wgmma tensor cores with fp16 hi/lo split operands (fp32-class accuracy).  N in {16, 64, 128, 192, 256}, K % 64 == 0.
- * workspace >= (M+N)*2K*2 + 256 bytes.  gelu != 0 applies the exact-erf GELU. */
-int mvsf_linear_tc_forward(const float* A, const float* W, const float* bias, float* C, void* workspace,
-                           size_t workspace_bytes, int M, int N, int K, int gelu, mvsf_stream_t stream);
-/* test seam: the same layer with any of its fused epilogues, as FMT and the transformer regulariser call it.
- * epi: 0 C = acc + bias, 1 C = gelu(acc + bias), 2 C = col < elu_cols ? elu(acc + bias) + 1 : acc + bias,
+/* test seam: a token-wise linear layer (nn.Linear) with one of its fused epilogues, as FMT and the transformer regulariser
+ * call it: C[M,N] = epi(A[M,K] W[N,K]^T + bias) on the wgmma tensor cores with fp16 hi/lo split operands (fp32-class
+ * accuracy), weights resident in shared memory, K % 64 == 0.
+ * epi: 0 C = acc + bias, 1 C = gelu(acc + bias) (exact erf), 2 C = col < elu_cols ? elu(acc + bias) + 1 : acc + bias,
  * 3 C = res + gamma * (acc + bias), 4 C = LN(res + gamma * (acc + bias)), 5 C = LN(acc + bias); LN = LayerNorm over
- * the row with ln_w, ln_b, ln_eps (epilogues 4 and 5 need N == 64).  A [M][lda] and W [N][K] are fp32 and split into
- * fp16 hi/lo parts inside the call.  bias [N] may be NULL; res [M][ldres] and gamma [N] are read by epilogues 3 and 4.
+ * the row with ln_w, ln_b, ln_eps.  Only the (N, epi) pairs that FMT and the transformer regulariser run, and the single
+ * GEMMs mvsf_token_mlp_forward is compared against, are built (kTcPairs in csrc/linear_tc.cu); any other pair is -1.
+ * A [M][lda] and W [N][K] are fp32 and split into fp16 hi/lo parts inside the call.  bias [N] may be NULL;
+ * res [M][ldres] and gamma [N] are read by epilogues 3 and 4.
  * Outputs, each optional (C or C2 required): C [M][ldc] fp32; Cpre [M][ldcpre] = the value before the LayerNorm
  * (epilogues 4 and 5 only, may alias res); C2 [M][ldc2] fp16 = [hi(N) | lo(N)] split of C per row.
  * Operands and outputs 16-byte aligned.  workspace >= (M+N)*2K*2 + 256 bytes. */

@@ -22,12 +22,9 @@ SIGNATURES = {
     "mvsf_position3d": ([P, P, P, I, P, I, P, I, I, I, P], I),
     "mvsf_homo_warp": ([P, P, P, P, P, I, I, I, I, P], I),
     "mvsf_warp_corr_set_tile_path": ([I], I),
-    "mvsf_warp_corr_set_max_window_miss": ([I], I),
-    "mvsf_set_prefer_shared_carveout": ([I], I),
     "mvsf_warp_corr_last_selection": ([ctypes.POINTER(I), ctypes.POINTER(I)], I),
     "mvsf_warp_corr_plan": ([I, I, I, I, I, I, Z], I),
     "mvsf_warp_corr_entropy": ([P, P, P, P, I, I, I, I, I, I, P], I),
-    "mvsf_vis_cnn_set_precision": ([I], I),
     "mvsf_vis_cnn": ([P, P, P, I, I, I, P], I),
     "mvsf_warp_corr_aggregate": ([P, P, P, P, P, I, I, I, I, I, I, P], I),
     "mvsf_warp_corr_entropy_store": ([P, P, P, P, P, I, I, I, I, I, I, P], I),
@@ -42,7 +39,6 @@ SIGNATURES = {
     "mvsf_split_weights_f16": ([P, P, Z, P], I),
     "mvsf_attention_forward": ([P, P, P, Z, I, F, P], I),
     "mvsf_attention_split_plan": ([I, I, ctypes.POINTER(I), ctypes.POINTER(I)], I),
-    "mvsf_linear_tc_forward": ([P, P, P, P, P, Z, I, I, I, I, P], I),
     "mvsf_linear_tc_epilogue": ([I, P, I, P, P, P, I, P, P, P, F, I, P, I, P, I, P, I, P, Z, I, I, I, P], I),
     "mvsf_softargmax": ([P, P, F, P, P, P, I, I, I, P], I),
     "mvsf_conf_accumulate": ([P, I, I, P, I, I, F, I, P], I),
@@ -87,14 +83,6 @@ def lib():
             fn = getattr(L, name)  # AttributeError if the symbol is not exported
             fn.argtypes = argt
             fn.restype = rest
-        if os.environ.get("MVSF_VIS_XLO") in ("0", "1"):   # A-B measurements of the vis-CNN activation precision
-            L.mvsf_vis_cnn_set_precision(int(os.environ["MVSF_VIS_XLO"]))
-        if os.environ.get("MVSF_WARP_TILE", "1") in ("0", "2"):   # A-B measurements: 0 force the L1-gather kernels, 2 force the window kernels
-            L.mvsf_warp_corr_set_tile_path(int(os.environ["MVSF_WARP_TILE"]))
-        if os.environ.get("MVSF_PREFER_SHARED") in ("0", "1"):   # measurement: one shared-memory carve-out for every kernel
-            L.mvsf_set_prefer_shared_carveout(int(os.environ["MVSF_PREFER_SHARED"]))
-        if os.environ.get("MVSF_WT_MAX_MISS"):
-            L.mvsf_warp_corr_set_max_window_miss(int(os.environ["MVSF_WT_MAX_MISS"]))
         _lib = L
     return _lib
 
@@ -124,8 +112,7 @@ class profile_calls:
         for name in SIGNATURES:
             if name.endswith("_workspace_bytes") or name in ("mvsf_abi_version", "mvsf_launch_count", "mvsf_ktimer_enable",
                                                              "mvsf_ktimer_read", "mvsf_warp_corr_plan", "mvsf_attention_split_plan",
-                                                             "mvsf_warp_corr_set_tile_path", "mvsf_warp_corr_set_max_window_miss", "mvsf_set_prefer_shared_carveout",
-                                                             "mvsf_warp_corr_last_selection", "mvsf_vis_cnn_set_precision"):
+                                                             "mvsf_warp_corr_set_tile_path", "mvsf_warp_corr_last_selection"):
                 continue
             fn = getattr(L, name)
             self._orig[name] = fn

@@ -98,13 +98,6 @@ __global__ void transpose_hwc_chw_kernel(const float* __restrict__ src, float* _
 
 extern "C" {
 
-/* measurement hook (two-stream deadlock, DESIGN.md 5 / 9): ask the driver for the largest shared-memory carve-out for every
- * kernel of this context, so that an SM never has to switch carve-outs between CTAs of different kernels */
-int mvsf_set_prefer_shared_carveout(int on) {
-  MVSF_CUDA_OK(cudaDeviceSetCacheConfig(on ? cudaFuncCachePreferShared : cudaFuncCachePreferNone));
-  return MVSF_OK;
-}
-
 const char* mvsf_last_error(void) { return mvsf::g_err; }
 int mvsf_abi_version(void) { return 1; }
 long long mvsf_launch_count(int reset) {

@@ -12,6 +12,8 @@
 // Used by the stage-1 transformer regulariser (module.py:507-646) and FMT (FMT.py, block.py:336-346).
 #include "linear_tc.cuh"
 
+#include <utility>
+
 #include "wgmma.cuh"
 
 namespace mvsf {
@@ -273,28 +275,35 @@ static int launch_tc(const TcLinArgs& a, size_t smem, int grid, cudaStream_t s) 
   return MVSF_OK;
 }
 
-template <int N>
-static int launch_tc_n(const TcLinArgs& a, int epi, size_t smem, int grid, cudaStream_t s) {
-  switch (epi) {
-    case LIN_BIAS: return launch_tc<N, LIN_BIAS>(a, smem, grid, s);
-    case LIN_GELU: return launch_tc<N, LIN_GELU>(a, smem, grid, s);
-    case LIN_ELU1: return launch_tc<N, LIN_ELU1>(a, smem, grid, s);
-    case LIN_RES: return launch_tc<N, LIN_RES>(a, smem, grid, s);
-    default: break;
-  }
-  if constexpr (N == 64) {
-    if (epi == LIN_RES_LN) return launch_tc<64, LIN_RES_LN>(a, smem, grid, s);
-    if (epi == LIN_LN) return launch_tc<64, LIN_LN>(a, smem, grid, s);
-  }
-  return fail(MVSF_ERR_INVALID, "linear_tc: unknown epilogue %d", epi);
+// The (N, epilogue) pairs linear_tc_kernel is built for, and the only ones launch_linear_tc accepts: those the transformer
+// regulariser (costreg_tr.cu) and FMT (fmt.cu) run, and the single GEMMs the fused token MLP is compared against bit for bit
+// (tests/test_gpu_token_mlp.py).
+struct TcPair { int n, epi; };
+constexpr TcPair kTcPairs[] = {
+    {64, LIN_LN}, {192, LIN_BIAS}, {256, LIN_BIAS},      // transformer regulariser
+    {192, LIN_ELU1}, {64, LIN_ELU1}, {128, LIN_ELU1},    // FMT
+    {64, LIN_RES_LN}, {256, LIN_GELU}, {64, LIN_RES}};   // token MLP reference
+constexpr size_t kNumTcPairs = sizeof(kTcPairs) / sizeof(kTcPairs[0]);
+
+static bool tc_pair_built(int n, int epi) {
+  for (const TcPair& p : kTcPairs)
+    if (p.n == n && p.epi == epi) return true;
+  return false;
+}
+
+template <size_t... I>
+static int launch_tc_pair(const TcLinArgs& a, int epi, size_t smem, int grid, cudaStream_t s, std::index_sequence<I...>) {
+  int rc = MVSF_ERR_INVALID;   // not reached: check_linear_tc admits built pairs only
+  ((a.N == kTcPairs[I].n && epi == kTcPairs[I].epi &&
+    (rc = launch_tc<kTcPairs[I].n, kTcPairs[I].epi>(a, smem, grid, s), true)) || ...);
+  return rc;
 }
 
 // host-side argument checks of launch_linear_tc; touch no device state, so callers can run them before any launch
 static int check_linear_tc(const TcLinArgs& a, int epi) {
   MVSF_REQUIRE(epi >= LIN_BIAS && epi <= LIN_LN, "linear_tc: unknown epilogue %d", epi);
   MVSF_REQUIRE(a.Ah && a.Al && a.Bh && a.Bl && (a.C || a.C2) && a.M > 0, "linear_tc: bad arguments");
-  MVSF_REQUIRE((a.N == 16 || a.N == 64 || a.N == 128 || a.N == 192 || a.N == 256) && a.K % TC_BK == 0 && a.K >= TC_BK,
-               "linear_tc: need N in {16, 64, 128, 192, 256}, K %% 64 == 0");
+  MVSF_REQUIRE(a.K % TC_BK == 0 && a.K >= TC_BK, "linear_tc: need K %% 64 == 0");
   MVSF_REQUIRE((a.lda % 8) == 0 && (a.ldb % 8) == 0 && ((uintptr_t)a.Ah & 15) == 0 && ((uintptr_t)a.Al & 15) == 0 &&
                    ((uintptr_t)a.Bh & 15) == 0 && ((uintptr_t)a.Bl & 15) == 0, "linear_tc: operands must be 16-byte aligned");
   if (a.C) MVSF_REQUIRE((a.ldc % 4) == 0 && ((uintptr_t)a.C & 15) == 0, "linear_tc: C must be 16-byte aligned");
@@ -306,6 +315,8 @@ static int check_linear_tc(const TcLinArgs& a, int epi) {
   if (a.bias) MVSF_REQUIRE(((uintptr_t)a.bias & 15) == 0, "linear_tc: bias must be 16-byte aligned");
   if (a.Cpre) MVSF_REQUIRE((epi == LIN_RES_LN || epi == LIN_LN) && (a.ldcpre % 4) == 0 && ((uintptr_t)a.Cpre & 15) == 0,
                            "linear_tc: Cpre needs a LayerNorm epilogue and 16-byte alignment");
+  MVSF_REQUIRE(tc_pair_built(a.N, epi), "linear_tc: no kernel for (N = %d, epilogue %d); need N in a built pair (kTcPairs)",
+               a.N, epi);
   const size_t smem = tc_smem_bytes(a.N, a.K);
   MVSF_REQUIRE(smem <= 227 * 1024, "linear_tc: N*K too large for resident weights (%zu bytes of shared memory)", smem);
   return MVSF_OK;
@@ -318,13 +329,7 @@ int launch_linear_tc(const TcLinArgs& a, int epi, cudaStream_t s) {
   const int num_sms = device_sm_count(current_device());
   const int ntiles = cdiv(a.M, TC_BM);
   const int grid = ntiles < num_sms ? ntiles : num_sms;  // persistent: one CTA per SM, tiles strided by gridDim.x
-  switch (a.N) {
-    case 16: return launch_tc_n<16>(a, epi, smem, grid, s);
-    case 64: return launch_tc_n<64>(a, epi, smem, grid, s);
-    case 128: return launch_tc_n<128>(a, epi, smem, grid, s);
-    case 192: return launch_tc_n<192>(a, epi, smem, grid, s);
-    default: return launch_tc_n<256>(a, epi, smem, grid, s);
-  }
+  return launch_tc_pair(a, epi, smem, grid, s, std::make_index_sequence<kNumTcPairs>{});
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -845,23 +850,6 @@ int launch_split_f16(const float* x, int ldx, __half* out, int ldo, int M, int K
 }  // namespace mvsf
 
 using namespace mvsf;
-
-extern "C" int mvsf_linear_tc_forward(const float* A, const float* W, const float* bias, float* C, void* workspace,
-                                      size_t workspace_bytes, int M, int N, int K, int gelu, mvsf_stream_t stream) {
-  MVSF_REQUIRE(A && W && C && workspace, "linear_tc_forward: null pointer");
-  const size_t need = ((size_t)M * 2 * K + (size_t)N * 2 * K) * sizeof(__half) + 256;
-  if (workspace_bytes < need) return fail(MVSF_ERR_WORKSPACE, "linear_tc_forward: workspace %zu < %zu bytes", workspace_bytes, need);
-  cudaStream_t s = (cudaStream_t)stream;
-  __half* A2 = reinterpret_cast<__half*>(workspace);
-  __half* B2 = A2 + align_up((size_t)M * 2 * K, 64);
-  int rc;
-  if ((rc = launch_split_f16(A, K, A2, 2 * K, M, K, s))) return rc;
-  if ((rc = launch_split_f16(W, K, B2, 2 * K, N, K, s))) return rc;
-  TcLinArgs a{};
-  a.Ah = A2; a.Al = A2 + K; a.lda = 2 * K; a.Bh = B2; a.Bl = B2 + K; a.ldb = 2 * K;
-  a.M = M; a.N = N; a.K = K; a.bias = bias; a.C = C; a.ldc = N;
-  return launch_linear_tc(a, gelu ? LIN_GELU : LIN_BIAS, s);
-}
 
 extern "C" int mvsf_linear_tc_epilogue(int epi, const float* A, int lda, const float* W, const float* bias,
                                        const float* res, int ldres, const float* gamma, const float* ln_w,

@@ -388,7 +388,7 @@ using namespace mvsf;
 // test hook: 0 forces the L1-gather organisation (warp_corr.cu) for every shape, 1 (default) lets C = 8 / 16 stages use
 // the TMA-staged window kernels (warp_tile.cu).  Both compute the same function; tests compare them.
 static int g_use_tile = 1;            // 0: L1-gather kernels everywhere, 1: adaptive (default), 2: window / pipeline kernels wherever they exist
-static int g_max_miss_permille = 60;  // adaptive choice: the pipeline kernel serves a call when <= this share of the sampled taps miss its window
+constexpr int kMaxMissPermille = 60;  // adaptive choice: the pipeline kernel serves a call when <= this share of the sampled taps miss its window
 
 // Selection slots of the adaptive pass-A choice: 8 ints per call (decision, miss share, 3 scratch counters), a ring per device so that calls in
 // flight on different streams do not share a slot.  Allocated on the first call (like the kernels' attribute set-up).
@@ -418,11 +418,6 @@ extern "C" {
 
 int mvsf_warp_corr_set_tile_path(int enable) {
   g_use_tile = enable < 0 ? 0 : (enable > 2 ? 2 : enable);
-  return MVSF_OK;
-}
-int mvsf_warp_corr_set_max_window_miss(int permille) {
-  MVSF_REQUIRE(permille >= 0 && permille <= 1000, "warp_corr_set_max_window_miss: 0..1000");
-  g_max_miss_permille = permille;
   return MVSF_OK;
 }
 int mvsf_warp_corr_last_selection(int* used_pipeline, int* miss_permille) {
@@ -480,14 +475,14 @@ static int warp_corr_entropy_impl(const float* feat, const float* homs, const fl
   // L1 kernel: the pipeline was not faster on either workload (DTU 0.345 vs 0.336 ms, T&T 1.88 vs 0.94 ms).
   const bool pipeline = corr && g_use_tile && warp_stream_store_supported(feat, corr, C, G, D, H, W);
   if (pipeline && g_use_tile == 2) {   // forced
-    int rc = warp_stream_entropy_store(feat, homs, depth, entropy, corr, V, H, W, nullptr, g_max_miss_permille, s);
+    int rc = warp_stream_entropy_store(feat, homs, depth, entropy, corr, V, H, W, nullptr, kMaxMissPermille, s);
     if (rc) return rc;
     MVSF_LAUNCH_CHECK("warp_stream_entropy_store");
     return MVSF_OK;
   }
   int* select = pipeline ? select_slot() : nullptr;
   if (select) {   // adaptive: the selection kernel, the pipeline kernel and the L1 kernel; the one not chosen returns at once
-    int rc = warp_stream_entropy_store(feat, homs, depth, entropy, corr, V, H, W, select, g_max_miss_permille, s);
+    int rc = warp_stream_entropy_store(feat, homs, depth, entropy, corr, V, H, W, select, kMaxMissPermille, s);
     if (rc) return rc;
     count_launch();   // the selection kernel
     MVSF_LAUNCH_CHECK("warp_stream_entropy_store");

@@ -15,10 +15,17 @@ def P(t):
     return ctypes.c_void_p(t.data_ptr())
 
 
-@pytest.mark.parametrize("M,N,K,gelu", [(128, 64, 64, 0), (300, 64, 64, 0), (1000, 256, 64, 1), (513, 64, 256, 0),
-                                         (27648, 192, 64, 0), (27648, 64, 256, 1), (130, 16, 128, 0),
-                                         (110592, 64, 64, 0), (110592, 256, 64, 1)])   # 6 tiles per persistent CTA
-def test_linear_tc_vs_fp64(M, N, K, gelu):
+BIAS, GELU, ELU1, RES, RES_LN, LN = range(6)
+EPI_NAMES = ["bias", "gelu", "elu1", "res", "res_ln", "ln"]
+# The cases use the (N, epilogue) pairs the library builds (kTcPairs in linear_tc.cu).  Bias-only products whose weights
+# fit no N that BIAS is built for (K = 256) run as ELU1 with elu_cols = 0: the same arithmetic.
+LINEAR_CASES = [(128, 192, 64, BIAS), (300, 192, 64, BIAS), (1000, 256, 64, GELU), (513, 64, 256, ELU1),
+                (27648, 192, 64, BIAS), (27648, 256, 64, GELU), (130, 192, 128, BIAS), (110592, 192, 64, BIAS),
+                (110592, 256, 64, GELU)]   # 110 592 rows: 6 tiles per persistent CTA
+
+
+@pytest.mark.parametrize("M,N,K,epi", LINEAR_CASES, ids=[f"{EPI_NAMES[e]}-M{M}-N{N}-K{K}" for M, N, K, e in LINEAR_CASES])
+def test_linear_tc_vs_fp64(M, N, K, epi):
     from mvsformerplusplus_b200 import _lib
     L = _lib.lib()
     dev = torch.device("cuda:0")
@@ -29,9 +36,11 @@ def test_linear_tc_vs_fp64(M, N, K, gelu):
     C = torch.full((M, N), float("nan"), device=dev)
     ws = torch.empty(((M + N) * 2 * K * 2 + 1024) // 4 + 64, device=dev)
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    _lib.check(L.mvsf_linear_tc_forward(P(A), P(W), P(b), P(C), P(ws), ctypes.c_size_t(ws.numel() * 4), M, N, K, gelu, st),
-               "linear_tc_forward")
+    NP = ctypes.c_void_p(None)
+    _lib.check(L.mvsf_linear_tc_epilogue(epi, P(A), K, P(W), P(b), NP, 0, NP, NP, NP, 1e-5, 0, P(C), N, NP, 0, NP, 0,
+                                         P(ws), ctypes.c_size_t(ws.numel() * 4), M, N, K, st), "linear_tc_epilogue")
     torch.cuda.synchronize()
+    gelu = epi == GELU
     want = A.double() @ W.double().t() + b.double()
     if gelu:
         want = torch.nn.functional.gelu(want)
@@ -43,7 +52,7 @@ def test_linear_tc_vs_fp64(M, N, K, gelu):
     from tests.common import REPORT_DIR
     os.makedirs(REPORT_DIR, exist_ok=True)
     with open(os.path.join(REPORT_DIR, "linear_tc_report.jsonl"), "a") as f:
-        f.write(json.dumps(dict(M=M, N=N, K=K, gelu=gelu, tc_vs_f64=err, torch_f32_vs_f64=err32, scale=float(want.abs().max()))) + "\n")
+        f.write(json.dumps(dict(M=M, N=N, K=K, epi=epi, tc_vs_f64=err, torch_f32_vs_f64=err32, scale=float(want.abs().max()))) + "\n")
     assert err < 5e-6 * max(1.0, float(want.abs().max()))
 
 
@@ -51,30 +60,29 @@ def test_linear_tc_vs_fp64(M, N, K, gelu):
 #      (costreg_tr.cu) call them: strided outputs in NaN-filled buffers with spare rows and columns, the fp16 hi|lo
 #      output C2 that feeds the next GEMM, and M chosen so that tiles are partial, a MMA warpgroup has no valid row or
 #      only one, and a persistent CTA runs a second tile ("wave": M = SMs * 128 + 1).
-BIAS, GELU, ELU1, RES, RES_LN, LN = range(6)
 # |out - fp64| <= EPI_TOL * max(1, max|fp64|), for C, Cpre and hi + lo of C2.  Measured on an H100: at most 1.5e-6; a
 # dropped lo operand product or a lost lo half of C2 costs >= 1.8e-4
 EPI_TOL = 5e-6
 EPI_CASES = [
     # epi, N, K, M, bias, outputs, elu_cols / ln_eps
-    (BIAS, 16, 64, 1, True, "C", None),
-    (BIAS, 16, 256, "wave", False, "C+C2", None),
-    (BIAS, 64, 128, 65, False, "C+C2", None),
-    (BIAS, 64, 64, 110592, True, "C", None),
-    (BIAS, 128, 128, 127, True, "C2", None),
-    (BIAS, 128, 64, "wave", False, "C", None),
+    (BIAS, 192, 64, 1, True, "C", None),
+    (ELU1, 64, 256, "wave", False, "C+C2", 0),   # elu_cols = 0: the BIAS arithmetic
+    (BIAS, 192, 128, 65, False, "C+C2", None),
+    (BIAS, 192, 64, 110592, True, "C", None),
+    (BIAS, 192, 128, 127, True, "C2", None),
+    (BIAS, 192, 64, "wave", False, "C", None),
     (BIAS, 192, 128, 1000, False, "C+C2", None),
     (BIAS, 192, 64, 129, True, "C", None),
     (BIAS, 256, 64, 65, False, "C", None),
     (BIAS, 256, 64, "wave", True, "C+C2", None),
-    (ELU1, 16, 64, 65, False, "C+C2", 9),
+    (ELU1, 64, 64, 65, False, "C+C2", 9),
     (ELU1, 64, 256, 1, False, "C", 64),
     (ELU1, 64, 128, 1000, True, "C+C2", 37),
     (ELU1, 128, 64, 110592, False, "C", 64),   # FMT's cross-attention K/V GEMM (run_cross_kv)
     (ELU1, 128, 64, "wave", False, "C", 64),
     (ELU1, 192, 64, 129, False, "C", 128),     # FMT's self-attention QKV GEMM
     (ELU1, 192, 128, "wave", True, "C+C2", 128),
-    (ELU1, 256, 64, 127, True, "C", 37),
+    (ELU1, 192, 64, 127, True, "C", 37),
     (RES, 64, 64, 1000, True, "C", None),
     (RES, 64, 256, "wave", True, "C+C2", None),
     (RES, 64, 128, 65, False, "C", None),
@@ -91,7 +99,7 @@ EPI_CASES = [
 
 def _epi_id(c):
     epi, N, K, M, bias, outs, extra = c
-    name = ["bias", "gelu", "elu1", "res", "res_ln", "ln"][epi]
+    name = EPI_NAMES[epi]
     return f"{name}-N{N}-K{K}-M{M}-{'b' if bias else 'nob'}-{outs}" + ("" if extra is None else f"-{extra}")
 
 

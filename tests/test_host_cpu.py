@@ -48,7 +48,7 @@ def test_bad_arguments_are_rejected_without_touching_the_gpu(lib):
 
     # the linear-layer epilogue seam: every bad combination is refused before the operand split is launched.  The
     # pointers are aligned placeholders that are never dereferenced.
-    BIAS, ELU1, RES, RES_LN, LN = 0, 2, 3, 4, 5
+    BIAS, GELU, ELU1, RES, RES_LN, LN = 0, 1, 2, 3, 4, 5
     ptr = ctypes.c_void_p(1 << 20)
 
     def epi_call(epi, N=64, K=64, M=128, lda=None, res=True, gamma=True, ln=True, C=ptr, ldc=None, Cpre=None,
@@ -63,23 +63,25 @@ def test_bad_arguments_are_rejected_without_touching_the_gpu(lib):
         (dict(epi=LN, N=128), b"LayerNorm epilogue needs N == 64"),
         (dict(epi=RES_LN, N=192), b"LayerNorm epilogue needs N == 64"),
         (dict(epi=LN, ln=False), b"LayerNorm epilogue needs N == 64"),
-        (dict(epi=BIAS, K=96), b"K % 64 == 0"),
+        (dict(epi=BIAS, N=192, K=96), b"K % 64 == 0"),
         (dict(epi=ELU1, N=100), b"need N in"),
-        (dict(epi=BIAS, Cpre=ptr), b"Cpre needs a LayerNorm epilogue"),
+        (dict(epi=BIAS, N=192, Cpre=ptr), b"Cpre needs a LayerNorm epilogue"),
         (dict(epi=RES, Cpre=ptr), b"Cpre needs a LayerNorm epilogue"),
         (dict(epi=RES, res=False), b"residual epilogue needs"),
         (dict(epi=RES_LN, gamma=False), b"residual epilogue needs"),
         (dict(epi=6), b"unknown epilogue"),
-        (dict(epi=BIAS, C=None), b"bad arguments"),
+        (dict(epi=BIAS, N=192, C=None), b"bad arguments"),
         (dict(epi=BIAS, N=256, K=128), b"too large for resident weights"),
-        (dict(epi=BIAS, C=ctypes.c_void_p((1 << 20) + 4)), b"C must be 16-byte aligned"),
-        (dict(epi=BIAS, C2=ptr, ldc2=132), b"C2 must be 16-byte aligned"),
-        (dict(epi=BIAS, lda=60), b"need lda >= K"),
+        (dict(epi=BIAS, N=192, C=ctypes.c_void_p((1 << 20) + 4)), b"C must be 16-byte aligned"),
+        (dict(epi=BIAS, N=192, C2=ptr, ldc2=132), b"C2 must be 16-byte aligned"),
+        (dict(epi=BIAS, N=192, lda=60), b"need lda >= K"),
+        (dict(epi=BIAS, N=64), b"no kernel for (N = 64, epilogue 0)"),     # (N, epilogue) pairs that are not built
+        (dict(epi=GELU, N=192), b"no kernel for (N = 192, epilogue 1)"),
     ]
     for kw, msg in bad:
         assert epi_call(**kw) == -1, kw
         assert msg in lib.mvsf_last_error(), (kw, lib.mvsf_last_error())
-    assert epi_call(BIAS, ws_bytes=1024) == -3 and b"workspace" in lib.mvsf_last_error()
+    assert epi_call(BIAS, N=192, ws_bytes=1024) == -3 and b"workspace" in lib.mvsf_last_error()
     assert lib.mvsf_launch_count(0) == 0
 
 
