@@ -142,7 +142,8 @@ int mvsf_costreg_tr_workspace_bytes(int C, int D, int H, int W, size_t* bytes);
 int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, const void* wts16, size_t n_wts,
                             float* logits, void* workspace, size_t workspace_bytes, int C, int D, int H, int W,
                             int layers, float softmax_scale, mvsf_stream_t stream);
-/* install-time helper: fp32 weight blob (n floats, n % 8 == 0) -> out16 = [n fp16 hi parts | n fp16 lo parts] (4n bytes) */
+/* install-time helper: fp32 weight blob (n floats, n % 8 == 0) -> out16 = [n fp16 hi parts | n fp16 lo parts] (4n bytes);
+ * wts and out16 16-byte aligned */
 int mvsf_split_weights_f16(const float* wts, void* out16, size_t n, mvsf_stream_t stream);
 
 /* softmax attention of R1 alone: models/dino/layers/attention.py:141-170 (FlashAttention2.forward after the qkv linear).

@@ -62,7 +62,7 @@ __global__ void qkv_tile_kernel(const float* __restrict__ qkv, __half* __restric
 #pragma unroll
     for (int d = 0; d < 8; ++d) {
       __half hi, lo;
-      gmma::split_f16(v[d], hi, lo);
+      split_f16(v[d], hi, lo);
       pv[kc * 320 + (oct * 8 + d) * 8 + e] = lo;
       pv[kc * 320 + (16 + oct * 8 + d) * 8 + e] = hi;
     }
@@ -223,7 +223,7 @@ __global__ void attention_merge_kernel(const float* __restrict__ partials, float
     const int col = head * HD + d;
     const float r0 = o[d] * inv, r1 = o[d + 1] * inv;
     if (out) *reinterpret_cast<float2*>(out + (size_t)t * W + col) = make_float2(r0, r1);
-    if (out2) gmma::split_store2(out2 + (size_t)t * (2 * W) + col, out2 + (size_t)t * (2 * W) + W + col, r0, r1);
+    if (out2) split_store2(out2 + (size_t)t * (2 * W) + col, out2 + (size_t)t * (2 * W) + W + col, r0, r1);
   }
 }
 

@@ -138,7 +138,8 @@ static __global__ void conv2d_pack_kernel(const float* __restrict__ w, __half* _
     const int part = row / NS, co = nb * NS + row % NS;
     const int ci = CI == 8 ? e : g * 16 + kc * 8 + e;
     const float wv = w[((size_t)tap * CI + ci) * CO + co];
-    const __half hi = __float2half_rn(wv), lo = __float2half_rn(wv - __half2float(hi));
+    __half hi, lo;
+    split_f16(wv, hi, lo);
     __half v;
     if (CI == 8) v = part == 0 ? hi : (kc == 0 ? lo : __float2half_rn(0.f));
     else v = part == 0 ? hi : lo;

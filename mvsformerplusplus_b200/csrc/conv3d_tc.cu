@@ -491,8 +491,8 @@ __global__ void conv3d_tc_pack_kernel(const float* __restrict__ w32, __half* __r
   const int ci = (KG == 1 ? g : g * 2 + kc) * 8 + e;
   float w = 0.f;
   if (tap && n < cout) w = w32[((size_t)((kd * 3 + kh) * 3 + kw) * cin + ci) * cout + n];
-  const __half hi = __float2half_rn(w);
-  const __half lo = __float2half_rn(w - __half2float(hi));
+  __half hi, lo;
+  split_f16(w, hi, lo);
   __half v;
   if (KG == 1) v = mm == 0 ? hi : (kc == 0 ? lo : __float2half_rn(0.f));
   else v = mm == 0 ? hi : lo;
@@ -509,13 +509,6 @@ int conv3d_tc_pack(const float* w32, __half* out, int mode, int sd, int cin, int
   return MVSF_OK;
 }
 
-__global__ void split_vec8_kernel(const float* __restrict__ x, __half* __restrict__ hi, __half* __restrict__ lo, size_t n8) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n8) return;
-  const float4 a = ldg4(x + i * 8), b = ldg4(x + i * 8 + 4);
-  const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-  split_store8(hi + i * 8, lo + i * 8, v);
-}
 __global__ void merge_vec8_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, float* __restrict__ x, size_t n8) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n8) return;
@@ -531,12 +524,6 @@ __global__ void merge_vec8_kernel(const __half* __restrict__ hi, const __half* _
   }
   *reinterpret_cast<float4*>(x + i * 8) = make_float4(r[0], r[1], r[2], r[3]);
   *reinterpret_cast<float4*>(x + i * 8 + 4) = make_float4(r[4], r[5], r[6], r[7]);
-}
-int launch_split_vec8(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t s) {
-  MVSF_REQUIRE(x && hi && lo && n > 0 && n % 8 == 0, "split_vec8: bad arguments");
-  split_vec8_kernel<<<cdiv((long long)(n / 8), 256), 256, 0, s>>>(x, hi, lo, n / 8);
-  MVSF_LAUNCH_CHECK("split_vec8");
-  return MVSF_OK;
 }
 int launch_merge_vec8(const __half* hi, const __half* lo, float* x, size_t n, cudaStream_t s) {
   MVSF_REQUIRE(x && hi && lo && n > 0 && n % 8 == 0, "merge_vec8: bad arguments");
@@ -763,8 +750,8 @@ extern "C" int mvsf_conv3d_tc_layer(int mode, int sd, const float* in, const flo
   __half* xskip = xout + 2 * nout;
   __half* wtc = xskip + 2 * nout;
   int rc;
-  if ((rc = launch_split_vec8(in, xin, xin + nin, nin, s))) return rc;
-  if (skip && (rc = launch_split_vec8(skip, xskip, xskip + nout, nout, s))) return rc;
+  if ((rc = launch_split_f16(in, nin, xin, 2 * nin, 1, nin, s))) return rc;
+  if (skip && (rc = launch_split_f16(skip, nout, xskip, 2 * nout, 1, nout, s))) return rc;
   if ((rc = conv3d_tc_pack(w32, wtc, mode, sd, cin, cout, s))) return rc;
   ConvTcArgs a{};
   a.in_hi = xin; a.in_lo = xin + nin; a.wtc = wtc; a.bias = w32 + (size_t)27 * cin * cout;

@@ -30,8 +30,7 @@ size_t conv3d_tc_packed_halves(int mode, int cin, int cout);   // number of fp16
 int conv3d_tc_col(int mode, int sd, int cout);                 // 1: depth-streaming kernel (depth stride 1, Cout <= 32)
 int conv3d_tc_pack(const float* w32, __half* out, int mode, int sd, int cin, int cout, cudaStream_t s);
 int launch_conv3d_tc(const ConvTcArgs& a, int mode, int out_mode, cudaStream_t s);
-// x [n] fp32 -> hi[n], lo[n] fp16 (n % 8 == 0) and back
-int launch_split_vec8(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t s);
+// hi[n], lo[n] fp16 -> x [n] fp32 (n % 8 == 0), the inverse of launch_split_f16
 int launch_merge_vec8(const __half* hi, const __half* lo, float* x, size_t n, cudaStream_t s);
 
 }  // namespace mvsf

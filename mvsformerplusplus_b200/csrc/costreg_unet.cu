@@ -80,7 +80,7 @@ static int unet_forward_tc(int kind, const float* vol, const float* wts, const _
   }
   const float* wp = w32[8] + layer_floats(16, 8);
   int rc;
-  if ((rc = launch_split_vec8(vol, v0, v0 + n0, n0, s))) return rc;
+  if ((rc = launch_split_f16(vol, n0, v0, 2 * n0, 1, n0, s))) return rc;
   auto conv = [&](int l, const __half* in, size_t nin, __half* out, size_t nout, const __half* skip, size_t nskip,
                   int ID, int IH, int IW) {
     ConvTcArgs a{};

@@ -22,6 +22,7 @@ struct NhwcSrc {
   static constexpr uint32_t EXTRA = 0;
   __device__ void fill(unsigned char* smem, int n, int y0, int x0, int tid) const {
     constexpr int NPIX = L::PR * L::PC;
+#pragma unroll 2   // two pixel octets' loads in flight per thread
     for (int i = tid; i < L::NP * NPIX * L::NO; i += 256) {
       const int o = i % L::NO, rest = i / L::NO;
       const int pix = rest % NPIX, par = rest / NPIX;

@@ -140,12 +140,8 @@ linattn_apply_kernel(const float* __restrict__ q, int ldq, const float* __restri
       }
       r[mm] = t * z;
     }
-    const __half2 h01 = __floats2half2_rn(r[0], r[1]), h23 = __floats2half2_rn(r[2], r[3]);
-    const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
-    *reinterpret_cast<__half2*>(op + mq * 4) = h01;
-    *reinterpret_cast<__half2*>(op + mq * 4 + 2) = h23;
-    *reinterpret_cast<__half2*>(op + C + mq * 4) = __floats2half2_rn(r[0] - f01.x, r[1] - f01.y);
-    *reinterpret_cast<__half2*>(op + C + mq * 4 + 2) = __floats2half2_rn(r[2] - f23.x, r[3] - f23.y);
+    split_store2(op + mq * 4, op + C + mq * 4, r[0], r[1]);
+    split_store2(op + mq * 4 + 2, op + C + mq * 4 + 2, r[2], r[3]);
   }
 }
 
@@ -201,10 +197,7 @@ struct RowVec {
 #pragma unroll
     for (int e = 0; e < E; e += 2) {
       const int c = col(lane, e);
-      const __half2 hh = __floats2half2_rn(v[e], v[e + 1]);
-      const float2 hf = __half22float2(hh);
-      *reinterpret_cast<__half2*>(y2 + c) = hh;
-      *reinterpret_cast<__half2*>(y2 + C + c) = __floats2half2_rn(v[e] - hf.x, v[e + 1] - hf.y);
+      split_store2(y2 + c, y2 + C + c, v[e], v[e + 1]);
     }
   }
 };

@@ -22,26 +22,6 @@ using namespace gmma;
 
 constexpr int TC_BM = 128, TC_BK = 64;
 
-__global__ void split_f16_kernel(const float* __restrict__ x, int ldx, __half* __restrict__ out, int ldo, int M, int K) {
-  // out[m][k] = hi, out[m][K + k] = lo ; 4 elements per thread
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  size_t total = (size_t)M * (K / 4);
-  if (i >= total) return;
-  int m = (int)(i / (K / 4)), q = (int)(i % (K / 4));
-  float4 v = ldg4(x + (size_t)m * ldx + q * 4);
-  float f[4] = {v.x, v.y, v.z, v.w};
-  __half hi[4], lo[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    hi[e] = __float2half_rn(f[e]);
-    lo[e] = __float2half_rn(f[e] - __half2float(hi[e]));
-  }
-  __half2* ph = reinterpret_cast<__half2*>(out + (size_t)m * ldo + q * 4);
-  __half2* pl = reinterpret_cast<__half2*>(out + (size_t)m * ldo + K + q * 4);
-  ph[0] = __halves2half2(hi[0], hi[1]); ph[1] = __halves2half2(hi[2], hi[3]);
-  pl[0] = __halves2half2(lo[0], lo[1]); pl[1] = __halves2half2(lo[2], lo[3]);
-}
-
 // 384 threads: warpgroup 0 = producers (cp.async fills of the A ring), warpgroups 1 and 2 = MMA + epilogue of rows
 // [0, 64) and [64, 128) of every tile.  The weight tiles of all K-blocks stay resident in shared memory for the CTA's
 // lifetime.  Each MMA warpgroup keeps one K-block of MMAs in flight while it issues the next, and releases a ring stage
@@ -351,14 +331,6 @@ constexpr uint32_t MLP_OFF_F1 = 2 * MLP_T64, MLP_OFF_F2 = MLP_OFF_F1 + 2 * MLP_T
                    MLP_OFF_BAR = MLP_OFF_A + MLP_RING * 2 * MLP_TA, MLP_SMEM = MLP_OFF_BAR + 16 * MLP_RING;
 static_assert(MLP_SMEM <= 227 * 1024, "token MLP: resident weights + ring exceed shared memory");
 
-// hi|lo split of the pair (a, b) as two fp16x2 registers, rounded as split_store2 rounds
-__device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  const __half2 h = __floats2half2_rn(a, b);
-  const float2 hf = __half22float2(h);
-  const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
 // D (+)= A * B^T over K = 64 with the three split products per k16 step; A = register fragments [k16 step][4],
 // B = hi tile at b (lo tile b_lo bytes after it), leading byte offset lbo
 __device__ __forceinline__ void mlp_mma_rs(float (&d)[32], const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint32_t b,
@@ -824,26 +796,25 @@ int launch_linear_tcs(const TcsArgs& a, int epi, cudaStream_t s) {
   return a.N % 128 == 0 ? launch_tcs_bn<128>(a, epi, s) : launch_tcs_bn<64>(a, epi, s);
 }
 
-__global__ void split_blob_f16_kernel(const float* __restrict__ x, __half* __restrict__ hi, __half* __restrict__ lo, size_t n) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float v = x[i];
-  __half h = __float2half_rn(v);
-  hi[i] = h;
-  lo[i] = __float2half_rn(v - __half2float(h));
+// The fp16 hi + lo split of M rows of K fp32 values (launch_split_f16 in common.cuh): 8 values per thread, 16-byte
+// loads and stores
+__global__ void split_hi_lo_f16_kernel(const float* __restrict__ x, size_t ldx, __half* __restrict__ out, size_t ldo,
+                                       size_t K, unsigned total) {
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x, k8 = (unsigned)(K / 8);
+  if (i >= total) return;
+  const unsigned m = i / k8;
+  const size_t k = (size_t)(i - m * k8) * 8;
+  const float4 a = ldg4(x + m * ldx + k), b = ldg4(x + m * ldx + k + 4);
+  const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+  split_store8(out + m * ldo + k, out + m * ldo + K + k, v);
 }
-int launch_split_blob_f16(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t s) {
-  MVSF_REQUIRE(x && hi && lo && n > 0, "split_blob_f16: bad arguments");
-  split_blob_f16_kernel<<<cdiv((long long)n, 256), 256, 0, s>>>(x, hi, lo, n);
-  MVSF_LAUNCH_CHECK("split_blob_f16");
-  return MVSF_OK;
-}
-
-int launch_split_f16(const float* x, int ldx, __half* out, int ldo, int M, int K, cudaStream_t s) {
-  MVSF_REQUIRE(x && out && M > 0 && K % 4 == 0 && ldx % 4 == 0 && ldo % 2 == 0, "split_f16: bad arguments");
-  size_t total = (size_t)M * (K / 4);
-  split_f16_kernel<<<cdiv((long long)total, 256), 256, 0, s>>>(x, ldx, out, ldo, M, K);
-  MVSF_LAUNCH_CHECK("split_f16");
+int launch_split_f16(const float* x, size_t ldx, __half* out, size_t ldo, int M, size_t K, cudaStream_t s) {
+  MVSF_REQUIRE(x && out && M > 0 && K > 0 && K % 8 == 0 && ldx >= K && ldx % 4 == 0 && ldo >= 2 * K && ldo % 8 == 0 &&
+                   ((uintptr_t)x & 15) == 0 && ((uintptr_t)out & 15) == 0 && (size_t)M * (K / 8) <= 0xffffffffu,
+               "split_f16: bad arguments");
+  const unsigned total = (unsigned)((size_t)M * (K / 8));
+  split_hi_lo_f16_kernel<<<cdiv(total, 256), 256, 0, s>>>(x, ldx, out, ldo, K, total);
+  MVSF_LAUNCH_CHECK("split_hi_lo_f16");
   return MVSF_OK;
 }
 
@@ -900,9 +871,9 @@ extern "C" int mvsf_token_mlp_forward(int form, const float* A, const float* res
   if ((rc = check_token_mlp(a, form))) return rc;   // every rejection happens before the first launch
   cudaStream_t s = (cudaStream_t)stream;
   if ((rc = launch_split_f16(A, 64, A2, 128, M, 64, s))) return rc;
-  if ((rc = launch_split_blob_f16(proj_w, wp, wp + NP, NP, s))) return rc;
-  if ((rc = launch_split_blob_f16(f1_w, w1, w1 + NF, NF, s))) return rc;
-  if ((rc = launch_split_blob_f16(f2_w, w2, w2 + NF, NF, s))) return rc;
+  if ((rc = launch_split_f16(proj_w, NP, wp, 2 * NP, 1, NP, s))) return rc;
+  if ((rc = launch_split_f16(f1_w, NF, w1, 2 * NF, 1, NF, s))) return rc;
+  if ((rc = launch_split_f16(f2_w, NF, w2, 2 * NF, 1, NF, s))) return rc;
   return launch_token_mlp(a, form, s);
 }
 
@@ -936,5 +907,5 @@ extern "C" int mvsf_linear_tc_streamed_epilogue(int epi, const float* A, int lda
 extern "C" int mvsf_split_weights_f16(const float* wts, void* out16, size_t n, mvsf_stream_t stream) {
   MVSF_REQUIRE(wts && out16 && n > 0 && (n % 8) == 0, "split_weights_f16: n must be a multiple of 8");
   __half* hi = reinterpret_cast<__half*>(out16);
-  return launch_split_blob_f16(wts, hi, hi + n, n, (cudaStream_t)stream);
+  return launch_split_f16(wts, n, hi, 2 * n, 1, n, (cudaStream_t)stream);
 }

@@ -68,19 +68,5 @@ inline TcsArgs tcs_rows(const __half* A, int lda, int K, const __half* Bh, const
   return a;
 }
 int launch_linear_tcs(const TcsArgs& a, int epi, cudaStream_t s);
-// out row m = [hi(0..K) | lo(0..K)] (ldo >= 2K)
-int launch_split_f16(const float* x, int ldx, __half* out, int ldo, int M, int K, cudaStream_t s);
-// element-wise split of a flat fp32 blob into two fp16 blobs with the same indexing (weights, done once at install time)
-int launch_split_blob_f16(const float* x, __half* hi, __half* lo, size_t n, cudaStream_t s);
-__device__ __forceinline__ void split_store8(__half* hi_dst, __half* lo_dst, const float (&v)[8]) {
-  __align__(16) __half h[8], l[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    h[e] = __float2half_rn(v[e]);
-    l[e] = __float2half_rn(v[e] - __half2float(h[e]));
-  }
-  *reinterpret_cast<uint4*>(hi_dst) = *reinterpret_cast<uint4*>(h);
-  *reinterpret_cast<uint4*>(lo_dst) = *reinterpret_cast<uint4*>(l);
-}
 
 }  // namespace mvsf

@@ -61,7 +61,8 @@ vis_cnn_kernel(const float* __restrict__ entropy, const float* __restrict__ wts,
     float w = 0.f;
     if (layer == 0) w = __ldg(wts + OFF_W2 + (ci * 9 + tap) * 16 + n);
     else if (n < 8) w = __ldg(wts + OFF_W3 + (ci * 9 + tap) * 8 + n);
-    const __half hi = __float2half_rn(w), lo = __float2half_rn(w - __half2float(hi));
+    __half hi, lo;
+    split_f16(w, hi, lo);
     __half* t = reinterpret_cast<__half*>(smem + (layer ? OFF_B3T : OFF_B2T) + tap * 1024);
     t[kc * 256 + n * 8 + e] = hi;
     t[kc * 256 + (16 + n) * 8 + e] = lo;

@@ -82,9 +82,10 @@ __global__ void vit_qkv_tile_kernel(const float* __restrict__ qkv, int ldq, __ha
                  ((t & 127) >> 3) * (LBO_V / 2) + (t & 7);
 #pragma unroll
     for (int d = 0; d < 8; ++d) {
-      const __half hi = __float2half_rn(v[d]);
+      __half hi, lo;
+      split_f16(v[d], hi, lo);
       pv[(oct * 8 + d) * 8] = hi;
-      pv[(72 + oct * 8 + d) * 8] = __float2half_rn(v[d] - __half2float(hi));
+      pv[(72 + oct * 8 + d) * 8] = lo;
     }
     if (oct == 0) pv[64 * 8] = __float2half_rn(t < N ? 1.0f : 0.0f);
     if (oct == 1) {

@@ -187,7 +187,7 @@ extern "C" int mvsf_vit_decoder_pack_tc(const float* wts, void* wts_tc, size_t w
   MVSF_REQUIRE(wts && wts_tc && ((uintptr_t)wts_tc & 15) == 0, "vit_decoder_pack_tc: bad arguments");
   MVSF_REQUIRE(wts_tc_bytes >= NG * 2 * sizeof(__half), "vit_decoder_pack_tc: wts_tc too small");
   __half* hi = static_cast<__half*>(wts_tc);
-  return launch_split_blob_f16(wts, hi, hi + NG, NG, (cudaStream_t)stream);
+  return launch_split_f16(wts, NG, hi, 2 * NG, 1, NG, (cudaStream_t)stream);
 }
 
 extern "C" int mvsf_vit_decoder_forward(const float* x0, const float* x1, const float* x2, const float* wts,

@@ -229,18 +229,6 @@ __device__ __forceinline__ uint32_t pack_half2(float lo_elem, float hi_elem) {
   const __half2 h = __floats2half2_rn(lo_elem, hi_elem);
   return *reinterpret_cast<const uint32_t*>(&h);
 }
-// fp16 hi | lo split of one value
-__device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
-  hi = __float2half_rn(x);
-  lo = __float2half_rn(x - __half2float(hi));
-}
-// fp16 hi | lo split of two consecutive values, stored as one half2 each
-__device__ __forceinline__ void split_store2(__half* hi_dst, __half* lo_dst, float a, float b) {
-  const __half2 h = __floats2half2_rn(a, b);
-  const float2 hf = __half22float2(h);
-  *reinterpret_cast<__half2*>(hi_dst) = h;
-  *reinterpret_cast<__half2*>(lo_dst) = __floats2half2_rn(a - hf.x, b - hf.y);
-}
 
 // cuTensorMapEncodeTiled from the driver the runtime uses (nullptr if it has none)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,

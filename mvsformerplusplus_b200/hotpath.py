@@ -68,26 +68,33 @@ def to_nchw(x_nhwc):
     return out
 
 
+def _pack_f16(entry, flat, *args, query=None):
+    """fp32 parameter blob on the device -> the fp16 buffer that the library's pack entry point
+    mvsf_<entry>(*args, flat, out, size, stream) fills (install time, once).  query = (name, *query_args):
+    mvsf_<name>(*query_args, &size) gives the buffer's size in bytes.  Without a query the buffer is the hi | lo split
+    of the whole blob, 2 n halves, and size = n."""
+    L = _lib.lib()
+    if query is None:
+        size, halves = flat.numel(), 2 * flat.numel()
+    else:
+        need = ctypes.c_size_t(0)
+        _lib.check(getattr(L, "mvsf_" + query[0])(*query[1:], ctypes.byref(need)), query[0])
+        size, halves = need.value, need.value // 2
+    out = torch.empty(halves, device=flat.device, dtype=torch.float16)
+    _lib.check(getattr(L, "mvsf_" + entry)(*args, _ptr(flat), _ptr(out), ctypes.c_size_t(size), _stream()), entry)
+    return out
+
+
 def split_weights_f16(flat):
     """fp32 weight blob on the device -> fp16 [hi | lo] blob for the wgmma GEMMs (install time, once)."""
-    L = _lib.lib()
-    n = flat.numel()
-    assert n % 8 == 0
-    out = torch.empty(2 * n, device=flat.device, dtype=torch.float16)
-    _lib.check(L.mvsf_split_weights_f16(_ptr(flat), _ptr(out), ctypes.c_size_t(n), _stream()), "split_weights_f16")
-    return out
+    assert flat.numel() % 8 == 0
+    return _pack_f16("split_weights_f16", flat)
 
 
 def pack_unet_tc(kind, flat):
     """fp32 U-Net weight blob (packing.pack_costreg_unet) on the device -> fp16 hi/lo weight slabs of the wgmma
     implicit-GEMM convolutions (install time, once)."""
-    L = _lib.lib()
-    need = ctypes.c_size_t(0)
-    _lib.check(L.mvsf_costreg_unet_tc_bytes(ctypes.byref(need)), "costreg_unet_tc_bytes")
-    out = torch.empty(need.value // 2, device=flat.device, dtype=torch.float16)
-    _lib.check(L.mvsf_costreg_unet_pack_tc(kind, _ptr(flat), _ptr(out), ctypes.c_size_t(need.value), _stream()),
-               "costreg_unet_pack_tc")
-    return out
+    return _pack_f16("costreg_unet_pack_tc", flat, kind, query=("costreg_unet_tc_bytes",))
 
 
 @torch.no_grad()
@@ -119,7 +126,13 @@ def homo_warping_3D_with_mask(src_fea, src_proj, ref_proj, depth_values):
 
 
 class _PackedMixin:
-    """Packs the module's parameters for the CUDA library on first use / after load_state_dict."""
+    """Packs the module's parameters for the CUDA library on first use / after load_state_dict.  A module implements
+    _build_pack(device), which returns the dict of packed blobs; _pack(device) caches it per device."""
+
+    def _pack(self, device):
+        if self._packed is None or self._packed["device"] != device:
+            self._packed = dict(self._build_pack(device), device=device)
+        return self._packed
 
     def _invalidate(self, *a, **k):
         self._packed = None
@@ -163,11 +176,9 @@ class StageNet(_PackedMixin, nn.Module):
         self._init_packing()
 
     # ---- packing
-    def _pack(self, device):
-        if self._packed is not None and self._packed["device"] == device:
-            return self._packed
+    def _build_pack(self, device):
         sd = {k: v for k, v in self.state_dict().items()}
-        pk = {"device": device, "vis": packing.pack_vis(sd, "vis.").to(device)}
+        pk = {"vis": packing.pack_vis(sd, "vis.").to(device)}
         if self.cost_reg_type == "PureTransformerCostReg":
             tc = self.args["transformer_config"][self.stage_idx]
             if tuple(tc["down_rate"]) != (2, 4, 4) or tc["mid_channel"] != 64 or tc["num_heads"] != 4 or tc["mlp_ratio"] != 4:
@@ -182,7 +193,6 @@ class StageNet(_PackedMixin, nn.Module):
             pk["kind"] = kind
             pk["reg"] = flat.to(device)
             pk["reg_tc"] = pack_unet_tc(kind, pk["reg"])
-        self._packed = pk
         return pk
 
     def _softmax_scale(self, n_tokens):
@@ -304,12 +314,10 @@ class FMT_with_pathway(_PackedMixin, nn.Module):
         self.pe_dict = {}
         self._init_packing()
 
-    def _pack(self, device):
-        if self._packed is None or self._packed["device"] != device:
-            sd = {"FMT_module." + k: v for k, v in self.state_dict().items()}
-            w = packing.pack_fmt(sd).to(device)
-            self._packed = {"device": device, "w": w, "w16": split_weights_f16(w)}
-        return self._packed
+    def _build_pack(self, device):
+        sd = {"FMT_module." + k: v for k, v in self.state_dict().items()}
+        w = packing.pack_fmt(sd).to(device)
+        return {"w": w, "w16": split_weights_f16(w)}
 
     def _pe(self, H, W, device):
         """PositionEncodingSineNorm table (position_encoding.py:61-74) as [H*W, 64], cached per shape like the
@@ -464,15 +472,6 @@ def _check_fpn_size(H, W):
                          f"upsamplings), got {H}x{W}")
 
 
-def _fpn_pack_tc(part, flat):
-    L = _lib.lib()
-    need = ctypes.c_size_t(0)
-    _lib.check(L.mvsf_fpn_tc_bytes(part, ctypes.byref(need)), "fpn_tc_bytes")
-    out = torch.empty(need.value // 2, device=flat.device, dtype=torch.float16)
-    _lib.check(L.mvsf_fpn_pack_tc(part, _ptr(flat), _ptr(out), ctypes.c_size_t(need.value), _stream()), "fpn_pack_tc")
-    return out
-
-
 class FPNEncoder(_PackedMixin, nn.Module):
     """Drop-in for the reference FPNEncoder (models/module.py:208-239), eval mode: returns [conv01, conv11, conv21, conv31]
     as fp32 [N,C,h,w] views of channels-last buffers.  Any float dtype and strides are accepted."""
@@ -483,11 +482,9 @@ class FPNEncoder(_PackedMixin, nn.Module):
         build_fpn_encoder(self)
         self._init_packing()
 
-    def _pack(self, device):
-        if self._packed is None or self._packed["device"] != device:
-            w = packing.pack_fpn_encoder(self.state_dict(), "").to(device)
-            self._packed = {"device": device, "w": w, "tc": _fpn_pack_tc(0, w)}
-        return self._packed
+    def _build_pack(self, device):
+        w = packing.pack_fpn_encoder(self.state_dict(), "").to(device)
+        return {"w": w, "tc": _pack_f16("fpn_pack_tc", w, 0, query=("fpn_tc_bytes", 0))}
 
     @torch.no_grad()
     def forward(self, x, vit_feat=None):
@@ -534,11 +531,9 @@ class FPNDecoder(_PackedMixin, nn.Module):
         build_fpn_decoder(self)
         self._init_packing()
 
-    def _pack(self, device):
-        if self._packed is None or self._packed["device"] != device:
-            w = packing.pack_fpn_decoder(self.state_dict(), "").to(device)
-            self._packed = {"device": device, "w": w, "tc": _fpn_pack_tc(1, w)}
-        return self._packed
+    def _build_pack(self, device):
+        w = packing.pack_fpn_decoder(self.state_dict(), "").to(device)
+        return {"w": w, "tc": _pack_f16("fpn_pack_tc", w, 1, query=("fpn_tc_bytes", 1))}
 
     @torch.no_grad()
     def forward(self, conv01, conv11, conv21, conv31):
@@ -604,17 +599,9 @@ class CrossVITDecoder(_PackedMixin, nn.Module):
         build_vit_decoder(self, init_values=cfg["init_values"], prev_values=cfg.get("prev_values", 0.5))
         self._init_packing()
 
-    def _pack(self, device):
-        if self._packed is None or self._packed["device"] != device:
-            L = _lib.lib()
-            w = packing.pack_vit_decoder(self.state_dict()).to(device)
-            need = ctypes.c_size_t(0)
-            _lib.check(L.mvsf_vit_decoder_tc_bytes(ctypes.byref(need)), "vit_decoder_tc_bytes")
-            tc = torch.empty(need.value // 2, device=device, dtype=torch.float16)
-            _lib.check(L.mvsf_vit_decoder_pack_tc(_ptr(w), _ptr(tc), ctypes.c_size_t(need.value), _stream()),
-                       "vit_decoder_pack_tc")
-            self._packed = {"device": device, "w": w, "tc": tc}
-        return self._packed
+    def _build_pack(self, device):
+        w = packing.pack_vit_decoder(self.state_dict()).to(device)
+        return {"w": w, "tc": _pack_f16("vit_decoder_pack_tc", w, query=("vit_decoder_tc_bytes",))}
 
     @torch.no_grad()
     def forward(self, x, Fmats=None, vit_shape=None):
@@ -688,19 +675,13 @@ class DinoVisionTransformer(_PackedMixin, nn.Module):
             prm.requires_grad = False
         self._init_packing()
 
-    def _pack(self, device):
-        if self._packed is None or self._packed["device"] != device:
-            L = _lib.lib()
-            blob = packing.pack_vit(self.state_dict()).to(device)
-            need = ctypes.c_size_t(0)
-            _lib.check(L.mvsf_vit_tc_bytes(ctypes.byref(need)), "vit_tc_bytes")
-            tc = torch.empty(need.value // 2, device=device, dtype=torch.float16)
-            _lib.check(L.mvsf_vit_pack_tc(_ptr(blob), _ptr(tc), ctypes.c_size_t(need.value), _stream()), "vit_pack_tc")
-            # keep the fp16 hi / lo GEMM weights and the small fp32 parameters, not the fp32 GEMM weights
-            w = blob[packing.VIT_GEMM_WTS:].clone()
-            del blob
-            self._packed = {"device": device, "w": w, "tc": tc, "pos": {}}
-        return self._packed
+    def _build_pack(self, device):
+        blob = packing.pack_vit(self.state_dict()).to(device)
+        tc = _pack_f16("vit_pack_tc", blob, query=("vit_tc_bytes",))
+        # keep the fp16 hi / lo GEMM weights and the small fp32 parameters, not the fp32 GEMM weights
+        w = blob[packing.VIT_GEMM_WTS:].clone()
+        del blob
+        return {"w": w, "tc": tc, "pos": {}}
 
     def _pos(self, pk, gh, gw):
         """interpolated pos_embed of the grid (a weight transform), cached with the packed weights"""

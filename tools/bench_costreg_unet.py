@@ -3,7 +3,7 @@ cuda:0 at the sizes one depth map runs them, per U-Net and per conv layer.
 
   * per U-Net: median of --reps CUDA-event timings of one mvsf_costreg_unet_forward (after --warmup calls);
   * per layer: a separate torch.profiler run (CUDA activity only) over --prof-reps forwards; kernels are assigned to
-    layers by launch order (split_vec8, conv1 .. conv6, conv7 / conv9 / conv11 transposed, [prob3]), median per launch
+    layers by launch order (split_hi_lo_f16, conv1 .. conv6, conv7 / conv9 / conv11 transposed, [prob3]), median per launch
     over the forwards whose kernels the trace recorded completely.
 
 Next to each layer time it prints what the layer's kernel ISSUES to the tensor cores (the hi/lo split products - 2 MMA
@@ -168,10 +168,10 @@ def main():
         kern = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
                        and "memcpy" not in e.name.lower() and "memset" not in e.name.lower()),
                       key=lambda e: e.time_range.start)
-        # one forward = split_vec8, 9 convs[, prob3]; the trace can miss a kernel record, so only complete forwards count
+        # one forward = split_hi_lo_f16, 9 convs[, prob3]; the trace can miss a kernel record, so only complete forwards count
         fwds = []
         for e in kern:
-            if "split_vec8" in e.name:
+            if "split_hi_lo_f16" in e.name:
                 fwds.append([])
             if fwds:
                 fwds[-1].append(e)
