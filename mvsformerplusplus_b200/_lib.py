@@ -1,88 +1,70 @@
-"""ctypes binding of libmvsf_b200.so (include/mvsf_b200.h).  There is no fallback: if the library is missing or a
-call fails, a RuntimeError is raised (the reference's seams raise Python exceptions: SURVEY.md §8b)."""
+"""ctypes binding of libmvsf_b200.so, typed from include/mvsf_b200.h when the library is loaded: the header is the one
+place a signature is written.  There is no fallback: if the library is missing or a call fails, a RuntimeError is raised
+(the reference's seams raise Python exceptions: SURVEY.md §8b)."""
 import ctypes
 import os
+import re
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
+HEADER = os.path.join(_HERE, "..", "include", "mvsf_b200.h")
 LIB_PATH = os.environ.get("MVSF_LIB_PATH") or os.path.join(_HERE, "libmvsf_b200.so")   # override: A-B builds of the same library
 _lib = None
+_streamed = None   # names of the entry points whose last parameter is mvsf_stream_t: the ones that enqueue device work
 
-P, I, F, Z = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_size_t
-SIGNATURES = {
-    "mvsf_abi_version": ([], I),
-    "mvsf_launch_count": ([I], ctypes.c_longlong),
-    "mvsf_ktimer_enable": ([I], I),
-    "mvsf_ktimer_read": ([ctypes.c_char_p, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_longlong)], I),
-    "mvsf_nchw_to_nhwc": ([P, P, I, I, I, P], I),
-    "mvsf_nhwc_to_nchw": ([P, P, I, I, I, P], I),
-    "mvsf_compose_geometry": ([P, I, P, P, P], I),
-    "mvsf_homography_from_proj": ([P, P, I, P, P], I),
-    "mvsf_init_inverse_range": ([P, I, P, I, I, I, P], I),
-    "mvsf_schedule_inverse_range": ([P, P, I, F, P, I, I, I, P], I),
-    "mvsf_position3d": ([P, P, P, I, P, I, P, I, I, I, P], I),
-    "mvsf_homo_warp": ([P, P, P, P, P, I, I, I, I, P], I),
-    "mvsf_warp_corr_set_tile_path": ([I], I),
-    "mvsf_warp_corr_last_selection": ([ctypes.POINTER(I), ctypes.POINTER(I)], I),
-    "mvsf_warp_corr_plan": ([I, I, I, I, I, I, Z], I),
-    "mvsf_warp_corr_entropy": ([P, P, P, P, I, I, I, I, I, I, P], I),
-    "mvsf_vis_cnn": ([P, P, P, I, I, I, P], I),
-    "mvsf_warp_corr_aggregate": ([P, P, P, P, P, I, I, I, I, I, I, P], I),
-    "mvsf_warp_corr_entropy_store": ([P, P, P, P, P, I, I, I, I, I, I, P], I),
-    "mvsf_corr_aggregate": ([P, P, P, I, I, I, I, I, P], I),
-    "mvsf_costreg_unet_workspace_bytes": ([I, I, I, I, I, ctypes.POINTER(Z)], I),
-    "mvsf_costreg_unet_tc_bytes": ([ctypes.POINTER(Z)], I),
-    "mvsf_costreg_unet_pack_tc": ([I, P, P, Z, P], I),
-    "mvsf_costreg_unet_forward": ([I, P, P, P, P, P, Z, I, I, I, I, P], I),
-    "mvsf_conv3d_tc_layer": ([I, I, P, P, P, P, P, Z, I, I, I, I, I, P], I),
-    "mvsf_costreg_tr_workspace_bytes": ([I, I, I, I, ctypes.POINTER(Z)], I),
-    "mvsf_costreg_tr_forward": ([P, P, P, P, Z, P, P, Z, I, I, I, I, I, F, P], I),
-    "mvsf_split_weights_f16": ([P, P, Z, P], I),
-    "mvsf_attention_forward": ([P, P, P, Z, I, F, P], I),
-    "mvsf_attention_split_plan": ([I, I, ctypes.POINTER(I), ctypes.POINTER(I)], I),
-    "mvsf_linear_tc_epilogue": ([I, P, I, P, P, P, I, P, P, P, F, I, P, I, P, I, P, I, P, Z, I, I, I, P], I),
-    "mvsf_softargmax": ([P, P, F, P, P, P, I, I, I, P], I),
-    "mvsf_conf_accumulate": ([P, I, I, P, I, I, F, I, P], I),
-    "mvsf_fmt_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
-    "mvsf_fmt_forward": ([P] * 7 + [Z] + [P] * 5 + [Z, I, I, I, P], I),
-    "mvsf_fpn_encoder_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
-    "mvsf_fpn_encoder_forward": ([P] * 8 + [Z, I, I, I, P], I),
-    "mvsf_fpn_encoder_vit_forward": ([P, P, I] + [P] * 7 + [Z, I, I, I, P], I),
-    "mvsf_fpn_decoder_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
-    "mvsf_fpn_decoder_forward": ([P] * 11 + [Z, I, I, I, P], I),
-    "mvsf_fpn_tc_bytes": ([I, ctypes.POINTER(Z)], I),
-    "mvsf_fpn_pack_tc": ([I, P, P, Z, P], I),
-    "mvsf_token_mlp_forward": ([I, P, P, P, P, P, P, P, F, P, P, P, P, P, P, P, F, P, P, P, Z, I, P], I),
-    "mvsf_linear_tc_streamed_epilogue": ([I, P, I, P, P, P, I, P, I, P, I, P, I, P, Z, I, I, I, P], I),
-    "mvsf_vit_decoder_workspace_bytes": ([I, I, I, I, ctypes.POINTER(Z)], I),
-    "mvsf_vit_decoder_tc_bytes": ([ctypes.POINTER(Z)], I),
-    "mvsf_vit_decoder_pack_tc": ([P, P, Z, P], I),
-    "mvsf_vit_decoder_forward": ([P] * 7 + [Z, I, I, I, I, P], I),
-    "mvsf_vit_workspace_bytes": ([I, I, I, ctypes.POINTER(Z)], I),
-    "mvsf_vit_tc_bytes": ([ctypes.POINTER(Z)], I),
-    "mvsf_vit_pack_tc": ([P, P, Z, P], I),
-    "mvsf_vit_forward": ([P] * 8 + [Z, I, I, I, P], I),
-    "mvsf_vit_forward_image": ([P, I, I] + [P] * 7 + [Z, I, I, I, P], I),
-    "mvsf_vit_attention_forward": ([P, I, P, I, P, Z, I, I, P], I),
-    "mvsf_fusion_workspace_bytes": ([I, I, ctypes.POINTER(Z)], I),
-    "mvsf_fusion_prepare_cameras": ([P, I, P, P], I),
-    "mvsf_fusion_filter": ([I, P, P, P, P, I, I, ctypes.POINTER(I), I, I, I, F, F, F, F, F, P, P, P, Z, P], I),
-    "mvsf_fusion_extract": ([P, P, P, Z, P, P, P, P, ctypes.c_longlong, I, I, P], I),
+# C type spelling in the header -> ctypes type; any other pointer is passed as c_void_p
+_C_TYPES = {
+    "int": ctypes.c_int, "float": ctypes.c_float, "size_t": ctypes.c_size_t, "long long": ctypes.c_longlong,
+    "size_t*": ctypes.POINTER(ctypes.c_size_t), "int*": ctypes.POINTER(ctypes.c_int),
+    "const int*": ctypes.POINTER(ctypes.c_int), "double*": ctypes.POINTER(ctypes.c_double),
+    "long long*": ctypes.POINTER(ctypes.c_longlong), "const char*": ctypes.c_char_p, "mvsf_stream_t": ctypes.c_void_p,
 }
 
 
+def _spelling(t):
+    """one spelling per C type: single spaces, no space before a '*'"""
+    return re.sub(r" ?\*", "*", " ".join(t.split()))
+
+
+def ctype(spelling):
+    """ctypes type of a C type as prototypes() spells it; an unknown spelling raises instead of guessing."""
+    if spelling in _C_TYPES:
+        return _C_TYPES[spelling]
+    if spelling.endswith("*"):
+        return ctypes.c_void_p
+    raise ValueError(f"{HEADER}: no ctypes type for the C type {spelling!r}")
+
+
+def prototypes(path=HEADER):
+    """{name: (return type, [parameter types])} of every mvsf_* function the header declares, as C type spellings."""
+    with open(path) as f:   # without comments and preprocessor lines
+        text = re.sub(r"/\*.*?\*/|//[^\n]*|^\s*#[^\n]*", " ", f.read(), flags=re.S | re.M)
+    protos = {}
+    for stmt in text.split(";"):
+        if not re.search(r"\bmvsf_\w+\s*\(", stmt):
+            continue
+        m = re.fullmatch(r"\s*([\w\s*]+?)\s*\b(mvsf_\w+)\s*\(([^()]*)\)\s*", stmt)
+        if m is None:
+            raise ValueError(f"{path}: cannot parse the declaration {' '.join(stmt.split())!r}")
+        params = [] if m.group(3).strip() == "void" else [_spelling(re.sub(r"\w+\s*$", "", p)) for p in m.group(3).split(",")]
+        protos[m.group(2)] = (_spelling(m.group(1)), params)
+    return protos
+
+
 def lib():
-    global _lib
+    global _lib, _streamed
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(f"{LIB_PATH} is missing: build it with `python -m mvsformerplusplus_b200.build` "
                                "(the hot path has no CPU/PyTorch fallback)")
         L = ctypes.CDLL(LIB_PATH)
-        L.mvsf_last_error.restype = ctypes.c_char_p
-        L.mvsf_last_error.argtypes = []
-        for name, (argt, rest) in SIGNATURES.items():
+        protos = prototypes()
+        for name, (ret, params) in protos.items():
             fn = getattr(L, name)  # AttributeError if the symbol is not exported
-            fn.argtypes = argt
-            fn.restype = rest
+            fn.restype = ctype(ret)
+            fn.argtypes = [ctype(p) for p in params]
+        _streamed = frozenset(name for name, (_, params) in protos.items() if params[-1:] == ["mvsf_stream_t"])
         _lib = L
     return _lib
 
@@ -93,27 +75,44 @@ def check(rc, what):
         raise RuntimeError(f"{what} failed (status {rc}): {msg}")
 
 
+def call(name, *args):
+    """Calls the entry point `name` and raises if it fails.  Tensors are passed as their data pointers and None as NULL;
+    an entry point that takes a stream is enqueued on the current torch stream, appended as its last argument."""
+    L = lib()
+    args = [ctypes.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else a for a in args]
+    if name in _streamed:
+        args.append(torch.cuda.current_stream().cuda_stream)
+    check(getattr(L, name)(*args), name)
+
+
+def size(name, *args):
+    """The byte count a size query (mvsf_*_workspace_bytes, mvsf_*_tc_bytes) returns through its last parameter."""
+    n = ctypes.c_size_t(0)
+    call(name, *args, ctypes.byref(n))
+    return n.value
+
+
+def workspace(name, *args, device):
+    """fp32 device buffer of at least the bytes the size query `name` asks for."""
+    return torch.empty(size(name, *args) // 4 + 4, device=device, dtype=torch.float32)
+
+
 def launch_count(reset=False):
     return int(lib().mvsf_launch_count(1 if reset else 0))
 
 
 class profile_calls:
-    """Context manager: brackets every library call with CUDA events on the current stream and reports device
-    milliseconds per entry point (used by bench.py for the roofline of the warp+correlation kernels).
-    Timing-only instrumentation; it does not change what is launched."""
+    """Context manager: brackets every library call that enqueues work (the entry points that take a stream) with CUDA
+    events on the current stream and reports device milliseconds per entry point (used by bench.py for the roofline of
+    the warp+correlation kernels).  Timing-only instrumentation; it does not change what is launched."""
 
     def __init__(self):
         self.records = []  # (name, start_event, end_event)
 
     def __enter__(self):
-        import torch
         L = lib()
         self._orig = {}
-        for name in SIGNATURES:
-            if name.endswith("_workspace_bytes") or name in ("mvsf_abi_version", "mvsf_launch_count", "mvsf_ktimer_enable",
-                                                             "mvsf_ktimer_read", "mvsf_warp_corr_plan", "mvsf_attention_split_plan",
-                                                             "mvsf_warp_corr_set_tile_path", "mvsf_warp_corr_last_selection"):
-                continue
+        for name in _streamed:
             fn = getattr(L, name)
             self._orig[name] = fn
 
@@ -134,7 +133,6 @@ class profile_calls:
         return False
 
     def summary(self):
-        import torch
         torch.cuda.synchronize()
         out = {}
         for name, s, e in self.records:

@@ -16,7 +16,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .hotpath import _ptr, _require_cuda, _stream
 
 METHODS = {"pcd": 0, "dpcd": 1}
 MAX_SRC_VIEWS = 16
@@ -57,7 +56,8 @@ def write_ply(path, xyz, rgb):
 
 def _check_scene(depths, confs, cams, images=None):
     for name, t in (("depths", depths), ("confs", confs), ("cams", cams)) + ((("images", images),) if images is not None else ()):
-        _require_cuda(t, f"fusion: {name}")
+        if not t.is_cuda:
+            raise RuntimeError(f"fusion: {name}: expected a CUDA tensor (the hot path has no CPU fallback)")
         if t.dtype != torch.float32 or not t.is_contiguous():
             raise ValueError(f"fusion: {name} must be a contiguous float32 tensor, got {t.dtype}, strides {t.stride()}")
     if depths.dim() != 3 or depths.numel() == 0:
@@ -87,23 +87,20 @@ def _method(method):
 
 
 def _workspace_ints(H, W):
-    n = ctypes.c_size_t(0)
-    _lib.check(_lib.lib().mvsf_fusion_workspace_bytes(H, W, ctypes.byref(n)), "fusion_workspace_bytes")
-    return n.value // 4
+    return _lib.size("mvsf_fusion_workspace_bytes", H, W) // 4
 
 
 def _prepare_cameras(cams):
     inv = torch.empty_like(cams)
-    _lib.check(_lib.lib().mvsf_fusion_prepare_cameras(_ptr(cams), cams.shape[0], _ptr(inv), _stream()), "fusion_prepare_cameras")
+    _lib.call("mvsf_fusion_prepare_cameras", cams, cams.shape[0], inv)
     return inv
 
 
 def _filter(method, ref, srcs, depths, confs, cams, cams_inv, thr, mask, avg, ws):
     N, H, W = depths.shape
     idx = (ctypes.c_int * len(srcs))(*srcs)
-    _lib.check(_lib.lib().mvsf_fusion_filter(method, _ptr(depths), _ptr(confs), _ptr(cams), _ptr(cams_inv), N, ref, idx, len(srcs),
-                                             H, W, *thr, _ptr(mask), _ptr(avg), _ptr(ws), ws.numel() * 4, _stream()),
-               "fusion_filter")
+    _lib.call("mvsf_fusion_filter", method, depths, confs, cams, cams_inv, N, ref, idx, len(srcs), H, W, *thr, mask, avg, ws,
+              ws.numel() * 4)
 
 
 def filter_view(ref_idx, src_idx, depths, confs, cams, method, conf=0.5, thres_view=2, thres_disp=1.0, dist_base=4.0,
@@ -135,7 +132,7 @@ def fuse_scene(depths, confs, cams, images, pairs, method, n_src_views=10, conf=
     views = [_check_views(ref, list(srcs)[:n_src_views], N) for ref, srcs in pairs]
     if not views:
         raise ValueError("fusion: empty pair list")
-    dev, R, L = depths.device, len(views), _lib.lib()
+    dev, R = depths.device, len(views)
     cams_inv = _prepare_cameras(cams)
     nws = _workspace_ints(H, W)
     masks = torch.empty(R, H, W, dtype=torch.uint8, device=dev)
@@ -151,8 +148,7 @@ def fuse_scene(depths, confs, cams, images, pairs, method, n_src_views=10, conf=
     base = 0
     for k, (ref, _) in enumerate(views):
         if counts[k]:
-            _lib.check(L.mvsf_fusion_extract(_ptr(masks[k]), _ptr(avgs[k]), _ptr(ws[k]), nws * 4, _ptr(cams_inv[ref]),
-                                             _ptr(images[ref]), _ptr(xyz[base:]), _ptr(rgb[base:]), counts[k], H, W, _stream()),
-                       "fusion_extract")
+            _lib.call("mvsf_fusion_extract", masks[k], avgs[k], ws[k], nws * 4, cams_inv[ref], images[ref], xyz[base:],
+                      rgb[base:], counts[k], H, W)
         base += counts[k]
     return xyz, rgb

@@ -17,7 +17,6 @@ Tensors crossing the seams keep the reference's logical shapes ([B,V,C,H,W] feat
 maps produced by FMT_with_pathway are channels-last in memory (a permuted view), which StageNet consumes
 without a copy; any NCHW-contiguous input is converted by a transpose kernel.
 """
-import ctypes
 import math
 
 import torch
@@ -26,14 +25,6 @@ import torch.nn as nn
 from . import _lib, packing
 from .config import load_args, stage_list, validate_args
 from .params import build_fmt, build_fpn_decoder, build_fpn_encoder, build_stage, build_vit, build_vit_decoder
-
-
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _f32c(t):
@@ -55,16 +46,14 @@ def to_nhwc(x):
         return xp
     x = _f32c(x)
     out = torch.empty((n, h, w, c), device=x.device, dtype=torch.float32)
-    L = _lib.lib()
-    _lib.check(L.mvsf_nchw_to_nhwc(_ptr(x), _ptr(out), n, c, h * w, _stream()), "nchw_to_nhwc")
+    _lib.call("mvsf_nchw_to_nhwc", x, out, n, c, h * w)
     return out
 
 
 def to_nchw(x_nhwc):
     n, h, w, c = x_nhwc.shape
     out = torch.empty((n, c, h, w), device=x_nhwc.device, dtype=torch.float32)
-    L = _lib.lib()
-    _lib.check(L.mvsf_nhwc_to_nchw(_ptr(x_nhwc), _ptr(out), n, c, h * w, _stream()), "nhwc_to_nchw")
+    _lib.call("mvsf_nhwc_to_nchw", x_nhwc, out, n, c, h * w)
     return out
 
 
@@ -73,15 +62,13 @@ def _pack_f16(entry, flat, *args, query=None):
     mvsf_<entry>(*args, flat, out, size, stream) fills (install time, once).  query = (name, *query_args):
     mvsf_<name>(*query_args, &size) gives the buffer's size in bytes.  Without a query the buffer is the hi | lo split
     of the whole blob, 2 n halves, and size = n."""
-    L = _lib.lib()
     if query is None:
         size, halves = flat.numel(), 2 * flat.numel()
     else:
-        need = ctypes.c_size_t(0)
-        _lib.check(getattr(L, "mvsf_" + query[0])(*query[1:], ctypes.byref(need)), query[0])
-        size, halves = need.value, need.value // 2
+        size = _lib.size("mvsf_" + query[0], *query[1:])
+        halves = size // 2
     out = torch.empty(halves, device=flat.device, dtype=torch.float16)
-    _lib.check(getattr(L, "mvsf_" + entry)(*args, _ptr(flat), _ptr(out), ctypes.c_size_t(size), _stream()), entry)
+    _lib.call("mvsf_" + entry, *args, flat, out, size)
     return out
 
 
@@ -108,20 +95,17 @@ def homo_warping_3D_with_mask(src_fea, src_proj, ref_proj, depth_values):
     B, C, H, W = src_fea.shape
     D = depth_values.shape[1]
     dev = src_fea.device
-    L = _lib.lib()
-    st = _stream()
     depth_values = _f32c(depth_values.to(dev))
     if depth_values.dim() == 2:  # warping.py:73-74
         depth_values = depth_values.view(B, D, 1, 1).expand(B, D, H, W).contiguous()
     sp, rp = _f32c(src_proj.to(dev)), _f32c(ref_proj.to(dev))
     homs = torch.empty((B, 12), device=dev, dtype=torch.float32)
-    _lib.check(L.mvsf_homography_from_proj(_ptr(sp), _ptr(rp), B, _ptr(homs), st), "homography_from_proj")
+    _lib.call("mvsf_homography_from_proj", sp, rp, B, homs)
     src = to_nhwc(src_fea)
     warped = torch.empty((B, C, D, H, W), device=dev, dtype=torch.float32)
     mask = torch.empty((B, D, H, W), device=dev, dtype=torch.uint8)
     for b in range(B):
-        _lib.check(L.mvsf_homo_warp(_ptr(src[b]), _ptr(homs[b]), _ptr(depth_values[b]), _ptr(warped[b]), _ptr(mask[b]),
-                                    C, D, H, W, st), "homo_warp")
+        _lib.call("mvsf_homo_warp", src[b], homs[b], depth_values[b], warped[b], mask[b], C, D, H, W)
     return warped, mask.bool()
 
 
@@ -204,8 +188,6 @@ class StageNet(_PackedMixin, nn.Module):
 
     # ---- one sample
     def _forward_one(self, feat_nhwc, proj, depth_values, tmp, position3d, pk, keep=False):
-        L = _lib.lib()
-        st = _stream()
         V, H, W, C = feat_nhwc.shape
         D = depth_values.shape[0]
         dev = feat_nhwc.device
@@ -215,51 +197,39 @@ class StageNet(_PackedMixin, nn.Module):
         f32 = dict(device=dev, dtype=torch.float32)
         homs = torch.empty((V - 1) * 12, **f32)
         kinv = torch.empty(9, **f32)
-        _lib.check(L.mvsf_compose_geometry(_ptr(proj), V, _ptr(homs), _ptr(kinv), st), "compose_geometry")
+        _lib.call("mvsf_compose_geometry", proj, V, homs, kinv)
         entropy = torch.empty((V - 1, H, W), **f32)
         vis = torch.empty((V - 1, H, W), **f32)
         volume = torch.empty((D, H, W, G), **f32)
         # spill plan (pass A stores the per-view group correlations, the aggregation streams them) unless the buffer would
         # exceed the budget: then both passes gather (TMA-staged window kernels at C = 8 / 16), no intermediate buffer
-        two_gathers = L.mvsf_warp_corr_plan(C, G, D, H, W, V, ctypes.c_size_t(self.corr_spill_budget_bytes)) == 1
+        two_gathers = _lib.lib().mvsf_warp_corr_plan(C, G, D, H, W, V, self.corr_spill_budget_bytes) == 1
         if not two_gathers:
             # pass A also stores the per-view group correlations; the view aggregation then streams them (no second gather)
             corr = torch.empty((V - 1, D, H, W, G), **f32)
-            _lib.check(L.mvsf_warp_corr_entropy_store(_ptr(feat_nhwc), _ptr(homs), _ptr(depth_values), _ptr(entropy),
-                                                      _ptr(corr), V, C, G, D, H, W, st), "warp_corr_entropy_store")
-            _lib.check(L.mvsf_vis_cnn(_ptr(entropy), _ptr(pk["vis"]), _ptr(vis), V - 1, H, W, st), "vis_cnn")
-            _lib.check(L.mvsf_corr_aggregate(_ptr(corr), _ptr(vis), _ptr(volume), V, G, D, H, W, st), "corr_aggregate")
+            _lib.call("mvsf_warp_corr_entropy_store", feat_nhwc, homs, depth_values, entropy, corr, V, C, G, D, H, W)
+            _lib.call("mvsf_vis_cnn", entropy, pk["vis"], vis, V - 1, H, W)
+            _lib.call("mvsf_corr_aggregate", corr, vis, volume, V, G, D, H, W)
             del corr
         else:
-            _lib.check(L.mvsf_warp_corr_entropy(_ptr(feat_nhwc), _ptr(homs), _ptr(depth_values), _ptr(entropy),
-                                                V, C, G, D, H, W, st), "warp_corr_entropy")
-            _lib.check(L.mvsf_vis_cnn(_ptr(entropy), _ptr(pk["vis"]), _ptr(vis), V - 1, H, W, st), "vis_cnn")
-            _lib.check(L.mvsf_warp_corr_aggregate(_ptr(feat_nhwc), _ptr(homs), _ptr(depth_values), _ptr(vis),
-                                                  _ptr(volume), V, C, G, D, H, W, st), "warp_corr_aggregate")
+            _lib.call("mvsf_warp_corr_entropy", feat_nhwc, homs, depth_values, entropy, V, C, G, D, H, W)
+            _lib.call("mvsf_vis_cnn", entropy, pk["vis"], vis, V - 1, H, W)
+            _lib.call("mvsf_warp_corr_aggregate", feat_nhwc, homs, depth_values, vis, volume, V, C, G, D, H, W)
         kept = dict(entropy=entropy, vis_weight=vis, volume_mean=volume.clone() if keep else None) if keep else None
         logits = torch.empty((D, H, W), **f32)
-        need = ctypes.c_size_t(0)
         if pk["kind"] == "tr":
-            _lib.check(L.mvsf_costreg_tr_workspace_bytes(G, D, H, W, ctypes.byref(need)), "costreg_tr_workspace_bytes")
-            ws = torch.empty(need.value // 4 + 4, **f32)
+            ws = _lib.workspace("mvsf_costreg_tr_workspace_bytes", G, D, H, W, device=dev)
             n_tok = (D // 2) * (H // 4) * (W // 4)
-            _lib.check(L.mvsf_costreg_tr_forward(_ptr(volume), _ptr(position3d), _ptr(pk["reg"]), _ptr(pk["reg16"]),
-                                                 ctypes.c_size_t(pk["reg"].numel()), _ptr(logits),
-                                                 _ptr(ws), ctypes.c_size_t(ws.numel() * 4), G, D, H, W, pk["layers"],
-                                                 float(self._softmax_scale(n_tok)), st), "costreg_tr_forward")
+            _lib.call("mvsf_costreg_tr_forward", volume, position3d, pk["reg"], pk["reg16"], pk["reg"].numel(), logits,
+                      ws, ws.numel() * 4, G, D, H, W, pk["layers"], float(self._softmax_scale(n_tok)))
         else:
-            _lib.check(L.mvsf_costreg_unet_workspace_bytes(pk["kind"], G, D, H, W, ctypes.byref(need)),
-                       "costreg_unet_workspace_bytes")
-            ws = torch.empty(need.value // 4 + 4, **f32)
-            _lib.check(L.mvsf_costreg_unet_forward(pk["kind"], _ptr(volume), _ptr(pk["reg"]), _ptr(pk["reg_tc"]),
-                                                   _ptr(logits), _ptr(ws),
-                                                   ctypes.c_size_t(ws.numel() * 4), G, D, H, W, st),
-                       "costreg_unet_forward")
+            ws = _lib.workspace("mvsf_costreg_unet_workspace_bytes", pk["kind"], G, D, H, W, device=dev)
+            _lib.call("mvsf_costreg_unet_forward", pk["kind"], volume, pk["reg"], pk["reg_tc"], logits, ws, ws.numel() * 4,
+                      G, D, H, W)
         prob = torch.empty((D, H, W), **f32)
         depth = torch.empty((H, W), **f32)
         conf = torch.empty((H, W), **f32)
-        _lib.check(L.mvsf_softargmax(_ptr(logits), _ptr(depth_values), float(tmp), _ptr(prob), _ptr(depth), _ptr(conf),
-                                     D, H, W, st), "softargmax")
+        _lib.call("mvsf_softargmax", logits, depth_values, float(tmp), prob, depth, conf, D, H, W)
         return depth, prob, conf, logits, kept
 
     @torch.no_grad()
@@ -342,13 +312,10 @@ class FMT_with_pathway(_PackedMixin, nn.Module):
         _require_cuda(f1, "FMT_with_pathway.forward(features)")
         B, V, C, H1, W1 = f1.shape
         assert C == 64, "FMT d_model must equal the stage-1 channel count"
-        L = _lib.lib()
         pk = self._pack(f1.device)
         pe = self._pe(H1, W1, f1.device)
         f32 = dict(device=f1.device, dtype=torch.float32)
-        need = ctypes.c_size_t(0)
-        _lib.check(L.mvsf_fmt_workspace_bytes(V, H1, W1, ctypes.byref(need)), "fmt_workspace_bytes")
-        ws = torch.empty(need.value // 4 + 4, **f32)
+        ws = _lib.workspace("mvsf_fmt_workspace_bytes", V, H1, W1, device=f1.device)
         outs = {k: [] for k in ("stage1", "stage2", "stage3", "stage4")}
         for b in range(B):
             ins = [_f32c(features[f"stage{k}"][b]) for k in (1, 2, 3, 4)]
@@ -356,10 +323,7 @@ class FMT_with_pathway(_PackedMixin, nn.Module):
                 if tuple(ins[k].shape) != (V, c, H1 * sc, W1 * sc):
                     raise AssertionError(f"stage{k + 1} features must be [V,{c},{H1 * sc},{W1 * sc}], got {tuple(ins[k].shape)}")
             o = [torch.empty((V, H1 * sc, W1 * sc, c), **f32) for c, sc in ((64, 1), (32, 2), (16, 4), (8, 8))]
-            _lib.check(L.mvsf_fmt_forward(_ptr(ins[0]), _ptr(ins[1]), _ptr(ins[2]), _ptr(ins[3]), _ptr(pe), _ptr(pk["w"]),
-                                          _ptr(pk["w16"]), ctypes.c_size_t(pk["w"].numel()),
-                                          _ptr(o[0]), _ptr(o[1]), _ptr(o[2]), _ptr(o[3]), _ptr(ws),
-                                          ctypes.c_size_t(ws.numel() * 4), V, H1, W1, _stream()), "fmt_forward")
+            _lib.call("mvsf_fmt_forward", *ins, pe, pk["w"], pk["w16"], pk["w"].numel(), *o, ws, ws.numel() * 4, V, H1, W1)
             for k in range(4):
                 outs[f"stage{k + 1}"].append(o[k])
         # logical [B,V,C,H,W]; channels-last in memory (StageNet consumes it without a copy)
@@ -396,7 +360,6 @@ class HotPathNet(nn.Module):
 def cascade_forward(fmt_module, fusions, args, features, proj_matrices, depth_values, tmp, keep_intermediates=False):
     """DINOv2_mvsformer_model.py:117-179 with the element-wise glue (hypothesis scheduling, 3-D positions, confidence
     averaging) as CUDA kernels.  `fusions[i]` must be this package's StageNet."""
-    L = _lib.lib()
     ndepths, ratios = args["ndepths"], args["depth_interals_ratio"]
     if fmt_module is not None:
         features = fmt_module.forward(features)
@@ -417,15 +380,12 @@ def cascade_forward(fmt_module, fusions, args, features, proj_matrices, depth_va
         _, V, C, H, W = f.shape
         D = ndepths[s]
         ds = torch.empty((B, D, H, W), **f32)
-        st = _stream()
         for b in range(B):
             if s == 0:
-                _lib.check(L.mvsf_init_inverse_range(_ptr(depth_values[b]), Dn, _ptr(ds[b]), D, H, W, st),
-                           "init_inverse_range")
+                _lib.call("mvsf_init_inverse_range", depth_values[b], Dn, ds[b], D, H, W)
             else:
-                _lib.check(L.mvsf_schedule_inverse_range(_ptr(so["depth"][b]), _ptr(so["depth_values"][b]),
-                                                         so["depth_values"].shape[1], float(ratios[s]), _ptr(ds[b]),
-                                                         D, H, W, st), "schedule_inverse_range")
+                _lib.call("mvsf_schedule_inverse_range", so["depth"][b], so["depth_values"][b], so["depth_values"].shape[1],
+                          float(ratios[s]), ds[b], D, H, W)
         p3d = None
         if args["cost_reg_type"][s] != "Normal" and args.get("use_pe3d", False):
             # position_encoding.py:138-161: extents (first PE stage only) and depth_values.min()/max() are reductions
@@ -434,23 +394,19 @@ def cascade_forward(fmt_module, fusions, args, features, proj_matrices, depth_va
             kinvs = torch.empty((B, 9), **f32)
             homs = torch.empty((V - 1) * 12, **f32)
             for b in range(B):
-                _lib.check(L.mvsf_compose_geometry(_ptr(pm[b]), V, _ptr(homs), _ptr(kinvs[b]), st), "compose_geometry")
+                _lib.call("mvsf_compose_geometry", pm[b], V, homs, kinvs[b])
                 if not have_extents:
-                    _lib.check(L.mvsf_position3d(_ptr(kinvs[b]), _ptr(ds[b]), None, 0, _ptr(stats), 2 if b == 0 else 3,
-                                                 None, D, H, W, st), "position3d(extents)")
+                    _lib.call("mvsf_position3d", kinvs[b], ds[b], None, 0, stats, 2 if b == 0 else 3, None, D, H, W)
             if not have_extents:
-                _lib.check(L.mvsf_position3d(None, None, _ptr(depth_values), B * Dn, _ptr(stats), 4, None, D, H, W, st),
-                           "position3d(finalize)")
+                _lib.call("mvsf_position3d", None, None, depth_values, B * Dn, stats, 4, None, D, H, W)
                 have_extents = True
             for b in range(B):
-                _lib.check(L.mvsf_position3d(_ptr(kinvs[b]), _ptr(ds[b]), None, 0, _ptr(stats), 5, _ptr(p3d[b]),
-                                             D, H, W, st), "position3d(normalise)")
+                _lib.call("mvsf_position3d", kinvs[b], ds[b], None, 0, stats, 5, p3d[b], D, H, W)
         so = fusions[s].forward(f, pm, ds, tmp=tmp[s], position3d=p3d, keep_intermediates=keep_intermediates)
         outputs[f"stage{s + 1}"] = so
         conf = so["photometric_confidence"]
         for b in range(B):
-            _lib.check(L.mvsf_conf_accumulate(_ptr(conf[b]), H, W, _ptr(prob_maps[b]), Hf, Wf, 1.0 / len(ndepths),
-                                              1 if s == 0 else 0, st), "conf_accumulate")
+            _lib.call("mvsf_conf_accumulate", conf[b], H, W, prob_maps[b], Hf, Wf, 1.0 / len(ndepths), 1 if s == 0 else 0)
         outputs.update(so)
     outputs["refined_depth"] = so["depth"]
     outputs["photometric_confidence"] = prob_maps
@@ -497,27 +453,20 @@ class FPNEncoder(_PackedMixin, nn.Module):
             raise AssertionError(f"FPNEncoder expects [N,3,H,W] images, got {tuple(x.shape)}")
         _check_fpn_size(H, W)
         _require_cuda(x, "FPNEncoder.forward(x)")
-        L = _lib.lib()
         pk = self._pack(x.device)
         x = _f32c(x)
         f32 = dict(device=x.device, dtype=torch.float32)
         outs = [torch.empty((N, H // s, W // s, c), **f32) for c, s in ((8, 1), (16, 2), (32, 4), (64, 8))]
-        need = ctypes.c_size_t(0)
-        _lib.check(L.mvsf_fpn_encoder_workspace_bytes(N, H, W, ctypes.byref(need)), "fpn_encoder_workspace_bytes")
-        ws = torch.empty(need.value // 4 + 4, **f32)
+        ws = _lib.workspace("mvsf_fpn_encoder_workspace_bytes", N, H, W, device=x.device)
         if vit_feat is None:
-            _lib.check(L.mvsf_fpn_encoder_forward(_ptr(x), _ptr(pk["w"]), _ptr(pk["tc"]), *[_ptr(o) for o in outs],
-                                                  _ptr(ws), ctypes.c_size_t(ws.numel() * 4), N, H, W, _stream()),
-                       "fpn_encoder_forward")
+            _lib.call("mvsf_fpn_encoder_forward", x, pk["w"], pk["tc"], *outs, ws, ws.numel() * 4, N, H, W)
         else:
             V = vit_feat.shape[0]
             if tuple(vit_feat.shape) != (V, 64, H // 8, W // 8):
                 raise AssertionError(f"FPNEncoder: vit_feat must be [V,64,{H // 8},{W // 8}], got {tuple(vit_feat.shape)}")
             _require_cuda(vit_feat, "FPNEncoder.forward(vit_feat)")
             vit = to_nhwc(vit_feat)
-            _lib.check(L.mvsf_fpn_encoder_vit_forward(_ptr(x), _ptr(vit), V, _ptr(pk["w"]), _ptr(pk["tc"]),
-                                                      *[_ptr(o) for o in outs], _ptr(ws), ctypes.c_size_t(ws.numel() * 4),
-                                                      N, H, W, _stream()), "fpn_encoder_vit_forward")
+            _lib.call("mvsf_fpn_encoder_vit_forward", x, vit, V, pk["w"], pk["tc"], *outs, ws, ws.numel() * 4, N, H, W)
         return [o.permute(0, 3, 1, 2) for o in outs]
 
 
@@ -546,17 +495,12 @@ class FPNDecoder(_PackedMixin, nn.Module):
             if tuple(t.shape) != (N, c, H // s, W // s):
                 raise AssertionError(f"FPNDecoder: expected a [{N},{c},{H // s},{W // s}] map, got {tuple(t.shape)}")
             _require_cuda(t, "FPNDecoder.forward")
-        L = _lib.lib()
         pk = self._pack(conv01.device)
         ins = [to_nhwc(t) for t in ins]
         f32 = dict(device=conv01.device, dtype=torch.float32)
         outs = [torch.empty((N, c, H // s, W // s), **f32) for c, s in ((64, 8), (32, 4), (16, 2), (8, 1))]
-        need = ctypes.c_size_t(0)
-        _lib.check(L.mvsf_fpn_decoder_workspace_bytes(N, H, W, ctypes.byref(need)), "fpn_decoder_workspace_bytes")
-        ws = torch.empty(need.value // 4 + 4, **f32)
-        _lib.check(L.mvsf_fpn_decoder_forward(*[_ptr(t) for t in ins], _ptr(pk["w"]), _ptr(pk["tc"]),
-                                              *[_ptr(o) for o in outs], _ptr(ws), ctypes.c_size_t(ws.numel() * 4),
-                                              N, H, W, _stream()), "fpn_decoder_forward")
+        ws = _lib.workspace("mvsf_fpn_decoder_workspace_bytes", N, H, W, device=conv01.device)
+        _lib.call("mvsf_fpn_decoder_forward", *ins, pk["w"], pk["tc"], *outs, ws, ws.numel() * 4, N, H, W)
         return outs
 
 
@@ -618,17 +562,12 @@ class CrossVITDecoder(_PackedMixin, nn.Module):
         for t in x:
             t = _f32c(t)
             xs.append(t if t.data_ptr() % 16 == 0 else t.clone())
-        L = _lib.lib()
         dev = xs[0].device
         pk = self._pack(dev)
         f32 = dict(device=dev, dtype=torch.float32)
         out = torch.empty((B * V, 4 * h, 4 * w, 64), **f32)
-        need = ctypes.c_size_t(0)
-        _lib.check(L.mvsf_vit_decoder_workspace_bytes(B, V, h, w, ctypes.byref(need)), "vit_decoder_workspace_bytes")
-        ws = torch.empty(need.value // 4 + 4, **f32)
-        _lib.check(L.mvsf_vit_decoder_forward(*[_ptr(t) for t in xs], _ptr(pk["w"]), _ptr(pk["tc"]), _ptr(out), _ptr(ws),
-                                              ctypes.c_size_t(ws.numel() * 4), B, V, h, w, _stream()),
-                   "vit_decoder_forward")
+        ws = _lib.workspace("mvsf_vit_decoder_workspace_bytes", B, V, h, w, device=dev)
+        _lib.call("mvsf_vit_decoder_forward", *xs, pk["w"], pk["tc"], out, ws, ws.numel() * 4, B, V, h, w)
         return out.permute(0, 3, 1, 2)
 
 
@@ -719,7 +658,6 @@ class DinoVisionTransformer(_PackedMixin, nn.Module):
         if c != 3:
             raise AssertionError(f"DinoVisionTransformer expects [n,3,H,W] images, got {tuple(x.shape)}")
         _require_cuda(x, "DinoVisionTransformer.forward_interval_features(x)")
-        L = _lib.lib()
         x = _f32c(x)
         if x.data_ptr() % 16:
             x = x.clone()
@@ -730,16 +668,11 @@ class DinoVisionTransformer(_PackedMixin, nn.Module):
         # out0 / out1 also carry the residual stream: the n cls rows follow the n * P patch rows
         outs = [torch.empty((n * (P + 1), 768), **f32), torch.empty((n * (P + 1), 768), **f32),
                 torch.empty((n * P, 768), **f32)]
-        need = ctypes.c_size_t(0)
-        _lib.check(L.mvsf_vit_workspace_bytes(n, gh, gw, ctypes.byref(need)), "vit_workspace_bytes")
-        ws = torch.empty(need.value // 4 + 4, **f32)
+        ws = _lib.workspace("mvsf_vit_workspace_bytes", n, gh, gw, device=x.device)
         if resize:
-            _lib.check(L.mvsf_vit_forward_image(_ptr(x), H, W, _ptr(pos), _ptr(pk["w"]), _ptr(pk["tc"]),
-                                                *[_ptr(o) for o in outs], _ptr(ws), ctypes.c_size_t(ws.numel() * 4), n, gh,
-                                                gw, _stream()), "vit_forward_image")
+            _lib.call("mvsf_vit_forward_image", x, H, W, pos, pk["w"], pk["tc"], *outs, ws, ws.numel() * 4, n, gh, gw)
         else:
-            _lib.check(L.mvsf_vit_forward(_ptr(x), _ptr(pos), _ptr(pk["w"]), _ptr(pk["tc"]), *[_ptr(o) for o in outs],
-                                          _ptr(ws), ctypes.c_size_t(ws.numel() * 4), n, gh, gw, _stream()), "vit_forward")
+            _lib.call("mvsf_vit_forward", x, pos, pk["w"], pk["tc"], *outs, ws, ws.numel() * 4, n, gh, gw)
         return [o[:n * P].view(n, P, 768) for o in outs]
 
 

@@ -16,11 +16,10 @@ def plan():
     from mvsformerplusplus_b200.build import build
     build()
     from mvsformerplusplus_b200 import _lib
-    L = _lib.lib()
 
     def f(N, sms):
         r, k = ctypes.c_int(-1), ctypes.c_int(-1)
-        _lib.check(L.mvsf_attention_split_plan(N, sms, ctypes.byref(r), ctypes.byref(k)), "attention_split_plan")
+        _lib.call("mvsf_attention_split_plan", N, sms, ctypes.byref(r), ctypes.byref(k))
         return r.value, k.value
     return f
 

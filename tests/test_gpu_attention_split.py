@@ -8,6 +8,7 @@ import math
 import pytest
 import torch
 
+from mvsformerplusplus_b200 import _lib
 from tests.common import max_abs, rec
 
 pytestmark = pytest.mark.gpu
@@ -16,24 +17,13 @@ MIN_PART_TILES = 16
 
 
 @pytest.fixture(scope="module")
-def L():
-    from mvsformerplusplus_b200 import _lib
-    return _lib.lib()
-
-
-@pytest.fixture(scope="module")
 def sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def P(t):
-    return ctypes.c_void_p(t.data_ptr())
-
-
-def plan(L, N, sms):
-    from mvsformerplusplus_b200 import _lib
+def plan(N, sms):
     r, k = ctypes.c_int(), ctypes.c_int()
-    _lib.check(L.mvsf_attention_split_plan(N, sms, ctypes.byref(r), ctypes.byref(k)), "attention_split_plan")
+    _lib.call("mvsf_attention_split_plan", N, sms, ctypes.byref(r), ctypes.byref(k))
     return r.value, k.value
 
 
@@ -50,20 +40,19 @@ CASES = {   # what the plan must do at N; the first N are the choices on 132 SMs
 }
 
 
-def pick(L, sms, case):
+def pick(sms, case):
     prefer, ok = CASES[case]
     for N in prefer + list(range(16000, 40000, 13)):
-        if ok(N, *plan(L, N, sms), sms):
+        if ok(N, *plan(N, sms), sms):
             return N
     pytest.skip(f"no N below 40 000 gives a {case} plan on {sms} SMs")
 
 
 @pytest.mark.parametrize("case", sorted(CASES))
-def test_split_attention_vs_fp64(L, sms, case):
-    from mvsformerplusplus_b200 import _lib
+def test_split_attention_vs_fp64(sms, case):
     dev = torch.device("cuda:0")
-    N = pick(L, sms, case)
-    r, k = plan(L, N, sms)
+    N = pick(sms, case)
+    r, k = plan(N, sms)
     assert (r > 0) == (case != "no_leftover")
     g = torch.Generator().manual_seed(N)
     qd = (torch.randn(N, 192, generator=g) * 1.5).to(dev)
@@ -73,8 +62,7 @@ def test_split_attention_vs_fp64(L, sms, case):
     for _ in range(2):
         o = torch.full((N, 64), float("nan"), device=dev)
         _lib.launch_count(reset=True)
-        _lib.check(L.mvsf_attention_forward(P(qd), P(o), P(ws), ctypes.c_size_t(ws.numel() * 4), N, float(scale),
-                                            ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "attention")
+        _lib.call("mvsf_attention_forward", qd, o, ws, ws.numel() * 4, N, float(scale))
         assert _lib.launch_count() == (3 if r else 2)   # operand tiling, attention, and the merge of the split items
         outs.append(o)
     torch.cuda.synchronize()

@@ -5,12 +5,11 @@
   * the transposed convs (one N = 4 * NPAD product per input shift, zero blocks for the classes it does not feed) with
     odd numbers of tiles in H and W;
   * both U-Net kinds end to end, with the fused OUT_F32 (CostRegNet) and OUT_PROB (CostRegNet3D) epilogues."""
-import ctypes
-
 import pytest
 import torch
 import torch.nn.functional as F
 
+from mvsformerplusplus_b200 import _lib
 from tests.common import max_abs, rec
 
 pytestmark = pytest.mark.gpu
@@ -19,25 +18,6 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope="module")
 def dev():
     return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def L():
-    from mvsformerplusplus_b200 import _lib
-    return _lib.lib()
-
-
-def P(t):
-    return ctypes.c_void_p(t.data_ptr())
-
-
-def S():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def ck(rc, what):
-    from mvsformerplusplus_b200 import _lib
-    _lib.check(rc, what)
 
 
 def _col_depth_run(D, IH, IW, mode, cin, cout):
@@ -63,7 +43,7 @@ def _col_depth_run(D, IH, IW, mode, cin, cout):
     return best
 
 
-def _layer(dev, L, mode, sd, cin, cout, ID, IH, IW, skip, seed):
+def _layer(dev, mode, sd, cin, cout, ID, IH, IW, skip, seed):
     g = torch.Generator().manual_seed(seed)
     x = torch.randn(ID, IH, IW, cin, generator=g)
     w = torch.randn(27, cin, cout, generator=g) / (27 * cin) ** 0.5 * 1.7
@@ -83,8 +63,7 @@ def _layer(dev, L, mode, sd, cin, cout, ID, IH, IW, skip, seed):
     sk_d = sk.contiguous().to(dev) if skip else None
     out = torch.empty(y.shape, device=dev)
     ws = torch.empty((2 * x.numel() + 4 * y.numel()) // 2 + 27 * cin * max(cout, 16) * 4 + 1024, device=dev)
-    ck(L.mvsf_conv3d_tc_layer(mode, sd, P(x_d), P(wb_d), P(sk_d) if skip else None, P(out), P(ws),
-                              ctypes.c_size_t(ws.numel() * 4), cin, cout, ID, IH, IW, S()), "conv3d_tc_layer")
+    _lib.call("mvsf_conv3d_tc_layer", mode, sd, x_d, wb_d, sk_d, out, ws, ws.numel() * 4, cin, cout, ID, IH, IW)
     e = float((out.cpu().double() - y).abs().max())
     return e, float(y.abs().max())
 
@@ -103,8 +82,8 @@ def test_col_cases_cover_single_and_split_depth_runs(dev):
 
 
 @pytest.mark.parametrize("mode,cin,cout,D,IH,IW", COL_CASES)
-def test_depth_streaming_conv(dev, L, mode, cin, cout, D, IH, IW):
-    e, scale = _layer(dev, L, mode, 1, cin, cout, D, IH, IW, False, seed=31 * D + cin + mode)
+def test_depth_streaming_conv(dev, mode, cin, cout, D, IH, IW):
+    e, scale = _layer(dev, mode, 1, cin, cout, D, IH, IW, False, seed=31 * D + cin + mode)
     dc = _col_depth_run(D, IH, IW, mode, cin, cout)
     rec(f"conv3d_col_mode{mode}_{cin}to{cout}_{D}x{IH}x{IW}_dc{dc}", abs=e, scale=scale)
     assert e < 1e-5 * max(1.0, scale)
@@ -114,8 +93,8 @@ def test_depth_streaming_conv(dev, L, mode, cin, cout, D, IH, IW):
 @pytest.mark.parametrize("sd,cin,cout,ID,IH,IW,skip", [
     (2, 32, 16, 3, 40, 72, True), (1, 16, 8, 5, 48, 88, True), (1, 64, 32, 3, 24, 56, True), (2, 16, 8, 1, 40, 40, False),
     (1, 8, 16, 3, 24, 40, False), (1, 32, 64, 2, 17, 23, False)])
-def test_transposed_conv_odd_tiles(dev, L, sd, cin, cout, ID, IH, IW, skip):
-    e, scale = _layer(dev, L, 2, sd, cin, cout, ID, IH, IW, skip, seed=7 * ID + cin + IW)
+def test_transposed_conv_odd_tiles(dev, sd, cin, cout, ID, IH, IW, skip):
+    e, scale = _layer(dev, 2, sd, cin, cout, ID, IH, IW, skip, seed=7 * ID + cin + IW)
     rec(f"conv3d_deconv_sd{sd}_{cin}to{cout}_{ID}x{IH}x{IW}_skip{int(skip)}", abs=e, scale=scale)
     assert e < 1e-5 * max(1.0, scale)
 
@@ -130,7 +109,7 @@ def _rand_sd(seed):
 
 # stage 1 = CostRegNet (fp32 OUT_F32 epilogue + prob3), stages 2, 3 = CostRegNet3D (fused OUT_PROB epilogue)
 @pytest.mark.parametrize("stage,D,H,W", [(1, 8, 40, 24), (1, 16, 24, 56), (2, 5, 40, 56), (3, 1, 24, 24), (3, 16, 16, 8)])
-def test_costreg_unet_pipelined(dev, L, stage, D, H, W):
+def test_costreg_unet_pipelined(dev, stage, D, H, W):
     from mvsformerplusplus_b200 import packing
     from mvsformerplusplus_b200.hotpath import pack_unet_tc
     from oracle import hotpath as O
@@ -141,15 +120,12 @@ def test_costreg_unet_pipelined(dev, L, stage, D, H, W):
     want = O.costreg_unet(vol, sd, p)[0, 0]
     kind, flat = packing.pack_costreg_unet(sd, p)
     assert kind == (0 if stage == 1 else 1)
-    need = ctypes.c_size_t(0)
-    ck(L.mvsf_costreg_unet_workspace_bytes(kind, 8, D, H, W, ctypes.byref(need)), "ws")
-    ws = torch.empty(need.value // 4 + 4, device=dev)
+    ws = _lib.workspace("mvsf_costreg_unet_workspace_bytes", kind, 8, D, H, W, device=dev)
     logits = torch.empty(D, H, W, device=dev)
     v = vol[0].permute(1, 2, 3, 0).contiguous().to(dev)
     flat_d = flat.to(dev)
     flat_tc = pack_unet_tc(kind, flat_d)
-    ck(L.mvsf_costreg_unet_forward(kind, P(v), P(flat_d), P(flat_tc), P(logits), P(ws), ctypes.c_size_t(ws.numel() * 4),
-                                   8, D, H, W, S()), "costreg_unet_forward")
+    _lib.call("mvsf_costreg_unet_forward", kind, v, flat_d, flat_tc, logits, ws, ws.numel() * 4, 8, D, H, W)
     e = max_abs(logits.cpu(), want)
     rec(f"costreg_unet_pipelined_stage{stage}_{D}x{H}x{W}", abs=e, scale=float(want.abs().max()))
     assert e < 2e-4 * max(1.0, float(want.abs().max()))

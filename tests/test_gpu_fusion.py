@@ -41,33 +41,24 @@ def test_camera_inverses(dev):
     assert float(((got.double() - want).abs() / want.abs().amax(dim=(2, 3), keepdim=True)).max()) < 1e-7
 
 
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr())
-
-
 def abi_view(sc, ref, srcs, method, thr=(0.5, 2.0, 1.0, 4.0, 1300.0)):
     """one reference view through the four C entry points -> mask bool [H,W], averaged depth, xyz [M,3], rgb [M,3]"""
-    L = _lib.lib()
     d, c, k, img = sc["depths"], sc["confs"], sc["cams"], sc["images"]
     N, H, W = d.shape
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    nbytes = ctypes.c_size_t(0)
-    _lib.check(L.mvsf_fusion_workspace_bytes(H, W, ctypes.byref(nbytes)), "workspace_bytes")
-    assert nbytes.value == 4 * ((H * W + 255) // 256 + 1)
-    ws = torch.empty(nbytes.value // 4, dtype=torch.int32, device=d.device)
+    nbytes = _lib.size("mvsf_fusion_workspace_bytes", H, W)
+    assert nbytes == 4 * ((H * W + 255) // 256 + 1)
+    ws = torch.empty(nbytes // 4, dtype=torch.int32, device=d.device)
     inv = torch.empty_like(k)
-    _lib.check(L.mvsf_fusion_prepare_cameras(_p(k), N, _p(inv), st), "prepare_cameras")
+    _lib.call("mvsf_fusion_prepare_cameras", k, N, inv)
     mask = torch.empty(H, W, dtype=torch.uint8, device=d.device)
     avg = torch.empty(H, W, dtype=torch.float32, device=d.device)
     idx = (ctypes.c_int * len(srcs))(*srcs)
-    _lib.check(L.mvsf_fusion_filter(FU.METHODS[method], _p(d), _p(c), _p(k), _p(inv), N, ref, idx, len(srcs), H, W, *thr,
-                                    _p(mask), _p(avg), _p(ws), nbytes.value, st), "filter")
+    _lib.call("mvsf_fusion_filter", FU.METHODS[method], d, c, k, inv, N, ref, idx, len(srcs), H, W, *thr, mask, avg, ws, nbytes)
     M = int(ws[-1])
     assert M == int(mask.sum())
     xyz = torch.full((M + 1, 3), -7.0, device=d.device)      # one row of room more than the survivors: it must stay untouched
     rgb = torch.full((M + 1, 3), 9, dtype=torch.uint8, device=d.device)
-    _lib.check(L.mvsf_fusion_extract(_p(mask), _p(avg), _p(ws), nbytes.value, _p(inv[ref]), _p(img[ref]), _p(xyz), _p(rgb), M, H, W,
-                                     st), "extract")
+    _lib.call("mvsf_fusion_extract", mask, avg, ws, nbytes, inv[ref], img[ref], xyz, rgb, M, H, W)
     assert bool((xyz[M] == -7.0).all()) and bool((rgb[M] == 9).all())
     return mask.bool(), avg, xyz[:M], rgb[:M]
 
@@ -225,13 +216,14 @@ def test_error_paths(dev):
     ws = torch.empty(8, dtype=torch.int32, device=dev)
     mask, avg = torch.empty(16, 24, dtype=torch.uint8, device=dev), torch.empty(16, 24, device=dev)
     idx = (ctypes.c_int * 17)(*([1] * 17))
-    st = ctypes.c_void_p(0)
     thr = (0.5, 2.0, 1.0, 4.0, 1300.0)
-    assert L.mvsf_fusion_filter(0, _p(d), _p(c), _p(k), _p(k), 3, 0, idx, 17, 16, 24, *thr, _p(mask), _p(avg), _p(ws), 32, st) == -1
+    scene_ptrs = [t.data_ptr() for t in (d, c, k, k)]
+    out_ptrs = [t.data_ptr() for t in (mask, avg, ws)]
+    assert L.mvsf_fusion_filter(0, *scene_ptrs, 3, 0, idx, 17, 16, 24, *thr, *out_ptrs, 32, None) == -1
     assert b"source views" in L.mvsf_last_error()
-    assert L.mvsf_fusion_filter(2, _p(d), _p(c), _p(k), _p(k), 3, 0, idx, 1, 16, 24, *thr, _p(mask), _p(avg), _p(ws), 32, st) == -1
-    assert L.mvsf_fusion_filter(0, _p(d), _p(c), _p(k), _p(k), 3, 0, idx, 1, 16, 24, *thr, _p(mask), _p(avg), _p(ws), 4, st) == -3
-    assert L.mvsf_fusion_filter(0, _p(d), _p(c), _p(k), _p(k), 3, 0, idx, 1, 0, 24, *thr, _p(mask), _p(avg), _p(ws), 32, st) == -1
+    assert L.mvsf_fusion_filter(2, *scene_ptrs, 3, 0, idx, 1, 16, 24, *thr, *out_ptrs, 32, None) == -1
+    assert L.mvsf_fusion_filter(0, *scene_ptrs, 3, 0, idx, 1, 16, 24, *thr, *out_ptrs, 4, None) == -3
+    assert L.mvsf_fusion_filter(0, *scene_ptrs, 3, 0, idx, 1, 0, 24, *thr, *out_ptrs, 32, None) == -1
 
 
 def test_model_to_point_cloud(dev):

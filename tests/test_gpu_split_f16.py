@@ -3,8 +3,6 @@ whole blobs by split_hi_lo_f16_kernel), through mvsf_split_weights_f16: hi and l
 conversions x.half() and (x - x.half().float()).half() bit for bit.  The inputs are adversarial: signed zeros, fp16
 subnormals, round-to-nearest-even ties, values at and just past the fp16 maximum 65504 (hi overflows to inf there, and
 lo is then -inf), fp32 extremes (largest, smallest normal, smallest subnormal) and random normals over many scales."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
@@ -38,10 +36,7 @@ def test_split_weights_f16_matches_torch_bit_for_bit(n):
     x = _inputs(n)
     xd = x.cuda()
     out = torch.full((2 * n,), float("nan"), device="cuda", dtype=torch.float16)
-    L = _lib.lib()
-    _lib.check(L.mvsf_split_weights_f16(ctypes.c_void_p(xd.data_ptr()), ctypes.c_void_p(out.data_ptr()),
-                                        ctypes.c_size_t(n), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)),
-               "split_weights_f16")
+    _lib.call("mvsf_split_weights_f16", xd, out, n)
     torch.cuda.synchronize()
     got = out.cpu().view(torch.int16)
     hi = x.half()

@@ -1,18 +1,15 @@
 """Tensor-core linear layer (linear_tc.cu, wgmma) against an fp64 GEMM evaluated with torch on the GPU (test-side ground
 truth).  The module keeps its original name (the layer first ran on tcgen05) so that its test ids stay stable.
 Run in its own process: a mis-programmed tensor-core pipeline traps the CUDA context."""
-import ctypes
 import json
 import os
 
 import pytest
 import torch
 
+from mvsformerplusplus_b200 import _lib
+
 pytestmark = pytest.mark.gpu
-
-
-def P(t):
-    return ctypes.c_void_p(t.data_ptr())
 
 
 BIAS, GELU, ELU1, RES, RES_LN, LN = range(6)
@@ -26,8 +23,6 @@ LINEAR_CASES = [(128, 192, 64, BIAS), (300, 192, 64, BIAS), (1000, 256, 64, GELU
 
 @pytest.mark.parametrize("M,N,K,epi", LINEAR_CASES, ids=[f"{EPI_NAMES[e]}-M{M}-N{N}-K{K}" for M, N, K, e in LINEAR_CASES])
 def test_linear_tc_vs_fp64(M, N, K, epi):
-    from mvsformerplusplus_b200 import _lib
-    L = _lib.lib()
     dev = torch.device("cuda:0")
     g = torch.Generator().manual_seed(M + N + K)
     A = (torch.randn(M, K, generator=g) * 1.5).to(dev)
@@ -35,10 +30,8 @@ def test_linear_tc_vs_fp64(M, N, K, epi):
     b = (0.1 * torch.randn(N, generator=g)).to(dev)
     C = torch.full((M, N), float("nan"), device=dev)
     ws = torch.empty(((M + N) * 2 * K * 2 + 1024) // 4 + 64, device=dev)
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    NP = ctypes.c_void_p(None)
-    _lib.check(L.mvsf_linear_tc_epilogue(epi, P(A), K, P(W), P(b), NP, 0, NP, NP, NP, 1e-5, 0, P(C), N, NP, 0, NP, 0,
-                                         P(ws), ctypes.c_size_t(ws.numel() * 4), M, N, K, st), "linear_tc_epilogue")
+    _lib.call("mvsf_linear_tc_epilogue", epi, A, K, W, b, None, 0, None, None, None, 1e-5, 0, C, N, None, 0, None, 0, ws,
+              ws.numel() * 4, M, N, K)
     torch.cuda.synchronize()
     gelu = epi == GELU
     want = A.double() @ W.double().t() + b.double()
@@ -117,9 +110,7 @@ def _check_spare_nan(buf, M, N, what):
 
 @pytest.mark.parametrize("epi,N,K,M,bias,outs,extra", EPI_CASES, ids=[_epi_id(c) for c in EPI_CASES])
 def test_linear_tc_epilogue_vs_fp64(epi, N, K, M, bias, outs, extra):
-    from mvsformerplusplus_b200 import _lib
     from tests.common import rec
-    L = _lib.lib()
     dev = torch.device("cuda:0")
     name = "linear_tc_epi_" + _epi_id((epi, N, K, M, bias, outs, extra))
     outs = set(outs.split("+"))
@@ -149,14 +140,10 @@ def test_linear_tc_epilogue_vs_fp64(epi, N, K, M, bias, outs, extra):
     else:
         Cpre, ldcpre = None, 0
     ws = torch.empty(((M + N) * 2 * K * 2 + 1024) // 4 + 64, device=dev)
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    NP = ctypes.c_void_p(None)
-    ptr = lambda t: P(t) if t is not None else NP
     eps = extra if epi in (RES_LN, LN) else 1e-5
     elu_cols = extra if epi == ELU1 else 0
-    _lib.check(L.mvsf_linear_tc_epilogue(epi, P(A), lda, P(W), ptr(b), ptr(res), ldres, P(gamma), P(ln_w), P(ln_b),
-                                         float(eps), elu_cols, ptr(C), ldc, ptr(Cpre), ldcpre, ptr(C2), ldc2,
-                                         P(ws), ctypes.c_size_t(ws.numel() * 4), M, N, K, st), "linear_tc_epilogue")
+    _lib.call("mvsf_linear_tc_epilogue", epi, A, lda, W, b, res, ldres, gamma, ln_w, ln_b, float(eps), elu_cols, C, ldc,
+              Cpre, ldcpre, C2, ldc2, ws, ws.numel() * 4, M, N, K)
     torch.cuda.synchronize()
 
     t = A[:, :K].double() @ W.double().t()

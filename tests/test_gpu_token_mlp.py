@@ -5,25 +5,16 @@ pre-norm block, last pre-norm block, post-norm layer.  M covers one row, partial
 CTA running a second tile (SMs * 128 + 1) and the FMT source-view batch at DTU (110 592 rows).  The MLP runs in place
 (C aliases res), as both callers run it.  Run in its own process: a mis-programmed tensor-core pipeline traps the CUDA
 context."""
-import ctypes
-
 import pytest
 import torch
 
+from mvsformerplusplus_b200 import _lib
 from tests.test_gpu_tcgen05 import EPI_TOL, GELU, RES, RES_LN
 
 pytestmark = pytest.mark.gpu
 
 PRE, PRE_LAST, POST = 0, 1, 2
 SPARE = 3   # rows past M in every output buffer, NaN-filled: the kernel must not write them
-
-
-def P(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(None)
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _inputs(M, form, dev):
@@ -40,30 +31,24 @@ def _nan(rows, cols, dtype, dev):
 
 
 def _fused(form, M, t, dev):
-    from mvsformerplusplus_b200 import _lib
     C = _nan(M + SPARE, 64, torch.float32, dev)
     C[:M] = t["res"]
     C2 = _nan(M + SPARE, 128, torch.float16, dev) if form != PRE_LAST else None
     ws = torch.empty((M * 128 + 73728) // 2 + 64, device=dev)
-    _lib.check(_lib.lib().mvsf_token_mlp_forward(
-        form, P(t["A"]), P(C), P(t["proj_w"]), P(t["proj_b"]), P(t["gamma1"]), P(t["mid_w"]), P(t["mid_b"]), 1e-5,
-        P(t["f1_w"]), P(t["f1_b"]), P(t["f2_w"]), P(t["f2_b"]), P(t["gamma2"]), P(t["out_w"]), P(t["out_b"]), 1e-6,
-        P(C), P(C2), P(ws), ctypes.c_size_t(ws.numel() * 4), M, _stream()), "token_mlp_forward")
+    _lib.call("mvsf_token_mlp_forward", form, t["A"], C, t["proj_w"], t["proj_b"], t["gamma1"], t["mid_w"], t["mid_b"], 1e-5,
+              t["f1_w"], t["f1_b"], t["f2_w"], t["f2_b"], t["gamma2"], t["out_w"], t["out_b"], 1e-6, C, C2, ws,
+              ws.numel() * 4, M)
     return C, C2
 
 
 def _three_gemms(form, M, t, dev):
     """proj, FFN1 and FFN2 as the single GEMMs with fused epilogues: fp32 intermediates re-split inside each call round
     exactly as the fp16 hi|lo outputs the callers used to chain"""
-    from mvsformerplusplus_b200 import _lib
-    L = _lib.lib()
     ws = torch.empty((M + 256) * 2 * 256 * 2 // 4 + 64, device=dev)
-    wsb = ctypes.c_size_t(ws.numel() * 4)
 
     def gemm(epi, A, K, W, bias, res, gamma, ln_w, ln_b, eps, C, Cpre, C2, N):
-        _lib.check(L.mvsf_linear_tc_epilogue(epi, P(A), K, P(W), P(bias), P(res), 64, P(gamma), P(ln_w), P(ln_b),
-                                             float(eps), 0, P(C), N, P(Cpre), 64, P(C2), 128, P(ws), wsb, M, N, K,
-                                             _stream()), "linear_tc_epilogue")
+        _lib.call("mvsf_linear_tc_epilogue", epi, A, K, W, bias, res, 64, gamma, ln_w, ln_b, float(eps), 0, C, N, Cpre, 64,
+                  C2, 128, ws, ws.numel() * 4, M, N, K)
 
     x = t["res"].clone()
     mid = torch.empty(M, 64, device=dev)   # LN_mid(...): the FFN input (and, post-norm, FFN2's residual)

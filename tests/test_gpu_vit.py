@@ -3,13 +3,12 @@
 restatement at full size, and through install() with the reference's glue.
 Bars: attention within 2e-4 * max|ref| (fp16 P, measured worst 1.2e-4); every module output within
 1e-4 * max(1, max|ref|).  Errors go to rec()."""
-import ctypes
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from mvsformerplusplus_b200 import synth
+from mvsformerplusplus_b200 import _lib, synth
 from oracle import vit as OVT
 from tests.common import load_golden, max_abs, rec
 from tests.fpn_common import fpn_state_dict
@@ -28,19 +27,11 @@ def dev():
     return torch.device("cuda:0")
 
 
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr())
-
-
 def _attention(qkv, n, N, ldo=776):
     """qkv [n*N][ldq] (row stride ldq >= 2304) -> out [n*N][ldo] NaN-filled, valid columns [:768]"""
-    from mvsformerplusplus_b200 import _lib
-    L = _lib.lib()
     out = torch.full((n * N, ldo), float("nan"), device=qkv.device)
     ws = torch.empty(n * 12 * ((N + 127) // 128) * 100352 // 4 + 64, device=qkv.device)
-    _lib.check(L.mvsf_vit_attention_forward(_p(qkv), qkv.stride(0), _p(out), ldo, _p(ws), ctypes.c_size_t(ws.numel() * 4),
-                                            n, N, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)),
-               "vit_attention_forward")
+    _lib.call("mvsf_vit_attention_forward", qkv, qkv.stride(0), out, ldo, ws, ws.numel() * 4, n, N)
     return out
 
 

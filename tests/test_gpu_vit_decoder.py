@@ -2,13 +2,12 @@
 GEMM it runs on (csrc/linear_tc.cu, mvsf_linear_tc_streamed_epilogue) against fp64 references, the reference-executed
 fixtures, the fp32 restatement at full size, and through install() with the reference's glue.
 Bar: every output within 1e-4 * max(1, max|ref|); errors go to rec()."""
-import ctypes
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from mvsformerplusplus_b200 import synth
+from mvsformerplusplus_b200 import _lib, synth
 from oracle import vit_decoder as OV
 from tests.common import load_golden, max_abs, rec
 from tests.fpn_common import fpn_state_dict
@@ -26,10 +25,6 @@ def dev():
     return torch.device("cuda:0")
 
 
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
 # (epilogue, M, N, K, elu_cols, write C2): every epilogue at N 768 and 3072, K 768 / 3072 / 6912, M not a multiple of 128
 GEMM_CASES = [
     (BIAS, 1728, 768, 768, 0, False), (BIAS, 6913, 3072, 6912, 0, True), (GELU, 2040, 3072, 768, 0, True),
@@ -42,8 +37,6 @@ GEMM_CASES = [
 
 @pytest.mark.parametrize("epi,M,N,K,elu_cols,c2", GEMM_CASES)
 def test_streamed_gemm_vs_fp64(dev, epi, M, N, K, elu_cols, c2):
-    from mvsformerplusplus_b200 import _lib
-    L = _lib.lib()
     g = torch.Generator(device=dev).manual_seed(M + N + K + epi)
     A = torch.randn(M, K + 4, device=dev, generator=g)[:, :K]            # lda = K + 4: strided rows
     W = torch.randn(N, K, device=dev, generator=g) / K ** 0.5
@@ -54,10 +47,8 @@ def test_streamed_gemm_vs_fp64(dev, epi, M, N, K, elu_cols, c2):
     C = torch.full((M, ldc), float("nan"), device=dev)
     C2 = torch.full((M, 2 * N + 8), float("nan"), device=dev, dtype=torch.float16) if c2 else None
     ws = torch.empty(((M + N) * 2 * K * 2 + 256) // 4 + 64, device=dev)
-    rc = L.mvsf_linear_tc_streamed_epilogue(epi, _p(A), K + 4, _p(W), _p(bias), _p(res), N, _p(gamma), elu_cols, _p(C),
-                                            ldc, _p(C2), 2 * N + 8, _p(ws), ctypes.c_size_t(ws.numel() * 4), M, N, K,
-                                            ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-    _lib.check(rc, "linear_tc_streamed_epilogue")
+    _lib.call("mvsf_linear_tc_streamed_epilogue", epi, A, K + 4, W, bias, res, N, gamma, elu_cols, C, ldc, C2, 2 * N + 8, ws,
+              ws.numel() * 4, M, N, K)
     t = A.double() @ W.double().t() + bias.double()
     if epi == GELU:
         t = F.gelu(t)

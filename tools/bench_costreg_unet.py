@@ -16,7 +16,6 @@ those give on an H100 SXM data sheet (989 TFLOP/s dense FP16, 3.35 TB/s HBM3; bo
   python tools/bench_costreg_unet.py [--workload dtu|tt] [--reps 20] [--warmup 3] [--prof-reps 5]
 """
 import argparse
-import ctypes
 import json
 import os
 import subprocess
@@ -115,15 +114,7 @@ def main():
         raise SystemExit("bench_costreg_unet: no CUDA device (timings are only taken on the GPU)")
     from mvsformerplusplus_b200 import _lib
     from mvsformerplusplus_b200.hotpath import pack_unet_tc
-    L = _lib.lib()
     dev = torch.device("cuda:0")
-
-    def P(t):
-        return ctypes.c_void_p(t.data_ptr())
-
-    def S():
-        return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
     torch.manual_seed(0)
     sd = synth.randomize_state_dict(build_hotpath_params(default_args()).eval(), seed=13)
     H0, W0 = WORKLOADS[a.workload]
@@ -136,15 +127,12 @@ def main():
         kind, flat = packing.pack_costreg_unet(sd, f"fusions.{fi}.cost_reg.")
         flat_d = flat.to(dev)
         flat_tc = pack_unet_tc(kind, flat_d)
-        need = ctypes.c_size_t(0)
-        _lib.check(L.mvsf_costreg_unet_workspace_bytes(kind, 8, D, H, W, ctypes.byref(need)), "ws")
-        ws = torch.empty(need.value // 4 + 4, device=dev)
+        ws = _lib.workspace("mvsf_costreg_unet_workspace_bytes", kind, 8, D, H, W, device=dev)
         vol = (torch.randn(D, H, W, 8, generator=torch.Generator().manual_seed(stage)) * 0.5).to(dev)
         logits = torch.empty(D, H, W, device=dev)
 
         def fwd():
-            _lib.check(L.mvsf_costreg_unet_forward(kind, P(vol), P(flat_d), P(flat_tc), P(logits), P(ws),
-                                                   ctypes.c_size_t(ws.numel() * 4), 8, D, H, W, S()), "costreg_unet_forward")
+            _lib.call("mvsf_costreg_unet_forward", kind, vol, flat_d, flat_tc, logits, ws, ws.numel() * 4, 8, D, H, W)
 
         for _ in range(a.warmup):
             fwd()

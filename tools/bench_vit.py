@@ -7,7 +7,6 @@ one JSON line.
   python tools/bench_vit.py [--reps 20] [--warmup 3] [--workloads dtu,tt]
 """
 import argparse
-import ctypes
 import json
 import os
 import sys
@@ -54,7 +53,6 @@ def main():
     sd_dev = {k: v.to(dev) for k, v in sd.items()}
     name, power = card()
     res = {"bench": "vit", "device": name, "power_limit": power, "reps": a.reps, "warmup": a.warmup, "workloads": {}}
-    L = _lib.lib()
     for wl in a.workloads.split(","):
         n, gh, gw = WORKLOADS[wl]
         img = synth.make_images(n, 14 * gh, 14 * gw, seed=1).to(dev)
@@ -86,10 +84,8 @@ def main():
         qkv = torch.randn(n * N, 2304, device=dev)
         out = torch.empty(n * N, 768, device=dev)
         ws = torch.empty(n * 12 * ((N + 127) // 128) * 100352 // 4 + 64, device=dev)
-        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        att_ms = timed(lambda: _lib.check(L.mvsf_vit_attention_forward(
-            ctypes.c_void_p(qkv.data_ptr()), 2304, ctypes.c_void_p(out.data_ptr()), 768, ctypes.c_void_p(ws.data_ptr()),
-            ctypes.c_size_t(ws.numel() * 4), n, N, st), "vit_attention_forward"), a.warmup, a.reps)
+        att_ms = timed(lambda: _lib.call("mvsf_vit_attention_forward", qkv, 2304, out, 768, ws, ws.numel() * 4, n, N),
+                       a.warmup, a.reps)
         del qkv, out, ws
         res["workloads"][wl] = {
             "images": n, "patches": [gh, gw], "gflop_per_depth_map": {"linears": round(lin, 1), "attention": round(att, 1)},
