@@ -247,12 +247,11 @@ int mvsf_fpn_pack_tc(int part, const float* wts, void* wts_tc, size_t wts_tc_byt
 /* ---- V1: models/module.py:273-364 CrossVITDecoder.forward, shipped config (d_model 768, 12 heads, linear attention,
  *      ffn 768 -> 3072, LayerScale, pre-norm CrossBlocks with pre_norm_query, 3 interval layers, eval-mode BN folded).
  * x0, x1, x2 [B][V][h*w][768] (the ViT tokens of dinov2.py:249-266 without the cls token, view 0 = reference)
- * -> out [B*V][4h][4w][64] (NHWC).  wts: packing.pack_vit_decoder (layout in csrc/vit_decoder.cu: the GEMM weights as
- * [N][K] rows, then norms, biases, LayerScales, prev_values and folded conv biases; 37 863 880 floats).
- * wts_tc = mvsf_vit_decoder_pack_tc(wts).  Bad shapes (B < 1, V < 2, h or w outside [1, 2048)): -1, nothing launched. */
+ * -> out [B*V][4h][4w][64] (NHWC).  wts: the small fp32 parameters (small part of packing.pack_vit_decoder, layout in
+ * csrc/vit_decoder.cu: norms, biases, LayerScales, prev_values and folded conv biases; 49 608 floats); wts_tc =
+ * mvsf_split_weights_f16(GEMM part of packing.pack_vit_decoder: the GEMM and conv weights as [N][K] rows, 37 814 272
+ * floats).  Bad shapes (B < 1, V < 2, h or w outside [1, 2048)): -1, nothing launched. */
 int mvsf_vit_decoder_workspace_bytes(int B, int V, int h, int w, size_t* bytes);
-int mvsf_vit_decoder_tc_bytes(size_t* bytes);
-int mvsf_vit_decoder_pack_tc(const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
 int mvsf_vit_decoder_forward(const float* x0, const float* x1, const float* x2, const float* wts, const void* wts_tc,
                              float* out, void* workspace, size_t workspace_bytes, int B, int V, int h, int w,
                              mvsf_stream_t stream);
@@ -264,12 +263,10 @@ int mvsf_vit_decoder_forward(const float* x0, const float* x1, const float* x2, 
  * (dinov2.py:176-200, computed once per grid at pack time).  Outputs, cls token dropped: out0 = block 3, out1 = block 7,
  * out2 = norm(block 11), each [n][gh gw][768] in its first n gh gw rows; out0 and out1 also hold the residual stream and
  * need n (gh gw + 1) rows (the n cls rows come after the patch rows), out2 needs n gh gw rows.
- * wts: the small fp32 parameters (tail of packing.pack_vit, layout in csrc/vit.cu, 141 312 floats); wts_tc =
- * mvsf_vit_pack_tc(GEMM prefix of packing.pack_vit: 85 426 176 floats).  Bad shapes (n outside [1, 65535], gh or gw
- * outside [1, 1024], n (gh gw + 1) > 2^21), null or misaligned pointers: -1; short workspace: -3; nothing launched. */
+ * wts: the small fp32 parameters (small part of packing.pack_vit, layout in csrc/vit.cu, 141 312 floats); wts_tc =
+ * mvsf_split_weights_f16(GEMM part of packing.pack_vit: 85 426 176 floats).  Bad shapes (n outside [1, 65535], gh or
+ * gw outside [1, 1024], n (gh gw + 1) > 2^21), null or misaligned pointers: -1; short workspace: -3; nothing launched. */
 int mvsf_vit_workspace_bytes(int n, int gh, int gw, size_t* bytes);
-int mvsf_vit_tc_bytes(size_t* bytes);
-int mvsf_vit_pack_tc(const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
 int mvsf_vit_forward(const float* img, const float* pos, const float* wts, const void* wts_tc, float* out0, float* out1,
                      float* out2, void* workspace, size_t workspace_bytes, int n, int gh, int gw, mvsf_stream_t stream);
 /* The same forward on images of any size: img [n][3][H][W] fp32 (contiguous) is resized to 14 gh x 14 gw as

@@ -21,12 +21,13 @@ namespace mvsf {
 namespace vit {
 
 constexpr int D = 768, HID = 3072, NBLK = 12, PATCH = 14, KP = 588, KPAD = 640;
-// ---- GEMM weights (packing.pack_vit), fp32 [N][K] rows; the tc blob holds their hi / lo splits with the same indexing
+// ---- GEMM weights (the gemm part of packing.pack_vit), fp32 [N][K] rows; the tc blob holds their hi / lo splits with
+// the same indexing
 constexpr size_t G_PATCH = 0, G_BLK0 = (size_t)D * KPAD;   // patch_embed.proj [768][640] (k = c * 196 + ky * 14 + kx)
 constexpr size_t G_QKV = 0, G_PROJ = (size_t)3 * D * D, G_FC1 = (size_t)4 * D * D, G_FC2 = G_FC1 + (size_t)HID * D,
                  G_BLK = G_FC2 + (size_t)D * HID;
 constexpr size_t NG = G_BLK0 + NBLK * G_BLK;
-// ---- small fp32 parameters (the tail of packing.pack_vit, kept on the device on their own): per block norm1 w, b,
+// ---- small fp32 parameters (the small part of packing.pack_vit, the wts argument): per block norm1 w, b,
 // qkv bias [2304], proj bias, ls1, norm2 w, b, fc1 bias [3072], fc2 bias, ls2; then patch bias, cls token, norm w, b
 constexpr size_t S_N1W = 0, S_N1B = D, S_QKVB = 2 * D, S_PB = 5 * D, S_LS1 = 6 * D, S_N2W = 7 * D, S_N2B = 8 * D,
                  S_F1B = 9 * D, S_F2B = 13 * D, S_LS2 = 14 * D, S_BLK = 15 * D;
@@ -201,19 +202,6 @@ extern "C" int mvsf_vit_workspace_bytes(int n, int gh, int gw, size_t* bytes) {
                n, gh, gw);
   *bytes = layout(n, gh, gw).total * sizeof(float);
   return MVSF_OK;
-}
-
-extern "C" int mvsf_vit_tc_bytes(size_t* bytes) {
-  MVSF_REQUIRE(bytes, "vit_tc_bytes: null pointer");
-  *bytes = NG * 2 * sizeof(__half);
-  return MVSF_OK;
-}
-
-extern "C" int mvsf_vit_pack_tc(const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream) {
-  MVSF_REQUIRE(wts && wts_tc && ((uintptr_t)wts_tc & 15) == 0, "vit_pack_tc: bad arguments");
-  MVSF_REQUIRE(wts_tc_bytes >= NG * 2 * sizeof(__half), "vit_pack_tc: wts_tc too small");
-  __half* hi = static_cast<__half*>(wts_tc);
-  return launch_split_f16(wts, NG, hi, 2 * NG, 1, NG, (cudaStream_t)stream);
 }
 
 extern "C" int mvsf_vit_attention_forward(const float* qkv, int ldq, float* out, int ldo, void* workspace,

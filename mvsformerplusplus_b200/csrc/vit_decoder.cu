@@ -19,20 +19,23 @@ constexpr int D = 768, HID = 3072, NBLK = 5;   // blocks: self0, self1, cross0, 
 using Attn = LinAttn<12, 64>;
 constexpr int KVSZ = Attn::KVSZ;
 
-// ---- packed fp32 blob (packing.pack_vit_decoder).  GEMM weights first, as [N][K] rows (the tc blob splits this prefix)
+// ---- GEMM weights (the gemm part of packing.pack_vit_decoder), fp32 [N][K] rows; the tc blob holds their hi / lo
+// splits with the same indexing
 constexpr size_t G_QKV = 0, G_PROJ = (size_t)3 * D * D, G_FC1 = (size_t)4 * D * D, G_FC2 = G_FC1 + (size_t)HID * D,
                  G_BLK = G_FC2 + (size_t)D * HID;
 constexpr size_t G_CONV = NBLK * G_BLK;                       // [256][9 taps * 768]     tap = ky * 3 + kx
 constexpr size_t G_UP0 = G_CONV + (size_t)256 * 9 * D;        // [4 classes][128][4 taps * 256]
 constexpr size_t G_UP1 = G_UP0 + (size_t)4 * 128 * 4 * 256;   // [4 classes][64][4 taps * 128]
 constexpr size_t NG = G_UP1 + (size_t)4 * 64 * 4 * 128;
-// small parameters per block: norm1 w, b, proj bias, ls1, norm2 w, b, fc1 bias [3072], fc2 bias, ls2
+// ---- small fp32 parameters (the small part of packing.pack_vit_decoder, the wts argument): per block norm1 w, b,
+// proj bias, ls1, norm2 w, b, fc1 bias [3072], fc2 bias, ls2
 constexpr size_t S_N1W = 0, S_N1B = D, S_PB = 2 * D, S_LS1 = 3 * D, S_N2W = 4 * D, S_N2B = 5 * D, S_F1B = 6 * D,
                  S_F2B = S_F1B + HID, S_LS2 = S_F2B + D, S_BLK = S_LS2 + D;
-constexpr size_t P_SMALL = NG, P_NORM = P_SMALL + NBLK * S_BLK,   // norm_layers[0] w, b, norm_layers[1] w, b
-                 P_PREV = P_NORM + 4 * D,                           // prev_values[0], [1], 6 floats of padding
-                 P_CB = P_PREV + 8,                                 // folded conv biases: proj [256], up0 [128], up1 [64]
+constexpr size_t P_NORM = NBLK * S_BLK,   // norm_layers[0] w, b, norm_layers[1] w, b
+                 P_PREV = P_NORM + 4 * D, // prev_values[0], [1], 6 floats of padding
+                 P_CB = P_PREV + 8,       // folded conv biases: proj [256], up0 [128], up1 [64]
                  N_WTS = P_CB + 448;
+static_assert(NG == 37814272 && N_WTS == 49608, "packing.VIT_DECODER_GEMM_WTS / VIT_DECODER_SMALL_WTS");
 
 // x <- LN_a(prev * x + xi)  (module.py:337-339,350-352: combine + norm_layers, eps 1e-6);  y2 <- split(LN_b(x)) when ln_b
 // weights are given (norm1 of the next block, eps 1e-5)
@@ -59,8 +62,8 @@ combine_kernel(float* __restrict__ x, const float* __restrict__ xi, const float*
 struct Ws {
   __half *xn2, *att2, *hid2;   // [Mx][2D], [Mx][2D], [Mx][2 HID] halves
   float *qkv, *kvp, *kvf, *kvc; // qkv >= max(L * 3D, Ms * D) floats; kvc [3][KVSZ]
-  const float* w;               // fp32 blob
-  const __half *wh, *wl;        // tc blob: hi / lo parts of the GEMM prefix
+  const float* w;               // small fp32 parameters
+  const __half *wh, *wl;        // tc blob: hi / lo parts of the GEMM weights
 };
 
 static TcsArgs gemm(const Ws& ws, const __half* A, int lda, int K, size_t woff, int N, int M) {
@@ -80,7 +83,7 @@ static int cross_kv(const float* r, int L, int blk, float* kvc_out, const Ws& ws
 // one CrossBlock over M tokens at x (in place): self attention when kvc == nullptr (M == L), else cross attention
 // against the summary kvc.  ln1_ready: ws.xn2 already holds split(norm1(x)).
 static int run_block(float* x, int M, int L, int blk, const float* kvc, bool ln1_ready, const Ws& ws, cudaStream_t s) {
-  const float* sp = ws.w + P_SMALL + blk * S_BLK;
+  const float* sp = ws.w + blk * S_BLK;
   int rc;
   if (!ln1_ready) {
     layernorm_split_kernel<D><<<cdiv(M, 8), 256, 0, s>>>(x, sp + S_N1W, sp + S_N1B, ws.xn2, M, 1e-5f);
@@ -117,7 +120,7 @@ static int run_block(float* x, int M, int L, int blk, const float* kvc, bool ln1
 
 static int combine(float* x, const float* xi, int M, int i, int next_blk, const Ws& ws, cudaStream_t s) {
   const float* nl = ws.w + P_NORM + 2 * i * D;
-  const float* nb = next_blk >= 0 ? ws.w + P_SMALL + next_blk * S_BLK : nullptr;
+  const float* nb = next_blk >= 0 ? ws.w + next_blk * S_BLK : nullptr;
   combine_kernel<<<cdiv(M, 8), 256, 0, s>>>(x, xi, ws.w + P_PREV + i, nl, nl + D, nb ? nb + S_N1W : nullptr,
                                             nb ? nb + S_N1B : nullptr, ws.xn2, M);
   MVSF_LAUNCH_CHECK("vit_decoder_combine");
@@ -175,19 +178,6 @@ extern "C" int mvsf_vit_decoder_workspace_bytes(int B, int V, int h, int w, size
                V, h, w);
   *bytes = layout(B, V, h, w).total * sizeof(float);
   return MVSF_OK;
-}
-
-extern "C" int mvsf_vit_decoder_tc_bytes(size_t* bytes) {
-  MVSF_REQUIRE(bytes, "vit_decoder_tc_bytes: null pointer");
-  *bytes = NG * 2 * sizeof(__half);
-  return MVSF_OK;
-}
-
-extern "C" int mvsf_vit_decoder_pack_tc(const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream) {
-  MVSF_REQUIRE(wts && wts_tc && ((uintptr_t)wts_tc & 15) == 0, "vit_decoder_pack_tc: bad arguments");
-  MVSF_REQUIRE(wts_tc_bytes >= NG * 2 * sizeof(__half), "vit_decoder_pack_tc: wts_tc too small");
-  __half* hi = static_cast<__half*>(wts_tc);
-  return launch_split_f16(wts, NG, hi, 2 * NG, 1, NG, (cudaStream_t)stream);
 }
 
 extern "C" int mvsf_vit_decoder_forward(const float* x0, const float* x1, const float* x2, const float* wts,

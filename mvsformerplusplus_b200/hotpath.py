@@ -544,8 +544,9 @@ class CrossVITDecoder(_PackedMixin, nn.Module):
         self._init_packing()
 
     def _build_pack(self, device):
-        w = packing.pack_vit_decoder(self.state_dict()).to(device)
-        return {"w": w, "tc": _pack_f16("vit_decoder_pack_tc", w, query=("vit_decoder_tc_bytes",))}
+        gemm, small = packing.pack_vit_decoder(self.state_dict())
+        tc = split_weights_f16(gemm.to(device))
+        return {"w": small.to(device), "tc": tc}
 
     @torch.no_grad()
     def forward(self, x, Fmats=None, vit_shape=None):
@@ -615,12 +616,9 @@ class DinoVisionTransformer(_PackedMixin, nn.Module):
         self._init_packing()
 
     def _build_pack(self, device):
-        blob = packing.pack_vit(self.state_dict()).to(device)
-        tc = _pack_f16("vit_pack_tc", blob, query=("vit_tc_bytes",))
-        # keep the fp16 hi / lo GEMM weights and the small fp32 parameters, not the fp32 GEMM weights
-        w = blob[packing.VIT_GEMM_WTS:].clone()
-        del blob
-        return {"w": w, "tc": tc, "pos": {}}
+        gemm, small = packing.pack_vit(self.state_dict())
+        tc = split_weights_f16(gemm.to(device))
+        return {"w": small.to(device), "tc": tc, "pos": {}}
 
     def _pos(self, pk, gh, gw):
         """interpolated pos_embed of the grid (a weight transform), cached with the packed weights"""

@@ -141,7 +141,8 @@ def pack_fmt(sd, p="FMT_module."):
 
 
 VIT_DECODER_BLOCKS = tuple(f"self_attn_blocks.{i}." for i in range(2)) + tuple(f"cross_attn_blocks.{i}." for i in range(3))
-VIT_DECODER_WTS = 37863880   # floats of the packed blob (csrc/vit_decoder.cu N_WTS)
+VIT_DECODER_GEMM_WTS = 37814272   # floats of the GEMM part of pack_vit_decoder (csrc/vit_decoder.cu NG)
+VIT_DECODER_SMALL_WTS = 49608     # floats of its small-parameter part (csrc/vit_decoder.cu N_WTS)
 
 
 def deconv_class_taps(py):
@@ -151,12 +152,12 @@ def deconv_class_taps(py):
 
 
 def pack_vit_decoder(sd, p=""):
-    """models/module.py:273-364 -> the fp32 blob of mvsf_vit_decoder_forward (layout in csrc/vit_decoder.cu).
-    GEMM weights as [N][K] rows: per block (self0, self1, cross0, cross1, cross2) [q; k; v] [2304][768], proj, fc1, fc2;
-    the 3x3 proj conv [256][tap * 768 + ci] (tap = ky * 3 + kx) and, per parity class (py, px) of the two transposed
-    convs, [co][tap * ci_n + ci] over the class's 2 x 2 gather taps; BN scale folded into every conv.  Then per block
-    norm1 w, b, proj bias, ls1, norm2 w, b, fc1 bias, fc2 bias, ls2; norm_layers; prev_values (padded to 8); the folded
-    conv biases [256], [128], [64]."""
+    """models/module.py:273-364 -> (gemm, small), the two fp32 parts of mvsf_vit_decoder_forward's weights (layout in
+    csrc/vit_decoder.cu).  gemm, the GEMM weights as [N][K] rows: per block (self0, self1, cross0, cross1, cross2)
+    [q; k; v] [2304][768], proj, fc1, fc2; the 3x3 proj conv [256][tap * 768 + ci] (tap = ky * 3 + kx) and, per parity
+    class (py, px) of the two transposed convs, [co][tap * ci_n + ci] over the class's 2 x 2 gather taps; BN scale
+    folded into every conv.  small, the wts argument: per block norm1 w, b, proj bias, ls1, norm2 w, b, fc1 bias, fc2
+    bias, ls2; norm_layers; prev_values (padded to 8); the folded conv biases [256], [128], [64]."""
     g, small = [], []
     for b in VIT_DECODER_BLOCKS:
         q = p + b
@@ -180,20 +181,20 @@ def pack_vit_decoder(sd, p=""):
     for i in range(2):
         small += [_d(sd[f"{p}norm_layers.{i}.weight"]), _d(sd[f"{p}norm_layers.{i}.bias"])]
     small += [torch.stack([_d(sd[f"{p}prev_values.{i}"]).reshape(()) for i in range(2)]), torch.zeros(6, dtype=torch.float64)]
-    out = _cat(g + small + biases, pad_to=8)
-    assert out.numel() == VIT_DECODER_WTS, out.numel()
-    return out
+    g, small = _cat(g), _cat(small + biases, pad_to=8)
+    assert g.numel() == VIT_DECODER_GEMM_WTS and small.numel() == VIT_DECODER_SMALL_WTS, (g.numel(), small.numel())
+    return g, small
 
 
-VIT_GEMM_WTS = 85426176   # floats of the GEMM prefix of pack_vit (csrc/vit.cu NG)
-VIT_SMALL_WTS = 141312    # floats of its small-parameter tail (csrc/vit.cu NS)
+VIT_GEMM_WTS = 85426176   # floats of the GEMM part of pack_vit (csrc/vit.cu NG)
+VIT_SMALL_WTS = 141312    # floats of its small-parameter part (csrc/vit.cu NS)
 
 
 def pack_vit(sd, p=""):
-    """models/dino/dinov2.py (ViT-B/14) -> the fp32 blob of mvsf_vit_forward (layout in csrc/vit.cu): the GEMM prefix
-    patch_embed.proj [768][640] (k = c * 196 + ky * 14 + kx, zero from 588), then per block qkv [2304][768], proj, fc1,
-    fc2 as [N][K] rows; then the small parameters, per block norm1 w, b, qkv bias, proj bias, ls1, norm2 w, b, fc1 bias,
-    fc2 bias, ls2, and patch bias, cls token, norm w, b.  The two parts are split at VIT_GEMM_WTS."""
+    """models/dino/dinov2.py (ViT-B/14) -> (gemm, small), the two fp32 parts of mvsf_vit_forward's weights (layout in
+    csrc/vit.cu).  gemm: patch_embed.proj [768][640] (k = c * 196 + ky * 14 + kx, zero from 588), then per block qkv
+    [2304][768], proj, fc1, fc2 as [N][K] rows.  small, the wts argument: per block norm1 w, b, qkv bias, proj bias, ls1,
+    norm2 w, b, fc1 bias, fc2 bias, ls2, and patch bias, cls token, norm w, b."""
     pw = _d(sd[p + "patch_embed.proj.weight"]).reshape(768, 588)
     g = [torch.cat([pw, torch.zeros(768, 640 - 588, dtype=torch.float64)], 1)]
     small = []
@@ -204,9 +205,9 @@ def pack_vit(sd, p=""):
                                           "norm2.weight", "norm2.bias", "mlp.fc1.bias", "mlp.fc2.bias", "ls2.gamma")]
     small += [_d(sd[p + "patch_embed.proj.bias"]), _d(sd[p + "cls_token"]), _d(sd[p + "norm.weight"]),
               _d(sd[p + "norm.bias"])]
-    out = _cat(g + small, pad_to=8)
-    assert out.numel() == VIT_GEMM_WTS + VIT_SMALL_WTS, out.numel()
-    return out
+    g, small = _cat(g), _cat(small, pad_to=8)
+    assert g.numel() == VIT_GEMM_WTS and small.numel() == VIT_SMALL_WTS, (g.numel(), small.numel())
+    return g, small
 
 
 def vit_pos_embed(pos_embed, gh, gw):

@@ -73,7 +73,7 @@ def test_header_parser_spellings_and_refusals(tmp_path):
 def test_profile_calls_wraps_exactly_the_stream_entry_points(lib):
     streamed = {n for n, (_, params) in _lib.prototypes().items() if params[-1:] == ["mvsf_stream_t"]}
     assert "mvsf_warp_corr_entropy_store" in streamed and "mvsf_fusion_filter" in streamed
-    assert not streamed & {"mvsf_vit_tc_bytes", "mvsf_fmt_workspace_bytes", "mvsf_warp_corr_plan",
+    assert not streamed & {"mvsf_fpn_tc_bytes", "mvsf_fmt_workspace_bytes", "mvsf_warp_corr_plan",
                            "mvsf_attention_split_plan", "mvsf_warp_corr_set_tile_path", "mvsf_ktimer_read"}
     names = list(_lib.prototypes())
     with _lib.profile_calls():

@@ -53,23 +53,23 @@ def test_vit_state_dict_keys_match_reference_inventory():
     assert {"vit." + k: tuple(v.shape) for k, v in _vit().state_dict().items()} == ref
 
 
-def test_pack_vit_layout():
+def test_pack_vit_two_part_layout():
     sd = sub_sd(vit_state_dict(5), "vit.")
-    blob = packing.pack_vit(sd)
-    assert blob.dtype == torch.float32 and blob.numel() == packing.VIT_GEMM_WTS + packing.VIT_SMALL_WTS
+    gemm, small = packing.pack_vit(sd)
+    assert gemm.dtype == small.dtype == torch.float32
+    assert gemm.numel() == packing.VIT_GEMM_WTS and small.numel() == packing.VIT_SMALL_WTS
     D, HID = 768, 3072
-    pw = blob[:D * 640].view(D, 640)
+    pw = gemm[:D * 640].view(D, 640)
     assert torch.equal(pw[:, :588], sd["patch_embed.proj.weight"].reshape(D, 588))
     assert not pw[:, 588:].any()
     blk = 4 * D * D + 2 * HID * D
     for i in (0, 11):
         o = D * 640 + i * blk
-        assert torch.equal(blob[o:o + 3 * D * D].view(3 * D, D), sd[f"blocks.{i}.attn.qkv.weight"])
-        assert torch.equal(blob[o + 3 * D * D:o + 4 * D * D].view(D, D), sd[f"blocks.{i}.attn.proj.weight"])
+        assert torch.equal(gemm[o:o + 3 * D * D].view(3 * D, D), sd[f"blocks.{i}.attn.qkv.weight"])
+        assert torch.equal(gemm[o + 3 * D * D:o + 4 * D * D].view(D, D), sd[f"blocks.{i}.attn.proj.weight"])
         o += 4 * D * D
-        assert torch.equal(blob[o:o + HID * D].view(HID, D), sd[f"blocks.{i}.mlp.fc1.weight"])
-        assert torch.equal(blob[o + HID * D:o + 2 * HID * D].view(D, HID), sd[f"blocks.{i}.mlp.fc2.weight"])
-    small = blob[packing.VIT_GEMM_WTS:]
+        assert torch.equal(gemm[o:o + HID * D].view(HID, D), sd[f"blocks.{i}.mlp.fc1.weight"])
+        assert torch.equal(gemm[o + HID * D:o + 2 * HID * D].view(D, HID), sd[f"blocks.{i}.mlp.fc2.weight"])
     sb = 15 * D
     assert torch.equal(small[2 * D:5 * D], sd["blocks.0.attn.qkv.bias"])
     assert torch.equal(small[11 * sb + 14 * D:12 * sb], sd["blocks.11.ls2.gamma"])
@@ -138,7 +138,7 @@ def test_vit_call_time_refusals():
         m.train().forward_interval_features(x)
 
 
-def test_vit_abi_refuses_bad_arguments_without_touching_the_gpu(lib):
+def test_vit_and_split_abi_refuse_bad_arguments_without_touching_the_gpu(lib):
     need = ctypes.c_size_t(0)
     ptr = ctypes.c_void_p(1 << 20)
     big = ctypes.c_size_t(1 << 40)
@@ -161,10 +161,10 @@ def test_vit_abi_refuses_bad_arguments_without_touching_the_gpu(lib):
     assert lib.mvsf_vit_forward(ptr, ptr, ptr, ptr, ptr, ptr, ptr, ptr, ctypes.c_size_t(need.value - 1), 2, 3, 4,
                                 None) == -3
     assert b"workspace" in lib.mvsf_last_error()
-    assert lib.mvsf_vit_tc_bytes(None) == -1
-    assert lib.mvsf_vit_tc_bytes(ctypes.byref(need)) == 0 and need.value == 4 * packing.VIT_GEMM_WTS
-    assert lib.mvsf_vit_pack_tc(ptr, ptr, ctypes.c_size_t(need.value - 2), None) == -1
-    assert lib.mvsf_vit_pack_tc(None, ptr, ctypes.c_size_t(need.value), None) == -1
+    # the split that makes wts_tc
+    assert lib.mvsf_split_weights_f16(None, ptr, ctypes.c_size_t(packing.VIT_GEMM_WTS), None) == -1
+    assert lib.mvsf_split_weights_f16(ptr, ptr, ctypes.c_size_t(packing.VIT_GEMM_WTS + 4), None) == -1
+    assert b"split_weights_f16" in lib.mvsf_last_error()
     # the attention seam
     for n, N in ((0, 10), (1, 0), (-1, 10), (1, -5)):
         assert lib.mvsf_vit_attention_forward(ptr, 2304, ptr, 768, ptr, big, n, N, None) == -1

@@ -45,20 +45,21 @@ def test_vit_decoder_state_dict_keys_match_reference_inventory():
     assert got == ref
 
 
-def test_vit_decoder_packing_folds_bn_and_gathers_transposed_convs():
+def test_vit_decoder_two_part_packing_folds_bn_and_gathers_transposed_convs():
     sd = sub_sd(vit_state_dict(5), "decoder_vit.")
-    blob = packing.pack_vit_decoder(sd).double()
-    assert blob.numel() == packing.VIT_DECODER_WTS
+    gemm, small = (t.double() for t in packing.pack_vit_decoder(sd))
     D, G_BLK = 768, 9216 * 768
     ng = 5 * G_BLK + 256 * 9 * D + 4 * 128 * 1024 + 4 * 64 * 512
     sb = 8 * D + 3072   # small parameters per block: 8 vectors of 768 and the fc1 bias
-    cb = ng + 5 * sb + 4 * D + 8
-    assert float(blob[cb - 8]) == pytest.approx(float(sd["prev_values.0"])) and float(blob[cb - 7]) == pytest.approx(
+    cb = 5 * sb + 4 * D + 8
+    assert gemm.numel() == ng == packing.VIT_DECODER_GEMM_WTS
+    assert small.numel() == cb + 448 == packing.VIT_DECODER_SMALL_WTS
+    assert float(small[cb - 8]) == pytest.approx(float(sd["prev_values.0"])) and float(small[cb - 7]) == pytest.approx(
         float(sd["prev_values.1"]))
     # the proj conv: [256][tap * 768 + ci] with the BN scale folded, the folded shift at the conv biases
     x = torch.randn(1, D, 5, 6, dtype=torch.float64)
-    w = blob[5 * G_BLK:5 * G_BLK + 256 * 9 * D].view(256, 3, 3, D).permute(0, 3, 1, 2)
-    got = F.conv2d(x, w, blob[cb:cb + 256], padding=1)
+    w = gemm[5 * G_BLK:5 * G_BLK + 256 * 9 * D].view(256, 3, 3, D).permute(0, 3, 1, 2)
+    got = F.conv2d(x, w, small[cb:cb + 256], padding=1)
     t = lambda k: sd["proj.1." + k].double()
     want = F.batch_norm(F.conv2d(x, sd["proj.0.weight"].double(), sd["proj.0.bias"].double(), padding=1),
                         t("running_mean"), t("running_var"), t("weight"), t("bias"), False, 0.0, 1e-5)
@@ -73,8 +74,8 @@ def test_vit_decoder_packing_folds_bn_and_gathers_transposed_convs():
     xp = F.pad(x, (1, 1, 1, 1))
     for cls in range(4):
         py, px = cls >> 1, cls & 1
-        wc = blob[off + cls * 128 * 1024:off + (cls + 1) * 128 * 1024].view(128, 4, 256)
-        acc = blob[cb + 256:cb + 384].view(1, 128, 1, 1).expand(1, 128, 4, 5).clone()
+        wc = gemm[off + cls * 128 * 1024:off + (cls + 1) * 128 * 1024].view(128, 4, 256)
+        acc = small[cb + 256:cb + 384].view(1, 128, 1, 1).expand(1, 128, 4, 5).clone()
         for ti, (dy, _) in enumerate(packing.deconv_class_taps(py)):
             for tj, (dx, _) in enumerate(packing.deconv_class_taps(px)):
                 src = xp[:, :, 1 + dy:1 + dy + 4, 1 + dx:1 + dx + 5]
@@ -113,7 +114,7 @@ def test_vit_decoder_fails_loudly_on_cpu():
         m(x, vit_shape=(1, 2, 3, 4, 768))
 
 
-def test_vit_decoder_abi_refuses_bad_arguments_without_touching_the_gpu(lib):
+def test_vit_decoder_entry_points_refuse_bad_arguments_without_touching_the_gpu(lib):
     need = ctypes.c_size_t(0)
     ptr = ctypes.c_void_p(1 << 20)
     lib.mvsf_launch_count(1)
@@ -133,10 +134,6 @@ def test_vit_decoder_abi_refuses_bad_arguments_without_touching_the_gpu(lib):
     assert lib.mvsf_vit_decoder_workspace_bytes(1, 3, 4, 4, ctypes.byref(need)) == 0
     assert lib.mvsf_vit_decoder_forward(ptr, ptr, ptr, ptr, ptr, ptr, ptr, ctypes.c_size_t(need.value - 1), 1, 3, 4, 4,
                                         None) == -3
-    assert lib.mvsf_vit_decoder_tc_bytes(None) == -1
-    assert lib.mvsf_vit_decoder_tc_bytes(ctypes.byref(need)) == 0 and need.value == 4 * 37814272
-    assert lib.mvsf_vit_decoder_pack_tc(ptr, ptr, ctypes.c_size_t(need.value - 2), None) == -1
-    assert lib.mvsf_vit_decoder_pack_tc(None, ptr, ctypes.c_size_t(need.value), None) == -1
 
     # the streamed-weight GEMM seam
     BIAS, GELU, RES, LN, SILU = 0, 1, 3, 5, 6
