@@ -119,11 +119,14 @@ int mvsf_corr_aggregate(const float* corr, const float* vis, float* volume, int 
 
 /* ---- R2-R4: models/module.py:367-408 (kind 0: CostRegNet, stride 2, 3^3 prob no bias) and
  *      :453-504 (kind 1: CostRegNet3D, stride (1,2,2), 1^3 prob + bias).  volume [D][H][W][C] -> logits [D][H][W].
- * wts: packed by packing.pack_costreg_unet (per layer [27][Cin][Cout] with BN scale folded, then bias[Cout]). */
+ * wts: the small fp32 parameters (small part of packing.pack_costreg_unet: per layer the folded bias[Cout], then the
+ * prob conv; 496 floats for kind 0, 292 for kind 1); wts_tc = mvsf_costreg_unet_pack_tc(conv part of
+ * packing.pack_costreg_unet: per layer [27][Cin][Cout] with BN scale folded, 290 304 floats). */
 int mvsf_costreg_unet_workspace_bytes(int kind, int C, int D, int H, int W, size_t* bytes);
-/* install time: wts -> wts_tc, the fp16 hi/lo weight slabs of the wgmma implicit-GEMM convolutions (csrc/conv3d_tc.cu) */
+/* install time: conv part -> wts_tc, the fp16 hi/lo weight slabs of the wgmma implicit-GEMM convolutions
+ * (csrc/conv3d_tc.cu) */
 int mvsf_costreg_unet_tc_bytes(size_t* bytes);
-int mvsf_costreg_unet_pack_tc(int kind, const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
+int mvsf_costreg_unet_pack_tc(int kind, const float* conv, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
 int mvsf_costreg_unet_forward(int kind, const float* volume, const float* wts, const void* wts_tc, float* logits,
                               void* workspace, size_t workspace_bytes, int C, int D, int H, int W, mvsf_stream_t stream);
 /* test seam: ONE 3x3x3 layer of the U-Nets on the wgmma implicit-GEMM path, fp32 in / out (module.py:367-504:
@@ -137,7 +140,10 @@ int mvsf_conv3d_tc_layer(int mode, int sd, const float* in, const float* w32, co
 /* ---- R1: models/module.py:602-646 PureTransformerCostReg (+ position_encoding.py:164-189 PositionEncoding3D).
  * volume [D][H][W][C] is modified in place by the PE add; pos [3][D][H][W] or NULL.
  * Fixed by the shipped config: down_rate (2,4,4), mid 64, heads 4, mlp 256.  softmax_scale = hd^-0.5*log_tal(N).
- * wts16 = mvsf_split_weights_f16(wts) (fp16 hi|lo parts for the wgmma GEMMs), n_wts = number of floats in wts. */
+ * wts: the small fp32 parameters (small part of packing.pack_costreg_tr, layout in csrc/costreg_tr.cu: pe_proj, biases,
+ * LayerNorms, gammas and prob; 672 + 768 layers floats); wts16 = mvsf_split_weights_f16(GEMM part of
+ * packing.pack_costreg_tr: the down, qkv, proj, FFN and up weights as [N][K] rows), n_wts = the floats of that GEMM part,
+ * 32 768 + 49 152 layers (any other value: -1, nothing launched). */
 int mvsf_costreg_tr_workspace_bytes(int C, int D, int H, int W, size_t* bytes);
 int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, const void* wts16, size_t n_wts,
                             float* logits, void* workspace, size_t workspace_bytes, int C, int D, int H, int W,
@@ -209,7 +215,10 @@ int mvsf_conf_accumulate(const float* conf, int h, int w, float* acc, int H, int
 /* ---- F1-F4: models/FMT.py:164-206 FMT_with_pathway.forward.
  * Inputs are the reference's NCHW pyramids: f1 [V][64][H1][W1], f2 [V][32][2H1][2W1], f3 [V][16][4H1][4W1],
  * f4 [V][8][8H1][8W1]; pe [H1*W1][64] is the PositionEncodingSineNorm table (position_encoding.py:61-74).
- * Outputs are channels-last: o1 [V][H1][W1][64] ... o4 [V][8H1][8W1][8].  wts: packing.pack_fmt. */
+ * Outputs are channels-last: o1 [V][H1][W1][64] ... o4 [V][8H1][8W1][8].  wts: the small fp32 parameters (small part
+ * of packing.pack_fmt, layout in csrc/fmt.cu: norms, biases, LayerScales, dim_reduction and smooth weights; 17 856
+ * floats); wts16 = mvsf_split_weights_f16(GEMM part of packing.pack_fmt: the qkv, proj and MLP weights as [N][K] rows),
+ * n_wts = the floats of that GEMM part, 196 608 (any other value: -1, nothing launched). */
 int mvsf_fmt_workspace_bytes(int V, int H1, int W1, size_t* bytes);
 int mvsf_fmt_forward(const float* f1, const float* f2, const float* f3, const float* f4, const float* pe,
                      const float* wts, const void* wts16, size_t n_wts, float* o1, float* o2, float* o3, float* o4,
@@ -218,9 +227,11 @@ int mvsf_fmt_forward(const float* f1, const float* f2, const float* f3, const fl
 /* ---- P1: models/module.py:208-239 FPNEncoder.forward (feat_chs [8,16,32,64], norm_type 'BN', eval; every layer
  *      Conv2d(bias=False) -> BatchNorm folded -> LeakyReLU(0.1), module.py:61-80).
  * x [N][3][H][W] (H, W positive multiples of 8) -> c01 [N][H][W][8], c11 [N][H/2][W/2][16], c21 [N][H/4][W/4][32],
- * c31 [N][H/8][W/8][64] (NHWC).  wts: packing.pack_fpn_encoder (per layer w [KS*KS][CI][CO] with BN scale folded, then
- * the folded shift [CO], layers conv00, conv01, downsample1, conv10, conv11, downsample2, conv20, conv21, downsample3,
- * conv30, conv31); wts_tc = mvsf_fpn_pack_tc(0, wts).  Bad shapes: -1, nothing launched. */
+ * c31 [N][H/8][W/8][64] (NHWC).  Layers conv00, conv01, downsample1, conv10, conv11, downsample2, conv20, conv21,
+ * downsample3, conv30, conv31, each w [KS*KS][CI][CO] with BN scale folded and the folded shift [CO].  wts: the small
+ * fp32 parameters (small part of packing.pack_fpn_encoder: conv00's w and shift, then the shifts of the other layers;
+ * 1 528 floats); wts_tc = mvsf_fpn_pack_tc(0, conv part of packing.pack_fpn_encoder: w of every layer after conv00,
+ * 132 800 floats).  Bad shapes: -1, nothing launched. */
 int mvsf_fpn_encoder_workspace_bytes(int N, int H, int W, size_t* bytes);
 int mvsf_fpn_encoder_forward(const float* x, const float* wts, const void* wts_tc, float* c01, float* c11, float* c21,
                              float* c31, void* workspace, size_t workspace_bytes, int N, int H, int W, mvsf_stream_t stream);
@@ -234,15 +245,17 @@ int mvsf_fpn_encoder_vit_forward(const float* x, const float* vit_feat, int V, c
 /* ---- P2: models/module.py:242-270 FPNDecoder.forward (F.interpolate bilinear, align_corners=True; BN folded).
  * c01..c31 as the encoder writes them (NHWC, full-resolution H x W) -> o0 [N][64][H/8][W/8], o1 [N][32][H/4][W/4],
  * o2 [N][16][H/2][W/2], o3 [N][8][H][W] (NCHW: the layout mvsf_fmt_forward reads, DINOv2_mvsformer_model.py:95-98).
- * wts: packing.pack_fpn_decoder (out0 [64 ci][64 co] + shift[64]; per level k: inner_k [CL][64] + bias[64], then out_k
- * [9][64][C_k] + shift[C_k]); wts_tc = mvsf_fpn_pack_tc(1, wts).  The full-resolution intra feature never reaches HBM. */
+ * wts: the small fp32 parameters (small part of packing.pack_fpn_decoder: out0 [64 ci][64 co] + shift[64]; per level
+ * k: inner_k [CL][64] + bias[64], then out_k's shift[C_k]; 7 992 floats); wts_tc = mvsf_fpn_pack_tc(1, conv part of
+ * packing.pack_fpn_decoder: out_k [9][64][C_k], 32 256 floats).  The full-resolution intra feature never reaches HBM. */
 int mvsf_fpn_decoder_workspace_bytes(int N, int H, int W, size_t* bytes);
 int mvsf_fpn_decoder_forward(const float* c01, const float* c11, const float* c21, const float* c31, const float* wts,
                              const void* wts_tc, float* o0, float* o1, float* o2, float* o3, void* workspace,
                              size_t workspace_bytes, int N, int H, int W, mvsf_stream_t stream);
-/* install time: fp32 blob -> fp16 hi/lo weight tiles of the wgmma convolutions (csrc/fpn.cu); part 0 encoder, 1 decoder */
+/* install time: fp32 conv part -> fp16 hi/lo weight tiles of the wgmma convolutions (csrc/fpn.cu); part 0 encoder,
+ * 1 decoder */
 int mvsf_fpn_tc_bytes(int part, size_t* bytes);
-int mvsf_fpn_pack_tc(int part, const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
+int mvsf_fpn_pack_tc(int part, const float* conv, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream);
 
 /* ---- V1: models/module.py:273-364 CrossVITDecoder.forward, shipped config (d_model 768, 12 heads, linear attention,
  *      ffn 768 -> 3072, LayerScale, pre-norm CrossBlocks with pre_norm_query, 3 interval layers, eval-mode BN folded).

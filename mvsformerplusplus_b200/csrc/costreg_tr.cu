@@ -16,17 +16,30 @@
 
 namespace mvsf {
 
-// packed weights (floats), produced by packing.pack_costreg_tr:
-//   pe_w[8][24] | down_w[64][256] (k = ((kd*4+kh)*4+kw)*8+ci) | down_b[64] | down_ln_w[64] | down_ln_b[64]
-//   per layer: qkv_w[192][64] | proj_w[64][64] | proj_b[64] | gamma1[64] | n1_w[64] | n1_b[64]
-//              | f1_w[256][64] | f1_b[256] | f2_w[64][256] | f2_b[64] | gamma2[64] | n2_w[64] | n2_b[64]
-//   up_w[256][64] (n = ((kd*4+kh)*4+kw)*8+co) | up_b[256] | up_ln_w[8] | up_ln_b[8] | prob_w[8] | prob_b[1] (+3 pad)
-constexpr int TR_PE = 0, TR_DOWN_W = 192, TR_DOWN_B = TR_DOWN_W + 64 * 256, TR_DOWN_LNW = TR_DOWN_B + 64,
-              TR_DOWN_LNB = TR_DOWN_LNW + 64, TR_LAYER0 = TR_DOWN_LNB + 64;
-constexpr int L_QKV = 0, L_PROJ_W = 192 * 64, L_PROJ_B = L_PROJ_W + 64 * 64, L_G1 = L_PROJ_B + 64, L_N1W = L_G1 + 64,
-              L_N1B = L_N1W + 64, L_F1W = L_N1B + 64, L_F1B = L_F1W + 256 * 64, L_F2W = L_F1B + 256,
-              L_F2B = L_F2W + 64 * 256, L_G2 = L_F2B + 64, L_N2W = L_G2 + 64, L_N2B = L_N2W + 64, TR_LAYER = L_N2B + 64;
-constexpr int U_W = 0, U_B = 256 * 64, U_LNW = U_B + 256, U_LNB = U_LNW + 8, U_PW = U_LNB + 8, U_PB = U_PW + 8;
+// ---- GEMM weights (the gemm part of packing.pack_costreg_tr), fp32 [N][K] rows; wts16 holds their hi / lo splits with
+// the same indexing:  down_w[64][256] (k = ((kd*4+kh)*4+kw)*8+ci)
+//   per layer: qkv_w[192][64] | proj_w[64][64] | f1_w[256][64] | f2_w[64][256]
+//   up_w[256][64] (n = ((kd*4+kh)*4+kw)*8+co)
+constexpr int G_DOWN_W = 0, G_LAYER0 = 64 * 256;
+constexpr int L_QKV = 0, L_PROJ_W = 192 * 64, L_F1W = L_PROJ_W + 64 * 64, L_F2W = L_F1W + 256 * 64,
+              G_LAYER = L_F2W + 64 * 256;
+constexpr size_t tr_gemm_floats(int layers) { return G_LAYER0 + (size_t)layers * G_LAYER + 256 * 64; }
+// ---- small fp32 parameters (the small part of packing.pack_costreg_tr, the wts argument):
+//   pe_w[8][24] | down_b[64] | down_ln_w[64] | down_ln_b[64]
+//   per layer: proj_b[64] | gamma1[64] | n1_w[64] | n1_b[64] | f1_b[256] | f2_b[64] | gamma2[64] | n2_w[64] | n2_b[64]
+//   up_b[256] | up_ln_w[8] | up_ln_b[8] | prob_w[8] | prob_b[1] (+7 pad)
+constexpr int TR_PE = 0, TR_DOWN_B = 192, TR_DOWN_LNW = TR_DOWN_B + 64, TR_DOWN_LNB = TR_DOWN_LNW + 64,
+              TR_LAYER0 = TR_DOWN_LNB + 64;
+constexpr int L_PROJ_B = 0, L_G1 = 64, L_N1W = L_G1 + 64, L_N1B = L_N1W + 64, L_F1B = L_N1B + 64, L_F2B = L_F1B + 256,
+              L_G2 = L_F2B + 64, L_N2W = L_G2 + 64, L_N2B = L_N2W + 64, TR_LAYER = L_N2B + 64;
+constexpr int U_B = 0, U_LNW = U_B + 256, U_LNB = U_LNW + 8, U_PW = U_LNB + 8, U_PB = U_PW + 8;
+constexpr size_t tr_small_floats(int layers) { return (TR_LAYER0 + (size_t)layers * TR_LAYER + U_PB + 1 + 7) / 8 * 8; }
+static_assert(tr_gemm_floats(0) == 32768 && G_LAYER == 49152 && tr_small_floats(0) == 672 && TR_LAYER == 768,
+              "packing.costreg_tr_wts");
+// float2 loads of the biases and gammas
+static_assert(TR_DOWN_B % 4 == 0 && TR_LAYER0 % 4 == 0 && TR_LAYER % 4 == 0 && L_PROJ_B % 4 == 0 && L_G1 % 4 == 0 &&
+                  L_F1B % 4 == 0 && L_F2B % 4 == 0 && L_G2 % 4 == 0 && U_B % 4 == 0,
+              "vector-loaded small parameters start at a multiple of 4 floats");
 
 // volume[d,y,x,:] += pe_w (8x24) * PE3D(pos[:,d,y,x])
 __global__ void pe3d_add_kernel(float* __restrict__ vol, const float* __restrict__ pos, const float* __restrict__ pe_w,
@@ -173,13 +186,14 @@ int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, c
   if (rc) return rc;
   if (workspace_bytes < need) return fail(MVSF_ERR_WORKSPACE, "costreg_tr: workspace %zu < %zu bytes", workspace_bytes, need);
   MVSF_REQUIRE(((uintptr_t)workspace & 15) == 0 && ((uintptr_t)wts & 15) == 0 && ((uintptr_t)volume & 15) == 0 &&
-                   ((uintptr_t)wts16 & 15) == 0 && (n_wts % 8) == 0,
+                   ((uintptr_t)wts16 & 15) == 0,
                "costreg_tr: pointers must be 16-byte aligned");
-  MVSF_REQUIRE(n_wts >= (size_t)TR_LAYER0 + (size_t)layers * TR_LAYER + U_PB + 1, "costreg_tr: weight blob too small");
+  MVSF_REQUIRE(n_wts == tr_gemm_floats(layers), "costreg_tr: n_wts %zu is not the %zu floats of the GEMM part",
+               n_wts, tr_gemm_floats(layers));
   cudaStream_t s = (cudaStream_t)stream;
   const size_t nvox = (size_t)D * H * W;
   const int N = (int)((size_t)(D / 2) * (H / 4) * (W / 4));
-  const __half* wh = reinterpret_cast<const __half*>(wts16);  // fp16 hi parts, same indexing as wts
+  const __half* wh = reinterpret_cast<const __half*>(wts16);  // fp16 hi parts of the GEMM weights
   const __half* wl = wh + n_wts;                              // fp16 lo parts
   float* big = (float*)workspace;                             // [N][256] floats
   __half* big2 = reinterpret_cast<__half*>(big);             // [N][512] halves: row = [hi(256) | lo(256)]
@@ -197,15 +211,15 @@ int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, c
   MVSF_LAUNCH_CHECK("patch_gather");
 
   TcLinArgs a{};
-  a.Ah = big2; a.Al = big2 + 256; a.lda = 512; a.Bh = wh + TR_DOWN_W; a.Bl = wl + TR_DOWN_W; a.ldb = 256;
+  a.Ah = big2; a.Al = big2 + 256; a.lda = 512; a.Bh = wh + G_DOWN_W; a.Bl = wl + G_DOWN_W; a.ldb = 256;
   a.M = N; a.N = 64; a.K = 256; a.bias = wts + TR_DOWN_B; a.ln_w = wts + TR_DOWN_LNW; a.ln_b = wts + TR_DOWN_LNB; a.ln_eps = 1e-6f;
   a.C = x; a.ldc = 64; a.C2 = x2; a.ldc2 = 128;
   if ((rc = launch_linear_tc(a, LIN_LN, s))) return rc;
 
   const float scale_log2e = softmax_scale * 1.4426950408889634f;
   for (int l = 0; l < layers; ++l) {
-    const size_t lo = (size_t)TR_LAYER0 + (size_t)l * TR_LAYER;
-    const float* lw = wts + lo;
+    const size_t lo = (size_t)G_LAYER0 + (size_t)l * G_LAYER;
+    const float* lw = wts + TR_LAYER0 + (size_t)l * TR_LAYER;
     TcLinArgs q{};
     q.Ah = x2; q.Al = x2 + 64; q.lda = 128; q.Bh = wh + lo + L_QKV; q.Bl = wl + lo + L_QKV; q.ldb = 64;
     q.M = N; q.N = 192; q.K = 64; q.C = qkv; q.ldc = 192;
@@ -220,12 +234,13 @@ int mvsf_costreg_tr_forward(float* volume, const float* pos, const float* wts, c
     p.mid_w = lw + L_N1W; p.mid_b = lw + L_N1B; p.mid_eps = 1e-5f; p.out_w = lw + L_N2W; p.out_b = lw + L_N2B; p.out_eps = 1e-5f;
     if ((rc = launch_token_mlp(p, MLP_POST_NORM, s))) return rc;
   }
-  const size_t uo = (size_t)TR_LAYER0 + (size_t)layers * TR_LAYER;
+  const size_t uo = (size_t)G_LAYER0 + (size_t)layers * G_LAYER;
+  const float* uw = wts + TR_LAYER0 + (size_t)layers * TR_LAYER;
   TcLinArgs u{};
-  u.Ah = x2; u.Al = x2 + 64; u.lda = 128; u.Bh = wh + uo + U_W; u.Bl = wl + uo + U_W; u.ldb = 64;
-  u.M = N; u.N = 256; u.K = 64; u.bias = wts + uo + U_B; u.C = big; u.ldc = 256;
+  u.Ah = x2; u.Al = x2 + 64; u.lda = 128; u.Bh = wh + uo; u.Bl = wl + uo; u.ldb = 64;
+  u.M = N; u.N = 256; u.K = 64; u.bias = uw + U_B; u.C = big; u.ldc = 256;
   if ((rc = launch_linear_tc(u, LIN_BIAS, s))) return rc;
-  unpatch_ln_prob_kernel<<<cdiv((long long)nvox, 256), 256, 0, s>>>(big, wts + uo + U_LNW, logits, D, H, W);
+  unpatch_ln_prob_kernel<<<cdiv((long long)nvox, 256), 256, 0, s>>>(big, uw + U_LNW, logits, D, H, W);
   MVSF_LAUNCH_CHECK("unpatch_ln_prob");
   return MVSF_OK;
 }

@@ -41,11 +41,21 @@ __global__ void prob3_kernel(const float* __restrict__ in, const float* __restri
 }
 
 // ---------------------------------------------------------------------------------------------------- host
-static size_t layer_floats(int cin, int cout) { return (size_t)27 * cin * cout + cout; }
-
 // ------------------------------------------------------------------------------------ tensor-core path (conv3d_tc.cu)
-static const int kLayerCh[9][2] = {{8, 16}, {16, 16}, {16, 32}, {32, 32}, {32, 64}, {64, 64}, {64, 32}, {32, 16}, {16, 8}};
+constexpr int kLayerCh[9][2] = {{8, 16}, {16, 16}, {16, 32}, {32, 32}, {32, 64}, {64, 64}, {64, 32}, {32, 16}, {16, 8}};
 static const int kLayerMode[9] = {CONV_S2, CONV_S1, CONV_S2, CONV_S1, CONV_S2, CONV_S1, DECONV_S2, DECONV_S2, DECONV_S2};
+
+// Two fp32 parts (packing.pack_costreg_unet), each counted from 0.  Conv part (the input of mvsf_costreg_unet_pack_tc):
+// per layer w [27][Cin][Cout].  Small part, the wts argument: per layer bias[Cout], then the prob conv: [27][8]
+// (kind 0) or w[8], b[1] (kind 1), padded to a multiple of 4.
+constexpr size_t unet_floats(bool conv) {
+  size_t n = 0;
+  for (int l = 0; l < 9; ++l) n += conv ? (size_t)27 * kLayerCh[l][0] * kLayerCh[l][1] : kLayerCh[l][1];
+  return n;
+}
+constexpr size_t NCONV = unet_floats(true), NSMALL[2] = {unet_floats(false) + 27 * 8, unet_floats(false) + 8 + 1 + 3};
+static_assert(NCONV == 290304 && NSMALL[0] == 496 && NSMALL[1] == 292,
+              "packing.COSTREG_UNET_CONV_WTS / COSTREG_UNET_SMALL_WTS");
 
 static size_t tc_total_halves() {
   size_t n = 0;
@@ -67,25 +77,25 @@ static int unet_forward_tc(int kind, const float* vol, const float* wts, const _
   __half* t3 = c2 + 2 * n1;   __half* c4 = t3 + 2 * n2;
   __half* t5 = c4 + 2 * n2;   __half* c6 = t5 + 2 * n3;
   float* x11 = reinterpret_cast<float*>(c6 + 2 * n3);   // kind 0 only: [D][H][W][8] fp32
-  const float* w32[9];
+  const float* bias[9];
   const __half* w16[9];
   {
     const float* p = wts;
     const __half* q = wtc;
     for (int l = 0; l < 9; ++l) {
-      w32[l] = p; w16[l] = q;
-      p += layer_floats(kLayerCh[l][0], kLayerCh[l][1]);
+      bias[l] = p; w16[l] = q;
+      p += kLayerCh[l][1];
       q += conv3d_tc_packed_halves(kLayerMode[l], kLayerCh[l][0], kLayerCh[l][1]);
     }
   }
-  const float* wp = w32[8] + layer_floats(16, 8);
+  const float* wp = bias[8] + 8;
   int rc;
   if ((rc = launch_split_f16(vol, n0, v0, 2 * n0, 1, n0, s))) return rc;
   auto conv = [&](int l, const __half* in, size_t nin, __half* out, size_t nout, const __half* skip, size_t nskip,
                   int ID, int IH, int IW) {
     ConvTcArgs a{};
     a.in_hi = in; a.in_lo = in + nin;
-    a.wtc = w16[l]; a.bias = w32[l] + (size_t)27 * kLayerCh[l][0] * kLayerCh[l][1];
+    a.wtc = w16[l]; a.bias = bias[l];
     a.skip_hi = skip; a.skip_lo = skip ? skip + nskip : nullptr;
     a.out_hi = out; a.out_lo = out + nout;
     a.CIN = kLayerCh[l][0]; a.COUT = kLayerCh[l][1]; a.SD = SD; a.ID = ID; a.IH = IH; a.IW = IW;
@@ -105,7 +115,7 @@ static int unet_forward_tc(int kind, const float* vol, const float* wts, const _
   {
     ConvTcArgs a{};
     a.in_hi = t1; a.in_lo = t1 + n1;
-    a.wtc = w16[8]; a.bias = w32[8] + (size_t)27 * 16 * 8;
+    a.wtc = w16[8]; a.bias = bias[8];
     a.skip32 = vol;
     a.CIN = 16; a.COUT = 8; a.SD = SD; a.ID = D1; a.IH = H1; a.IW = W1; a.KG = conv3d_tc_kg(DECONV_S2, 16);
     if (kind == 1) {
@@ -147,16 +157,16 @@ int mvsf_costreg_unet_tc_bytes(size_t* bytes) {
   return MVSF_OK;
 }
 
-int mvsf_costreg_unet_pack_tc(int kind, const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream) {
-  MVSF_REQUIRE(wts && wts_tc && ((uintptr_t)wts_tc & 15) == 0 && (kind == 0 || kind == 1), "costreg_unet_pack_tc: null or unaligned pointer, or bad kind");
+int mvsf_costreg_unet_pack_tc(int kind, const float* conv, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream) {
+  MVSF_REQUIRE(conv && wts_tc && ((uintptr_t)wts_tc & 15) == 0 && (kind == 0 || kind == 1), "costreg_unet_pack_tc: null or unaligned pointer, or bad kind");
   if (wts_tc_bytes < tc_total_halves() * sizeof(__half))
     return fail(MVSF_ERR_WORKSPACE, "costreg_unet_pack_tc: buffer %zu < %zu bytes", wts_tc_bytes, tc_total_halves() * sizeof(__half));
-  const float* p = wts;
+  const float* p = conv;
   __half* q = reinterpret_cast<__half*>(wts_tc);
   for (int l = 0; l < 9; ++l) {
     int rc = conv3d_tc_pack(p, q, kLayerMode[l], kind == 0 ? 2 : 1, kLayerCh[l][0], kLayerCh[l][1], (cudaStream_t)stream);
     if (rc) return rc;
-    p += layer_floats(kLayerCh[l][0], kLayerCh[l][1]);
+    p += (size_t)27 * kLayerCh[l][0] * kLayerCh[l][1];
     q += conv3d_tc_packed_halves(kLayerMode[l], kLayerCh[l][0], kLayerCh[l][1]);
   }
   return MVSF_OK;

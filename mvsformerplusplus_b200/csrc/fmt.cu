@@ -11,14 +11,22 @@
 
 namespace mvsf {
 
-// packed weights per CrossBlock (floats): n1_w[64] n1_b[64] qkv_w[192][64] proj_w[64][64] proj_b[64] g1[64]
-//                                          n2_w[64] n2_b[64] f1_w[256][64] f1_b[256] f2_w[64][256] f2_b[64] g2[64]
-constexpr int B_N1W = 0, B_N1B = 64, B_QKV = 128, B_PW = B_QKV + 192 * 64, B_PB = B_PW + 64 * 64, B_G1 = B_PB + 64,
-              B_N2W = B_G1 + 64, B_N2B = B_N2W + 64, B_F1W = B_N2B + 64, B_F1B = B_F1W + 256 * 64,
-              B_F2W = B_F1B + 256, B_F2B = B_F2W + 64 * 256, B_G2 = B_F2B + 64, B_SIZE = B_G2 + 64;
+// ---- GEMM weights (the gemm part of packing.pack_fmt), fp32 [N][K] rows; wts16 holds their hi / lo splits with the
+// same indexing.  Per CrossBlock: qkv_w[192][64] proj_w[64][64] f1_w[256][64] f2_w[64][256]
+constexpr int B_QKV = 0, B_PW = 192 * 64, B_F1W = B_PW + 64 * 64, B_F2W = B_F1W + 256 * 64, G_BLK = B_F2W + 64 * 256,
+              NG = 4 * G_BLK;
+// ---- small fp32 parameters (the small part of packing.pack_fmt, the wts argument).  Per CrossBlock: n1_w[64] n1_b[64]
+// proj_b[64] g1[64] n2_w[64] n2_b[64] f1_b[256] f2_b[64] g2[64]
+constexpr int B_N1W = 0, B_N1B = 64, B_PB = 128, B_G1 = B_PB + 64, B_N2W = B_G1 + 64, B_N2B = B_N2W + 64,
+              B_F1B = B_N2B + 64, B_F2B = B_F1B + 256, B_G2 = B_F2B + 64, B_SIZE = B_G2 + 64;
 // after 4 blocks: dr1[32][64] dr2[16][32] dr3[8][16] sm1[9][32][32] sm2[9][16][16] sm3[9][8][8]   ([tap][ci][co])
 constexpr int P_DR1 = 4 * B_SIZE, P_DR2 = P_DR1 + 32 * 64, P_DR3 = P_DR2 + 16 * 32, P_SM1 = P_DR3 + 8 * 16,
-              P_SM2 = P_SM1 + 9 * 32 * 32, P_SM3 = P_SM2 + 9 * 16 * 16, FMT_WTS = P_SM3 + 9 * 8 * 8;
+              P_SM2 = P_SM1 + 9 * 32 * 32, P_SM3 = P_SM2 + 9 * 16 * 16, NS = P_SM3 + 9 * 8 * 8;
+static_assert(NG == 196608 && NS == 17856, "packing.FMT_GEMM_WTS / FMT_SMALL_WTS");
+// float2 loads of the biases and LayerScales, float4 loads of the dim_reduction weights
+static_assert(B_SIZE % 4 == 0 && B_PB % 4 == 0 && B_G1 % 4 == 0 && B_F1B % 4 == 0 && B_F2B % 4 == 0 && B_G2 % 4 == 0 &&
+                  P_DR1 % 4 == 0 && P_DR2 % 4 == 0 && P_DR3 % 4 == 0,
+              "vector-loaded small parameters start at a multiple of 4 floats");
 using FmtAttn = LinAttn<4, 16>;
 constexpr int KVSZ = FmtAttn::KVSZ;  // KV[h][m][d] + ksum[h][d]
 
@@ -44,10 +52,11 @@ __global__ void tokens_add_pe_kernel(const float* __restrict__ f, const float* _
 struct FmtWs {
   __half *xn2, *att2;          // fp16 hi|lo split activations: [M][128], [M][128]
   float *qkv, *ref0, *kvpart, *kvfin, *kvc;
-  const __half *wh, *wl;       // fp16 hi / lo parts of the packed weight blob (same indexing as the fp32 blob)
+  const __half *wh, *wl;       // fp16 hi / lo parts of the GEMM weights
 };
 
-// one CrossBlock over `M` tokens (nviews views of L tokens each) stored at x (in place).
+// one CrossBlock over `M` tokens (nviews views of L tokens each) stored at x (in place); bw: the block's small
+// parameters, boff: the offset of its GEMM weights in ws.wh / ws.wl.
 // self attention: kv_src == nullptr ; cross attention: kvc = precomputed K/V summary of the reference view.
 // LayerNorms are fused into the epilogue of the GEMM that produces their input: proj emits x (residual stream) and
 // split(norm2(x)), FFN2 emits x and split(norm1 of the NEXT block) when `next_bw` is given; `ln1_ready` says the previous
@@ -243,7 +252,7 @@ int mvsf_fmt_forward(const float* f1, const float* f2, const float* f3, const fl
                      const float* wts, const void* wts16, size_t n_wts, float* o1, float* o2, float* o3, float* o4,
                      void* workspace, size_t workspace_bytes, int V, int H1, int W1, mvsf_stream_t stream) {
   MVSF_REQUIRE(f1 && f2 && f3 && f4 && pe && wts && wts16 && o1 && o2 && o3 && o4 && workspace, "fmt: null pointer");
-  MVSF_REQUIRE(n_wts >= (size_t)FMT_WTS && (n_wts % 8) == 0 && ((uintptr_t)wts16 & 15) == 0, "fmt: bad fp16 weight blob");
+  MVSF_REQUIRE(n_wts == (size_t)NG && ((uintptr_t)wts16 & 15) == 0, "fmt: bad fp16 weight blob");
   size_t need = 0;
   int rc = mvsf_fmt_workspace_bytes(V, H1, W1, &need);
   if (rc) return rc;
@@ -273,15 +282,15 @@ int mvsf_fmt_forward(const float* f1, const float* f2, const float* f3, const fl
   // reference view: the two self layers (FMT.py:96-107); keep the output of the first one for cross layer 1
   if ((rc = run_block(o1, 1, L, b0, 0, nullptr, ws, s, false, b2))) return rc;
   MVSF_CUDA_OK(cudaMemcpyAsync(ws.ref0, o1, (size_t)L * 64 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  if ((rc = run_block(o1, 1, L, b2, 2 * (size_t)B_SIZE, nullptr, ws, s, true, nullptr))) return rc;
-  if ((rc = run_cross_kv(ws.ref0, L, b1, (size_t)B_SIZE, ws.kvc, ws, s))) return rc;
-  if ((rc = run_cross_kv(o1, L, b3, 3 * (size_t)B_SIZE, ws.kvc + KVSZ, ws, s))) return rc;
+  if ((rc = run_block(o1, 1, L, b2, 2 * (size_t)G_BLK, nullptr, ws, s, true, nullptr))) return rc;
+  if ((rc = run_cross_kv(ws.ref0, L, b1, (size_t)G_BLK, ws.kvc, ws, s))) return rc;
+  if ((rc = run_cross_kv(o1, L, b3, 3 * (size_t)G_BLK, ws.kvc + KVSZ, ws, s))) return rc;
   // source views as one batch: self, cross(ref_list[0]), self, cross(ref_list[1])   (FMT.py:119-135)
   float* xs = o1 + (size_t)L * 64;
   if ((rc = run_block(xs, V - 1, L, b0, 0, nullptr, ws, s, false, b1))) return rc;
-  if ((rc = run_block(xs, V - 1, L, b1, (size_t)B_SIZE, ws.kvc, ws, s, true, b2))) return rc;
-  if ((rc = run_block(xs, V - 1, L, b2, 2 * (size_t)B_SIZE, nullptr, ws, s, true, b3))) return rc;
-  if ((rc = run_block(xs, V - 1, L, b3, 3 * (size_t)B_SIZE, ws.kvc + KVSZ, ws, s, true, nullptr))) return rc;
+  if ((rc = run_block(xs, V - 1, L, b1, (size_t)G_BLK, ws.kvc, ws, s, true, b2))) return rc;
+  if ((rc = run_block(xs, V - 1, L, b2, 2 * (size_t)G_BLK, nullptr, ws, s, true, b3))) return rc;
+  if ((rc = run_block(xs, V - 1, L, b3, 3 * (size_t)G_BLK, ws.kvc + KVSZ, ws, s, true, nullptr))) return rc;
 
   // top-down pathway (FMT.py:195-197), all views batched
   unsigned char* sm_tc = static_cast<unsigned char*>(workspace) + need - SM_TC;

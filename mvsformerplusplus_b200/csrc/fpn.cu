@@ -215,12 +215,16 @@ __global__ void __launch_bounds__(128) fpn_out0_kernel(const float* __restrict__
   }
 }
 
-// ---- layer table.  fp32 blobs (packing.pack_fpn_encoder / pack_fpn_decoder): per layer w [KS*KS][CI][CO] then b[CO]
+// ---- layer table.  Each module's weights come in two fp32 parts (packing.pack_fpn_encoder / pack_fpn_decoder), each
+// counted from 0: the conv part holds the weights w [KS*KS][CI][CO] of the tensor-core convolutions (the input of
+// mvsf_fpn_pack_tc); the small part, the wts argument, holds what the kernels read in fp32.
 struct LayerDesc { int ci, co, ks, ns; };
+// encoder conv part: conv01 ... conv31 w; small part: conv00 w [49][3][8] b[8] (SIMT), then b[CO] of conv01 ... conv31
 constexpr LayerDesc kEnc[11] = {{3, 8, 7, 0},    {8, 8, 5, 8},    {8, 16, 5, 16},  {16, 16, 3, 16},
                                 {16, 16, 3, 16}, {16, 32, 5, 32}, {32, 32, 3, 32}, {32, 32, 3, 32},
                                 {32, 64, 3, 32}, {64, 64, 3, 32}, {64, 64, 3, 32}};
-// decoder blob: out0 [64][64] b[64]; then per level k = 1..3: inner_k [CL][64] b[64], out_k [9][64][C_k] b[C_k]
+// decoder conv part: out_k [9][64][C_k], k = 1..3; small part: out0 [64][64] b[64], then per level k = 1..3:
+// inner_k [CL][64] b[64], out_k b[C_k]
 constexpr LayerDesc kDec[3] = {{64, 32, 3, 32}, {64, 16, 3, 16}, {64, 8, 3, 8}};
 constexpr int kLat[3] = {32, 16, 8};
 
@@ -228,15 +232,25 @@ template <int I> using EncL = Conv<kEnc[I].ci, kEnc[I].co, kEnc[I].ks, (I == 2 |
                                    (I >= 8) ? 8 : 16, kEnc[I].ns>;
 template <int K> using DecL = Conv<64, kDec[K].co, 3, 1, K == 0 ? 8 : 16, kDec[K].ns>;
 
-constexpr size_t layer_floats(const LayerDesc& d) { return (size_t)d.ks * d.ks * d.ci * d.co + d.co; }
+constexpr size_t conv_floats(const LayerDesc& d) { return (size_t)d.ks * d.ks * d.ci * d.co; }
 constexpr size_t layer_tc_bytes(const LayerDesc& d) { return conv2d_tc_bytes(d.ci, d.co, d.ks); }
-static size_t enc_off(int i) { size_t o = 0; for (int j = 0; j < i; ++j) o += layer_floats(kEnc[j]); return o; }
-static size_t enc_tc_off(int i) { size_t o = 0; for (int j = 1; j < i; ++j) o += layer_tc_bytes(kEnc[j]); return o; }
-static size_t dec_inner_off(int k) {   // float offset of inner_{k+1}
-  size_t o = 64 * 64 + 64;
-  for (int j = 0; j < k; ++j) o += (size_t)kLat[j] * 64 + 64 + layer_floats(kDec[j]);
+constexpr size_t enc_conv_off(int i) { size_t o = 0; for (int j = 1; j < i; ++j) o += conv_floats(kEnc[j]); return o; }
+constexpr size_t enc_bias_off(int i) {   // small-part offset of b of encoder layer i
+  size_t o = conv_floats(kEnc[0]);
+  for (int j = 0; j < i; ++j) o += kEnc[j].co;
   return o;
 }
+static size_t enc_tc_off(int i) { size_t o = 0; for (int j = 1; j < i; ++j) o += layer_tc_bytes(kEnc[j]); return o; }
+constexpr size_t dec_conv_off(int k) { size_t o = 0; for (int j = 0; j < k; ++j) o += conv_floats(kDec[j]); return o; }
+constexpr size_t dec_inner_off(int k) {   // small-part offset of inner_{k+1}
+  size_t o = 64 * 64 + 64;
+  for (int j = 0; j < k; ++j) o += (size_t)kLat[j] * 64 + 64 + kDec[j].co;
+  return o;
+}
+constexpr size_t dec_bias_off(int k) { return dec_inner_off(k) + (size_t)kLat[k] * 64 + 64; }   // b of out_{k+1}
+static_assert(enc_conv_off(11) == 132800 && enc_bias_off(11) == 1528 && dec_conv_off(3) == 32256 &&
+                  dec_inner_off(3) == 7992,
+              "packing.FPN_ENCODER_CONV_WTS / FPN_ENCODER_SMALL_WTS / FPN_DECODER_CONV_WTS / FPN_DECODER_SMALL_WTS");
 static size_t dec_tc_off(int k) { size_t o = 0; for (int j = 0; j < k; ++j) o += layer_tc_bytes(kDec[j]); return o; }
 static size_t enc_tc_total() { return enc_tc_off(11); }
 static size_t dec_tc_total() { return dec_tc_off(3); }
@@ -247,17 +261,16 @@ static int enc_layer(const float* in, float* out, const float* wts, const unsign
                      cudaStream_t s) {
   using L = EncL<I>;
   const int OH = IH / L::S, OW = IW / L::S;
-  const float* bias = wts + enc_off(I) + (size_t)L::KS * L::KS * L::CI * L::CO;
-  return launch_conv<L>(NhwcSrc<L>{in, IH, IW}, NhwcLeaky<L::CO>{out}, wtc + enc_tc_off(I), bias, N, OH, OW, s);
+  return launch_conv<L>(NhwcSrc<L>{in, IH, IW}, NhwcLeaky<L::CO>{out}, wtc + enc_tc_off(I), wts + enc_bias_off(I), N,
+                        OH, OW, s);
 }
 
 template <int K>
 static int dec_level(const float* prev, const float* lat, const float* wts, const unsigned char* wtc, float* intra_out,
                      float* out, int N, int h, int w, cudaStream_t s) {
   using L = DecL<K>;
-  const size_t inner = dec_inner_off(K), conv = inner + (size_t)kLat[K] * 64 + 64;
-  return launch_conv<L>(IntraSrc<L, kLat[K]>{prev, lat, wts + inner, intra_out, h, w},
-                        NchwSwish<L::CO>{out}, wtc + dec_tc_off(K), wts + conv + (size_t)9 * 64 * L::CO, N, 2 * h, 2 * w, s);
+  return launch_conv<L>(IntraSrc<L, kLat[K]>{prev, lat, wts + dec_inner_off(K), intra_out, h, w},
+                        NchwSwish<L::CO>{out}, wtc + dec_tc_off(K), wts + dec_bias_off(K), N, 2 * h, 2 * w, s);
 }
 
 // conv31: the last encoder layer, optionally with the model's + vit_feat in its epilogue
@@ -265,9 +278,8 @@ static int enc_last(const float* in, float* out, const float* vit, int V, const 
                     int N, int IH, int IW, cudaStream_t s) {
   if (vit == nullptr) return enc_layer<10>(in, out, wts, wtc, N, IH, IW, s);
   using L = EncL<10>;
-  const float* bias = wts + enc_off(10) + (size_t)L::KS * L::KS * L::CI * L::CO;
-  return launch_conv<L>(NhwcSrc<L>{in, IH, IW}, NhwcLeakyAddVit<L::CO>{out, vit, V}, wtc + enc_tc_off(10), bias, N, IH,
-                        IW, s);
+  return launch_conv<L>(NhwcSrc<L>{in, IH, IW}, NhwcLeakyAddVit<L::CO>{out, vit, V}, wtc + enc_tc_off(10),
+                        wts + enc_bias_off(10), N, IH, IW, s);
 }
 
 static bool shape_ok(int N, int H, int W) {
@@ -286,14 +298,14 @@ extern "C" int mvsf_fpn_tc_bytes(int part, size_t* bytes) {
   return MVSF_OK;
 }
 
-extern "C" int mvsf_fpn_pack_tc(int part, const float* wts, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream) {
-  MVSF_REQUIRE(wts && wts_tc && (part == 0 || part == 1), "fpn_pack_tc: bad arguments");
+extern "C" int mvsf_fpn_pack_tc(int part, const float* conv, void* wts_tc, size_t wts_tc_bytes, mvsf_stream_t stream) {
+  MVSF_REQUIRE(conv && wts_tc && (part == 0 || part == 1), "fpn_pack_tc: bad arguments");
   MVSF_REQUIRE(wts_tc_bytes >= (part == 0 ? enc_tc_total() : dec_tc_total()), "fpn_pack_tc: wts_tc too small");
   unsigned char* out = static_cast<unsigned char*>(wts_tc);
   const int n = part == 0 ? 10 : 3;
   for (int j = 0; j < n; ++j) {
     const LayerDesc& d = part == 0 ? kEnc[j + 1] : kDec[j];
-    const float* w = wts + (part == 0 ? enc_off(j + 1) : dec_inner_off(j) + (size_t)kLat[j] * 64 + 64);
+    const float* w = conv + (part == 0 ? enc_conv_off(j + 1) : dec_conv_off(j));
     unsigned char* o = out + (part == 0 ? enc_tc_off(j + 1) : dec_tc_off(j));
     const int rc = pack_conv2d_tc(w, o, d.ci, d.co, d.ks, d.ns, (cudaStream_t)stream);
     if (rc) return rc;
@@ -320,8 +332,8 @@ static int encoder_forward(const float* x, const float* vit, int V, const float*
   float* t0 = static_cast<float*>(workspace);
   float* t1 = t0 + (size_t)N * H * W * 4;
   using L1 = EncL<1>;
-  int rc = launch_conv<L1>(Conv00Src<L1>{x, wts + enc_off(0), H, W}, NhwcLeaky<8>{c01}, wtc + enc_tc_off(1),
-                           wts + enc_off(1) + 25 * 8 * 8, N, H, W, s);
+  int rc = launch_conv<L1>(Conv00Src<L1>{x, wts, H, W}, NhwcLeaky<8>{c01}, wtc + enc_tc_off(1), wts + enc_bias_off(1),
+                           N, H, W, s);
   if (rc) return rc;
   if ((rc = enc_layer<2>(c01, t0, wts, wtc, N, H, W, s))) return rc;
   if ((rc = enc_layer<3>(t0, t1, wts, wtc, N, H / 2, W / 2, s))) return rc;

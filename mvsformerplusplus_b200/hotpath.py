@@ -78,10 +78,10 @@ def split_weights_f16(flat):
     return _pack_f16("split_weights_f16", flat)
 
 
-def pack_unet_tc(kind, flat):
-    """fp32 U-Net weight blob (packing.pack_costreg_unet) on the device -> fp16 hi/lo weight slabs of the wgmma
-    implicit-GEMM convolutions (install time, once)."""
-    return _pack_f16("costreg_unet_pack_tc", flat, kind, query=("costreg_unet_tc_bytes",))
+def pack_unet_tc(kind, conv):
+    """fp32 U-Net conv weights (the conv part of packing.pack_costreg_unet) on the device -> fp16 hi/lo weight slabs of
+    the wgmma implicit-GEMM convolutions (install time, once)."""
+    return _pack_f16("costreg_unet_pack_tc", conv, kind, query=("costreg_unet_tc_bytes",))
 
 
 @torch.no_grad()
@@ -164,19 +164,17 @@ class StageNet(_PackedMixin, nn.Module):
         sd = {k: v for k, v in self.state_dict().items()}
         pk = {"vis": packing.pack_vis(sd, "vis.").to(device)}
         if self.cost_reg_type == "PureTransformerCostReg":
-            tc = self.args["transformer_config"][self.stage_idx]
-            if tuple(tc["down_rate"]) != (2, 4, 4) or tc["mid_channel"] != 64 or tc["num_heads"] != 4 or tc["mlp_ratio"] != 4:
+            cfg = self.args["transformer_config"][self.stage_idx]
+            if (tuple(cfg["down_rate"]) != (2, 4, 4) or cfg["mid_channel"] != 64 or cfg["num_heads"] != 4
+                    or cfg["mlp_ratio"] != 4):
                 raise NotImplementedError("transformer regulariser: only the shipped geometry (down_rate (2,4,4), "
                                           "mid 64, 4 heads, mlp_ratio 4) is implemented")
-            pk["kind"] = "tr"
-            pk["layers"] = tc["layer_num"]
-            pk["reg"] = packing.pack_costreg_tr(sd, "cost_reg.", tc["layer_num"]).to(device)
-            pk["reg16"] = split_weights_f16(pk["reg"])
+            gemm, small = packing.pack_costreg_tr(sd, "cost_reg.", cfg["layer_num"])
+            pk.update(kind="tr", layers=cfg["layer_num"], tc=split_weights_f16(gemm.to(device)))
         else:
-            kind, flat = packing.pack_costreg_unet(sd, "cost_reg.")
-            pk["kind"] = kind
-            pk["reg"] = flat.to(device)
-            pk["reg_tc"] = pack_unet_tc(kind, pk["reg"])
+            kind, conv, small = packing.pack_costreg_unet(sd, "cost_reg.")
+            pk.update(kind=kind, tc=pack_unet_tc(kind, conv.to(device)))
+        pk["w"] = small.to(device)
         return pk
 
     def _softmax_scale(self, n_tokens):
@@ -220,11 +218,11 @@ class StageNet(_PackedMixin, nn.Module):
         if pk["kind"] == "tr":
             ws = _lib.workspace("mvsf_costreg_tr_workspace_bytes", G, D, H, W, device=dev)
             n_tok = (D // 2) * (H // 4) * (W // 4)
-            _lib.call("mvsf_costreg_tr_forward", volume, position3d, pk["reg"], pk["reg16"], pk["reg"].numel(), logits,
+            _lib.call("mvsf_costreg_tr_forward", volume, position3d, pk["w"], pk["tc"], pk["tc"].numel() // 2, logits,
                       ws, ws.numel() * 4, G, D, H, W, pk["layers"], float(self._softmax_scale(n_tok)))
         else:
             ws = _lib.workspace("mvsf_costreg_unet_workspace_bytes", pk["kind"], G, D, H, W, device=dev)
-            _lib.call("mvsf_costreg_unet_forward", pk["kind"], volume, pk["reg"], pk["reg_tc"], logits, ws, ws.numel() * 4,
+            _lib.call("mvsf_costreg_unet_forward", pk["kind"], volume, pk["w"], pk["tc"], logits, ws, ws.numel() * 4,
                       G, D, H, W)
         prob = torch.empty((D, H, W), **f32)
         depth = torch.empty((H, W), **f32)
@@ -286,8 +284,9 @@ class FMT_with_pathway(_PackedMixin, nn.Module):
 
     def _build_pack(self, device):
         sd = {"FMT_module." + k: v for k, v in self.state_dict().items()}
-        w = packing.pack_fmt(sd).to(device)
-        return {"w": w, "w16": split_weights_f16(w)}
+        gemm, small = packing.pack_fmt(sd)
+        tc = split_weights_f16(gemm.to(device))
+        return {"w": small.to(device), "tc": tc}
 
     def _pe(self, H, W, device):
         """PositionEncodingSineNorm table (position_encoding.py:61-74) as [H*W, 64], cached per shape like the
@@ -323,7 +322,8 @@ class FMT_with_pathway(_PackedMixin, nn.Module):
                 if tuple(ins[k].shape) != (V, c, H1 * sc, W1 * sc):
                     raise AssertionError(f"stage{k + 1} features must be [V,{c},{H1 * sc},{W1 * sc}], got {tuple(ins[k].shape)}")
             o = [torch.empty((V, H1 * sc, W1 * sc, c), **f32) for c, sc in ((64, 1), (32, 2), (16, 4), (8, 8))]
-            _lib.call("mvsf_fmt_forward", *ins, pe, pk["w"], pk["w16"], pk["w"].numel(), *o, ws, ws.numel() * 4, V, H1, W1)
+            _lib.call("mvsf_fmt_forward", *ins, pe, pk["w"], pk["tc"], pk["tc"].numel() // 2, *o, ws, ws.numel() * 4,
+                      V, H1, W1)
             for k in range(4):
                 outs[f"stage{k + 1}"].append(o[k])
         # logical [B,V,C,H,W]; channels-last in memory (StageNet consumes it without a copy)
@@ -439,8 +439,9 @@ class FPNEncoder(_PackedMixin, nn.Module):
         self._init_packing()
 
     def _build_pack(self, device):
-        w = packing.pack_fpn_encoder(self.state_dict(), "").to(device)
-        return {"w": w, "tc": _pack_f16("fpn_pack_tc", w, 0, query=("fpn_tc_bytes", 0))}
+        conv, small = packing.pack_fpn_encoder(self.state_dict(), "")
+        tc = _pack_f16("fpn_pack_tc", conv.to(device), 0, query=("fpn_tc_bytes", 0))
+        return {"w": small.to(device), "tc": tc}
 
     @torch.no_grad()
     def forward(self, x, vit_feat=None):
@@ -481,8 +482,9 @@ class FPNDecoder(_PackedMixin, nn.Module):
         self._init_packing()
 
     def _build_pack(self, device):
-        w = packing.pack_fpn_decoder(self.state_dict(), "").to(device)
-        return {"w": w, "tc": _pack_f16("fpn_pack_tc", w, 1, query=("fpn_tc_bytes", 1))}
+        conv, small = packing.pack_fpn_decoder(self.state_dict(), "")
+        tc = _pack_f16("fpn_pack_tc", conv.to(device), 1, query=("fpn_tc_bytes", 1))
+        return {"w": small.to(device), "tc": tc}
 
     @torch.no_grad()
     def forward(self, conv01, conv11, conv21, conv31):

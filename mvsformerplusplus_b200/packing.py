@@ -39,16 +39,23 @@ def pack_vis(sd, p):
     return out
 
 
+COSTREG_UNET_CONV_WTS = 290304          # floats of the conv part of pack_costreg_unet (csrc/costreg_unet.cu NCONV)
+COSTREG_UNET_SMALL_WTS = (496, 292)     # floats of its small part by kind (csrc/costreg_unet.cu NSMALL)
+
+
 def pack_costreg_unet(sd, p):
-    """p = 'fusions.{s}.cost_reg.'  -> (kind, flat) ; kind 0 = CostRegNet, 1 = CostRegNet3D"""
+    """p = 'fusions.{s}.cost_reg.'  -> (kind, conv, small); kind 0 = CostRegNet, 1 = CostRegNet3D.  conv: per layer
+    conv1 ... conv6, conv7, conv9, conv11 the weights [27 taps][ci][co] with BN scale folded (the input of
+    mvsf_costreg_unet_pack_tc).  small, the wts argument: per layer the folded shift [co]; then the prob conv, [27][8]
+    (kind 0) or w[8], b (kind 1)."""
     is3d = (p + "conv7.0.weight") in sd
-    parts = []
+    conv, small = [], []
     for name in ("conv1", "conv2", "conv3", "conv4", "conv5", "conv6"):
         w = _d(sd[f"{p}{name}.conv.weight"])  # [cout, cin, 3,3,3]
         scale, shift = _fold_bn(sd, f"{p}{name}.bn.")
         w = w * scale.view(-1, 1, 1, 1, 1)
-        parts.append(w.permute(2, 3, 4, 1, 0).reshape(27, w.shape[1], w.shape[0]))  # [tap][ci][co]
-        parts.append(shift)
+        conv.append(w.permute(2, 3, 4, 1, 0).reshape(27, w.shape[1], w.shape[0]))  # [tap][ci][co]
+        small.append(shift)
     for name in ("conv7", "conv9", "conv11"):
         if is3d:
             w = _d(sd[f"{p}{name}.0.weight"])  # [cin, cout, 3,3,3]
@@ -57,34 +64,49 @@ def pack_costreg_unet(sd, p):
             w = _d(sd[f"{p}{name}.conv.weight"])
             scale, shift = _fold_bn(sd, f"{p}{name}.bn.")
         w = w * scale.view(1, -1, 1, 1, 1)
-        parts.append(w.permute(2, 3, 4, 0, 1).reshape(27, w.shape[0], w.shape[1]))  # [tap][ci][co]
-        parts.append(shift)
+        conv.append(w.permute(2, 3, 4, 0, 1).reshape(27, w.shape[0], w.shape[1]))  # [tap][ci][co]
+        small.append(shift)
     pw = _d(sd[p + "prob.weight"])
     if is3d:
-        parts += [pw.reshape(8), _d(sd[p + "prob.bias"]).reshape(1)]
+        small += [pw.reshape(8), _d(sd[p + "prob.bias"]).reshape(1)]
     else:
-        parts.append(pw[0].permute(1, 2, 3, 0).reshape(27, 8))  # [tap][ci]
-    return (1 if is3d else 0), _cat(parts)
+        small.append(pw[0].permute(1, 2, 3, 0).reshape(27, 8))  # [tap][ci]
+    kind = 1 if is3d else 0
+    conv, small = _cat(conv), _cat(small)
+    sizes = conv.numel(), small.numel()
+    assert sizes == (COSTREG_UNET_CONV_WTS, COSTREG_UNET_SMALL_WTS[kind]), sizes
+    return kind, conv, small
+
+
+def costreg_tr_wts(layers):
+    """floats of the (gemm, small) parts of pack_costreg_tr (csrc/costreg_tr.cu tr_gemm_floats / tr_small_floats)"""
+    return 32768 + 49152 * layers, 672 + 768 * layers
 
 
 def pack_costreg_tr(sd, p, layers):
-    """p = 'fusions.{s}.cost_reg.' ; layout documented in csrc/costreg_tr.cu"""
-    parts = [_d(sd[p + "pe_proj.weight"]).reshape(8, 24)]
+    """p = 'fusions.{s}.cost_reg.' -> (gemm, small), the two fp32 parts of mvsf_costreg_tr_forward's weights (layout
+    in csrc/costreg_tr.cu).  gemm, as [N][K] rows: down [64][256], per layer qkv [192][64], proj, linear1, linear2, then
+    up [256][64].  small, the wts argument: pe_proj, the down bias and LayerNorm, per layer proj bias, gamma1, norm1,
+    linear1 bias, linear2 bias, gamma2, norm2; the up bias (repeated per voxel), its LayerNorm and prob."""
     wd = _d(sd[p + "down.0.weight"])  # [64, 8, 2,4,4] -> [64][kd][kh][kw][ci]
-    parts += [wd.permute(0, 2, 3, 4, 1).reshape(64, 256), _d(sd[p + "down.0.bias"]),
-              _d(sd[p + "down.1.weight"]), _d(sd[p + "down.1.bias"])]
+    g = [wd.permute(0, 2, 3, 4, 1).reshape(64, 256)]
+    small = [_d(sd[p + "pe_proj.weight"]).reshape(8, 24), _d(sd[p + "down.0.bias"]),
+             _d(sd[p + "down.1.weight"]), _d(sd[p + "down.1.bias"])]
     for i in range(layers):
         q = f"{p}attention_layers.{i}."
-        parts += [_d(sd[q + "attn.qkv.weight"]), _d(sd[q + "attn.proj.weight"]), _d(sd[q + "attn.proj.bias"]),
-                  _d(sd[q + "gamma1"]).reshape(1).expand(64), _d(sd[q + "norm1.weight"]), _d(sd[q + "norm1.bias"]),
-                  _d(sd[q + "ffn.linear1.weight"]), _d(sd[q + "ffn.linear1.bias"]),
-                  _d(sd[q + "ffn.linear2.weight"]), _d(sd[q + "ffn.linear2.bias"]),
+        g += [_d(sd[q + k]) for k in ("attn.qkv.weight", "attn.proj.weight", "ffn.linear1.weight",
+                                      "ffn.linear2.weight")]
+        small += [_d(sd[q + "attn.proj.bias"]), _d(sd[q + "gamma1"]).reshape(1).expand(64), _d(sd[q + "norm1.weight"]),
+                  _d(sd[q + "norm1.bias"]), _d(sd[q + "ffn.linear1.bias"]), _d(sd[q + "ffn.linear2.bias"]),
                   _d(sd[q + "gamma2"]).reshape(1).expand(64), _d(sd[q + "norm2.weight"]), _d(sd[q + "norm2.bias"])]
     wu = _d(sd[p + "up.0.weight"])  # [64 ci, 8 co, 2,4,4] -> [kd][kh][kw][co][ci] = [256][64]
-    parts += [wu.permute(2, 3, 4, 1, 0).reshape(256, 64), _d(sd[p + "up.0.bias"]).repeat(32),
-              _d(sd[p + "up.1.weight"]), _d(sd[p + "up.1.bias"]),
+    g.append(wu.permute(2, 3, 4, 1, 0).reshape(256, 64))
+    small += [_d(sd[p + "up.0.bias"]).repeat(32), _d(sd[p + "up.1.weight"]), _d(sd[p + "up.1.bias"]),
               _d(sd[p + "prob.weight"]).reshape(8), _d(sd[p + "prob.bias"]).reshape(1)]
-    return _cat(parts, pad_to=8)  # multiple of 8 floats: the fp16 hi/lo copies stay 16-byte aligned
+    g, small = _cat(g, pad_to=8), _cat(small, pad_to=8)
+    sizes = g.numel(), small.numel()
+    assert sizes == costreg_tr_wts(layers), sizes
+    return g, small
 
 
 def fold_conv_bn(sd, conv, bn, bias=None):
@@ -98,46 +120,74 @@ def fold_conv_bn(sd, conv, bn, bias=None):
     return w.permute(2, 3, 1, 0).reshape(w.shape[2] * w.shape[3], w.shape[1], w.shape[0]), shift
 
 
+FPN_ENCODER_CONV_WTS = 132800   # floats of the conv part of pack_fpn_encoder (csrc/fpn.cu enc_conv_off(11))
+FPN_ENCODER_SMALL_WTS = 1528    # floats of its small part (csrc/fpn.cu enc_bias_off(11))
+
+
 def pack_fpn_encoder(sd, p="encoder."):
-    """models/module.py:208-239 -> per layer (conv00 ... conv31) w [k*k][ci][co] with BN folded, then shift [co]
-    (layout documented in include/mvsf_b200.h, mvsf_fpn_encoder_forward)"""
+    """models/module.py:208-239 -> (conv, small), the two fp32 parts of the encoder's weights (layout documented in
+    include/mvsf_b200.h, mvsf_fpn_encoder_forward).  conv: the weights [k*k][ci][co] with BN folded of conv01 ...
+    conv31, the layers that run on the tensor cores (the input of mvsf_fpn_pack_tc).  small, the wts argument: conv00's
+    weights and shift (computed in SIMT), then the shifts [co] of conv01 ... conv31."""
     from .params import FPN_ENCODER_LAYERS
-    parts = []
-    for name, *_ in FPN_ENCODER_LAYERS:
-        parts += list(fold_conv_bn(sd, f"{p}{name}.conv.weight", f"{p}{name}.bn."))
-    return _cat(parts)
+    conv, small = [], []
+    for i, (name, *_) in enumerate(FPN_ENCODER_LAYERS):
+        w, shift = fold_conv_bn(sd, f"{p}{name}.conv.weight", f"{p}{name}.bn.")
+        (small if i == 0 else conv).append(w)
+        small.append(shift)
+    conv, small = _cat(conv), _cat(small)
+    sizes = conv.numel(), small.numel()
+    assert sizes == (FPN_ENCODER_CONV_WTS, FPN_ENCODER_SMALL_WTS), sizes
+    return conv, small
+
+
+FPN_DECODER_CONV_WTS = 32256    # floats of the conv part of pack_fpn_decoder (csrc/fpn.cu dec_conv_off(3))
+FPN_DECODER_SMALL_WTS = 7992    # floats of its small part (csrc/fpn.cu dec_inner_off(3))
 
 
 def pack_fpn_decoder(sd, p="decoder."):
-    """models/module.py:242-270 -> out0 [64][64] + shift; per level k = 1..3: inner_k [cl][64] + bias[64], out_k
-    [9][64][c_k] + shift (conv bias and BN folded; layout documented in include/mvsf_b200.h, mvsf_fpn_decoder_forward)"""
-    parts = list(fold_conv_bn(sd, p + "out0.0.weight", p + "out0.1.", p + "out0.0.bias"))
+    """models/module.py:242-270 -> (conv, small), the two fp32 parts of the decoder's weights (conv bias and BN folded;
+    layout documented in include/mvsf_b200.h, mvsf_fpn_decoder_forward).  conv: out_k [9][64][c_k], k = 1..3 (the input
+    of mvsf_fpn_pack_tc).  small, the wts argument: out0 [64][64] + shift; per level k = 1..3: inner_k [cl][64] +
+    bias[64], out_k's shift [c_k]."""
+    small = list(fold_conv_bn(sd, p + "out0.0.weight", p + "out0.1.", p + "out0.0.bias"))
+    conv = []
     for k in (1, 2, 3):
         wi = _d(sd[f"{p}inner{k}.weight"])  # [64, cl, 1, 1]
-        parts += [wi.reshape(wi.shape[0], wi.shape[1]).t(), _d(sd[f"{p}inner{k}.bias"])]
-        parts += list(fold_conv_bn(sd, f"{p}out{k}.0.weight", f"{p}out{k}.1.", f"{p}out{k}.0.bias"))
-    return _cat(parts)
+        w, shift = fold_conv_bn(sd, f"{p}out{k}.0.weight", f"{p}out{k}.1.", f"{p}out{k}.0.bias")
+        small += [wi.reshape(wi.shape[0], wi.shape[1]).t(), _d(sd[f"{p}inner{k}.bias"]), shift]
+        conv.append(w)
+    conv, small = _cat(conv), _cat(small)
+    sizes = conv.numel(), small.numel()
+    assert sizes == (FPN_DECODER_CONV_WTS, FPN_DECODER_SMALL_WTS), sizes
+    return conv, small
+
+
+FMT_GEMM_WTS = 196608   # floats of the GEMM part of pack_fmt (csrc/fmt.cu NG)
+FMT_SMALL_WTS = 17856   # floats of its small part (csrc/fmt.cu NS)
 
 
 def pack_fmt(sd, p="FMT_module."):
-    """layout documented in csrc/fmt.cu"""
-    parts = []
+    """-> (gemm, small), the two fp32 parts of mvsf_fmt_forward's weights (layout in csrc/fmt.cu).  gemm, per block as
+    [N][K] rows: [q; k; v] [192][64], proj, fc1, fc2.  small, the wts argument: per block norm1 w, b, proj bias, ls1,
+    norm2 w, b, fc1 bias, fc2 bias, ls2; then dim_reduction_1..3 [co][ci] and smooth_1..3 [tap][ci][co]."""
+    g, small = [], []
     for i in range(4):
         q = f"{p}FMT.layers.{i}."
-        parts += [_d(sd[q + "norm1.weight"]), _d(sd[q + "norm1.bias"]),
-                  torch.cat([_d(sd[q + "attn.q_proj.weight"]), _d(sd[q + "attn.k_proj.weight"]),
-                             _d(sd[q + "attn.v_proj.weight"])], 0),
-                  _d(sd[q + "attn.proj.weight"]), _d(sd[q + "attn.proj.bias"]), _d(sd[q + "ls1.gamma"]),
-                  _d(sd[q + "norm2.weight"]), _d(sd[q + "norm2.bias"]),
-                  _d(sd[q + "mlp.fc1.weight"]), _d(sd[q + "mlp.fc1.bias"]),
-                  _d(sd[q + "mlp.fc2.weight"]), _d(sd[q + "mlp.fc2.bias"]), _d(sd[q + "ls2.gamma"])]
+        g += [torch.cat([_d(sd[q + "attn.q_proj.weight"]), _d(sd[q + "attn.k_proj.weight"]),
+                         _d(sd[q + "attn.v_proj.weight"])], 0),
+              _d(sd[q + "attn.proj.weight"]), _d(sd[q + "mlp.fc1.weight"]), _d(sd[q + "mlp.fc2.weight"])]
+        small += [_d(sd[q + k]) for k in ("norm1.weight", "norm1.bias", "attn.proj.bias", "ls1.gamma", "norm2.weight",
+                                          "norm2.bias", "mlp.fc1.bias", "mlp.fc2.bias", "ls2.gamma")]
     for k in (1, 2, 3):
         w = _d(sd[f"{p}dim_reduction_{k}.weight"])
-        parts.append(w.reshape(w.shape[0], w.shape[1]))
+        small.append(w.reshape(w.shape[0], w.shape[1]))
     for k in (1, 2, 3):
         w = _d(sd[f"{p}smooth_{k}.weight"])  # [co, ci, 3, 3] -> [tap][ci][co]
-        parts.append(w.permute(2, 3, 1, 0).reshape(9, w.shape[1], w.shape[0]))
-    return _cat(parts, pad_to=8)
+        small.append(w.permute(2, 3, 1, 0).reshape(9, w.shape[1], w.shape[0]))
+    g, small = _cat(g, pad_to=8), _cat(small, pad_to=8)
+    assert g.numel() == FMT_GEMM_WTS and small.numel() == FMT_SMALL_WTS, (g.numel(), small.numel())
+    return g, small
 
 
 VIT_DECODER_BLOCKS = tuple(f"self_attn_blocks.{i}." for i in range(2)) + tuple(f"cross_attn_blocks.{i}." for i in range(3))

@@ -45,28 +45,30 @@ def test_fpn_state_dict_keys_match_reference_inventory():
     assert got == ref
 
 
-def test_fpn_packing_folds_conv_bn():
+def test_fpn_two_part_packing_folds_conv_bn():
     sd = fpn_state_dict(5)
     x = torch.randn(1, 8, 11, 13, dtype=torch.float64)
-    enc = packing.pack_fpn_encoder(sd).double()
-    # layer 1 (conv01) follows conv00: [49][3][8] + 8 floats
-    off = 49 * 3 * 8 + 8
-    w = enc[off:off + 25 * 64].view(5, 5, 8, 8).permute(3, 2, 0, 1)
-    b = enc[off + 25 * 64:off + 25 * 64 + 8]
+    conv, small = (t.double() for t in packing.pack_fpn_encoder(sd))
+    # layer 1 (conv01): the first weights of the conv part; its shift follows conv00's [49][3][8] + 8 in the small part
+    w = conv[:25 * 64].view(5, 5, 8, 8).permute(3, 2, 0, 1)
+    b = small[49 * 3 * 8 + 8:49 * 3 * 8 + 16]
     got = F.conv2d(x, w, b, padding=2)
     want = OF._bn(F.conv2d(x, sd["encoder.conv01.conv.weight"].double(), padding=2), sd, "encoder.conv01.bn.")
     assert max_abs(got, want) < 1e-5
-    assert enc.numel() == sum(k * k * ci * co + co for _, ci, co, k, _ in FPN_ENCODER_LAYERS)
-    dec = packing.pack_fpn_decoder(sd).double()
-    # out1: after out0 (64*64 + 64) and inner1 (32*64 + 64); w [9][64][32] + shift[32]
+    assert conv.numel() == sum(k * k * ci * co for _, ci, co, k, _ in FPN_ENCODER_LAYERS[1:]) == 132800
+    assert small.numel() == 49 * 3 * 8 + sum(co for _, ci, co, k, _ in FPN_ENCODER_LAYERS) == 1528
+    conv, small = (t.double() for t in packing.pack_fpn_decoder(sd))
+    # out1: the first weights of the conv part, w [9][64][32]; its shift follows out0 (64*64 + 64) and inner1
+    # (32*64 + 64) in the small part
     off = 64 * 64 + 64 + 32 * 64 + 64
     x = torch.randn(1, 64, 7, 9, dtype=torch.float64)
-    w = dec[off:off + 9 * 64 * 32].view(3, 3, 64, 32).permute(3, 2, 0, 1)
-    b = dec[off + 9 * 64 * 32:off + 9 * 64 * 32 + 32]
+    w = conv[:9 * 64 * 32].view(3, 3, 64, 32).permute(3, 2, 0, 1)
+    b = small[off:off + 32]
     got = F.conv2d(x, w, b, padding=1)
     want = OF._bn(F.conv2d(x, sd["decoder.out1.0.weight"].double(), sd["decoder.out1.0.bias"].double(), padding=1), sd,
                   "decoder.out1.1.")
     assert max_abs(got, want) < 1e-5
+    assert (conv.numel(), small.numel()) == (32256, 7992)
 
 
 def test_fpn_rejects_unsupported_configurations_and_sizes():

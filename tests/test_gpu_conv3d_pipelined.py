@@ -109,7 +109,7 @@ def _rand_sd(seed):
 
 # stage 1 = CostRegNet (fp32 OUT_F32 epilogue + prob3), stages 2, 3 = CostRegNet3D (fused OUT_PROB epilogue)
 @pytest.mark.parametrize("stage,D,H,W", [(1, 8, 40, 24), (1, 16, 24, 56), (2, 5, 40, 56), (3, 1, 24, 24), (3, 16, 16, 8)])
-def test_costreg_unet_pipelined(dev, stage, D, H, W):
+def test_costreg_unet_two_part_pipelined(dev, stage, D, H, W):
     from mvsformerplusplus_b200 import packing
     from mvsformerplusplus_b200.hotpath import pack_unet_tc
     from oracle import hotpath as O
@@ -118,14 +118,13 @@ def test_costreg_unet_pipelined(dev, stage, D, H, W):
     vol = torch.randn(1, 8, D, H, W, generator=g) * 0.5
     p = f"fusions.{stage}.cost_reg."
     want = O.costreg_unet(vol, sd, p)[0, 0]
-    kind, flat = packing.pack_costreg_unet(sd, p)
+    kind, conv, small = packing.pack_costreg_unet(sd, p)
     assert kind == (0 if stage == 1 else 1)
     ws = _lib.workspace("mvsf_costreg_unet_workspace_bytes", kind, 8, D, H, W, device=dev)
     logits = torch.empty(D, H, W, device=dev)
     v = vol[0].permute(1, 2, 3, 0).contiguous().to(dev)
-    flat_d = flat.to(dev)
-    flat_tc = pack_unet_tc(kind, flat_d)
-    _lib.call("mvsf_costreg_unet_forward", kind, v, flat_d, flat_tc, logits, ws, ws.numel() * 4, 8, D, H, W)
+    tc = pack_unet_tc(kind, conv.to(dev))
+    _lib.call("mvsf_costreg_unet_forward", kind, v, small.to(dev), tc, logits, ws, ws.numel() * 4, 8, D, H, W)
     e = max_abs(logits.cpu(), want)
     rec(f"costreg_unet_pipelined_stage{stage}_{D}x{H}x{W}", abs=e, scale=float(want.abs().max()))
     assert e < 2e-4 * max(1.0, float(want.abs().max()))

@@ -292,7 +292,7 @@ def test_conv3d_tensor_core_layer(dev, mode, sd, cin, cout, ID, IH, IW, skip):
 
 
 @pytest.mark.parametrize("stage,D,H,W", [(1, 16, 16, 24), (1, 8, 8, 40), (2, 8, 16, 24), (3, 4, 24, 40), (3, 3, 8, 8)])
-def test_costreg_unet(dev, stage, D, H, W):
+def test_costreg_unet_two_part(dev, stage, D, H, W):
     from mvsformerplusplus_b200 import packing
     from oracle import hotpath as O
     sd = _rand_vis_sd(13)
@@ -300,14 +300,13 @@ def test_costreg_unet(dev, stage, D, H, W):
     vol = torch.randn(1, 8, D, H, W, generator=g) * 0.5
     p = f"fusions.{stage}.cost_reg."
     want = O.costreg_unet(vol, sd, p)[0, 0]
-    kind, flat = packing.pack_costreg_unet(sd, p)
+    kind, conv, small = packing.pack_costreg_unet(sd, p)
     ws = _lib.workspace("mvsf_costreg_unet_workspace_bytes", kind, 8, D, H, W, device=dev)
     logits = torch.empty(D, H, W, device=dev)
     v = vol[0].permute(1, 2, 3, 0).contiguous().to(dev)
     from mvsformerplusplus_b200.hotpath import pack_unet_tc
-    flat_d = flat.to(dev)
-    flat_tc = pack_unet_tc(kind, flat_d)
-    _lib.call("mvsf_costreg_unet_forward", kind, v, flat_d, flat_tc, logits, ws, ws.numel() * 4, 8, D, H, W)
+    tc = pack_unet_tc(kind, conv.to(dev))
+    _lib.call("mvsf_costreg_unet_forward", kind, v, small.to(dev), tc, logits, ws, ws.numel() * 4, 8, D, H, W)
     e = max_abs(logits.cpu(), want)
     rec(f"costreg_unet_stage{stage}_{D}x{H}x{W}", abs=e, scale=float(want.abs().max()))
     assert e < 2e-4 * max(1.0, float(want.abs().max()))
@@ -324,12 +323,12 @@ COSTREG_TR_SHAPES = [(8, 12, 16), (32, 16, 16), (4, 8, 8), (8, 48, 68), (16, 64,
 
 
 @pytest.mark.parametrize("D,H,W", COSTREG_TR_SHAPES)
-def test_costreg_transformer(dev, D, H, W):
+def test_costreg_transformer_two_part(dev, D, H, W):
     _check_costreg_transformer(dev, D, H, W, with_pos=True)
 
 
 @pytest.mark.parametrize("D,H,W", COSTREG_TR_SHAPES)
-def test_costreg_transformer_without_position(dev, D, H, W):
+def test_costreg_transformer_two_part_without_position(dev, D, H, W):
     _check_costreg_transformer(dev, D, H, W, with_pos=False)
 
 
@@ -348,7 +347,7 @@ def _check_costreg_transformer(dev, D, H, W, with_pos):
     with torch.no_grad():
         want = O.costreg_transformer(vol.double(), pos.double() if with_pos else None, O.state_dict_to(sd, torch.float64),
                                      p, cfg)[0, 0]
-    flat = packing.pack_costreg_tr(sd, p, cfg["layer_num"]).to(dev)
+    gemm, small = packing.pack_costreg_tr(sd, p, cfg["layer_num"])
     ws = _lib.workspace("mvsf_costreg_tr_workspace_bytes", 8, D, H, W, device=dev)
     logits = torch.empty(D, H, W, device=dev)
     v = vol[0].permute(1, 2, 3, 0).contiguous().to(dev)
@@ -356,9 +355,9 @@ def _check_costreg_transformer(dev, D, H, W, with_pos):
     scale = 16 ** -0.5 * math.log(n_tok, cfg["train_avg_length"])
     pos_d = pos[0].contiguous().to(dev) if with_pos else None
     from mvsformerplusplus_b200.hotpath import split_weights_f16
-    flat16 = split_weights_f16(flat)
-    _lib.call("mvsf_costreg_tr_forward", v, pos_d, flat, flat16, flat.numel(), logits, ws, ws.numel() * 4, 8, D, H, W,
-              cfg["layer_num"], float(scale))
+    tc = split_weights_f16(gemm.to(dev))
+    _lib.call("mvsf_costreg_tr_forward", v, pos_d, small.to(dev), tc, gemm.numel(), logits, ws, ws.numel() * 4, 8, D, H,
+              W, cfg["layer_num"], float(scale))
     e = max_abs(logits.cpu(), want)
     lim = COSTREG_TR_TOL * max(1.0, float(want.abs().max()))
     rec(f"costreg_tr_{D}x{H}x{W}" + ("" if with_pos else "_nopos"), abs=e, scale=float(want.abs().max()), tokens=n_tok)

@@ -82,6 +82,19 @@ def test_bad_arguments_are_rejected_without_touching_the_gpu(lib):
         assert epi_call(**kw) == -1, kw
         assert msg in lib.mvsf_last_error(), (kw, lib.mvsf_last_error())
     assert epi_call(BIAS, N=192, ws_bytes=1024) == -3 and b"workspace" in lib.mvsf_last_error()
+
+    # n_wts locates the lo half of the fp16 GEMM weights: anything but the float count of the GEMM part is refused
+    def fmt_call(n_wts, ws_bytes):
+        return lib.mvsf_fmt_forward(*[ptr] * 7, n_wts, *[ptr] * 5, ws_bytes, 3, 8, 8, None)
+
+    for n in (packing.FMT_GEMM_WTS + 8, packing.FMT_GEMM_WTS + packing.FMT_SMALL_WTS):
+        assert fmt_call(n, 1 << 40) == -1 and b"bad fp16 weight blob" in lib.mvsf_last_error()
+    assert fmt_call(packing.FMT_GEMM_WTS, 1024) == -3 and b"workspace" in lib.mvsf_last_error()
+    for layers in (6, 2):
+        gemm, small = packing.costreg_tr_wts(layers)
+        for n in (gemm - 8, gemm + small, packing.costreg_tr_wts(layers + 1)[0]):
+            rc = lib.mvsf_costreg_tr_forward(ptr, None, ptr, ptr, n, ptr, ptr, 1 << 40, 8, 4, 8, 8, layers, 0.25, None)
+            assert rc == -1 and b"not the" in lib.mvsf_last_error()
     assert lib.mvsf_launch_count(0) == 0
 
 
@@ -117,15 +130,15 @@ def test_config_schema_and_reference_errors():
         validate_args(bad)
 
 
-def test_packing_layout_sizes_and_bn_folding():
+def test_two_part_packing_layout_sizes_and_bn_folding():
     m = build_hotpath_params(default_args()).eval()
     sd = synth.randomize_state_dict(m, seed=4)
     assert packing.pack_vis(sd, "fusions.0.vis.").numel() == 3652
-    k0, f0 = packing.pack_costreg_unet(sd, "fusions.1.cost_reg.")
-    k1, f1 = packing.pack_costreg_unet(sd, "fusions.3.cost_reg.")
-    assert (k0, k1) == (0, 1) and f0.numel() == 290800 and f1.numel() == 290596
-    assert packing.pack_costreg_tr(sd, "fusions.0.cost_reg.", 6).numel() == 332960
-    assert packing.pack_fmt(sd).numel() == 214464
+    k0, c0, s0 = packing.pack_costreg_unet(sd, "fusions.1.cost_reg.")
+    k1, c1, s1 = packing.pack_costreg_unet(sd, "fusions.3.cost_reg.")
+    assert (k0, k1) == (0, 1) and c0.numel() == c1.numel() == 290304 and (s0.numel(), s1.numel()) == (496, 292)
+    assert [t.numel() for t in packing.pack_costreg_tr(sd, "fusions.0.cost_reg.", 6)] == [327680, 5280]
+    assert [t.numel() for t in packing.pack_fmt(sd)] == [196608, 17856]
     # folded conv+bias reproduces conv -> BatchNorm(eval)
     x = torch.randn(1, 1, 9, 9)
     w = sd["fusions.0.vis.0.conv.weight"]

@@ -124,15 +124,14 @@ def main():
     total_ms = 0.0
     for stage, fi, D, div in STAGES:
         H, W = H0 // div, W0 // div
-        kind, flat = packing.pack_costreg_unet(sd, f"fusions.{fi}.cost_reg.")
-        flat_d = flat.to(dev)
-        flat_tc = pack_unet_tc(kind, flat_d)
+        kind, conv, small = packing.pack_costreg_unet(sd, f"fusions.{fi}.cost_reg.")
+        small_d, tc = small.to(dev), pack_unet_tc(kind, conv.to(dev))
         ws = _lib.workspace("mvsf_costreg_unet_workspace_bytes", kind, 8, D, H, W, device=dev)
         vol = (torch.randn(D, H, W, 8, generator=torch.Generator().manual_seed(stage)) * 0.5).to(dev)
         logits = torch.empty(D, H, W, device=dev)
 
         def fwd():
-            _lib.call("mvsf_costreg_unet_forward", kind, vol, flat_d, flat_tc, logits, ws, ws.numel() * 4, 8, D, H, W)
+            _lib.call("mvsf_costreg_unet_forward", kind, vol, small_d, tc, logits, ws, ws.numel() * 4, 8, D, H, W)
 
         for _ in range(a.warmup):
             fwd()
@@ -189,7 +188,7 @@ def main():
         res["unets"].append({"stage": stage, "kind": ("CostRegNet", "CostRegNet3D")[kind], "D": D, "H": H, "W": W,
                              "ms_median": round(med, 4), "ms_min": round(ms[0], 4), "ms_max": round(ms[-1], 4),
                              "profiled_forwards": len(fwds), "launches": layers})
-        del ws, vol, logits, flat_tc
+        del ws, vol, logits, small_d, tc
         torch.cuda.empty_cache()
     res["ms_total_median"] = round(total_ms, 4)
 
