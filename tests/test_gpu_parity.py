@@ -12,6 +12,7 @@ import torch
 import torch.nn.functional as F
 
 from mvsformerplusplus_b200 import _lib
+from tests import cost_volume_common as R
 from tests.common import ROOT, TMP, build_case, load_golden, max_abs, rec, rel_linf
 
 pytestmark = pytest.mark.gpu
@@ -136,27 +137,38 @@ COST_CASES = [  # C, D, H, W, V, theta_step, depth jitter
     (8, 4, 31, 45, 3, 0.6, 0.02),   # wide baseline: many taps leave the image (zero padding per corner)
     (8, 48, 10, 14, 3, 0.1, 0.02),  # generic-D path (D-sweep configuration)
     (64, 8, 9, 11, 2, 0.1, 0.02),
+    (32, 16, 20, 28, 4, 0.6, 0.3), (64, 32, 14, 18, 4, 0.6, 0.3),   # wide baseline and depth jitter at the coarse stages
     # shapes served by the TMA-staged window kernels (C = 8 / 16, even H): several tiles, ragged right / bottom edges,
     # taps leaving the image, depth outliers that leave the staged window (global fallback), D = 4 / 8 / chunked D
     (8, 4, 64, 96, 3, 0.1, 0.02), (8, 4, 30, 44, 5, 0.6, 0.02), (8, 4, 48, 80, 3, 0.15, 0.4), (8, 8, 16, 40, 3, 0.1, 0.02),
     (8, 7, 18, 34, 2, 0.1, 0.02), (16, 8, 32, 48, 4, 0.1, 0.02), (16, 8, 28, 68, 3, 0.5, 0.3), (16, 4, 12, 20, 3, 0.1, 0.02),
     (16, 24, 10, 36, 3, 0.1, 0.02), (8, 96, 12, 20, 3, 0.1, 0.0),
+    # grazing geometry (cost_volume_common.grazing_projections): taps behind a source camera land in the image, taps on
+    # its principal plane go to +-Inf / NaN
+    (8, 4, 36, 52, 3, "grazing", 0.0), (16, 8, 36, 52, 3, "grazing", 0.0),
 ]
 
 
 @pytest.mark.parametrize("C,D,H,W,V,th,jit", COST_CASES)
 def test_cost_volume_kernels(dev, C, D, H, W, V, th, jit):
-    """Pass A (entropy), vis CNN, pass B (aggregation) against the oracle, through every organisation the library has:
-    L1 gathers with recompute, L1 gathers with the correlation spill, and (where they apply) the window kernels."""
+    """Pass A (entropy, spilled correlations), vis CNN and pass B (aggregation) of every organisation the library has
+    (L1 gathers with recompute, L1 gathers with the correlation spill and, where they apply, the window kernels and the
+    pipeline kernel, forced and chosen per call) against the fp64 reference at the library's own sample coordinates
+    (tests/cost_volume_common.py), and against each other.  The fp32 oracle's errors are recorded only: they are sized by
+    its own coordinate rounding."""
     from mvsformerplusplus_b200 import packing, synth
     from oracle import hotpath as O
     sd = _rand_vis_sd(5)
     g = torch.Generator().manual_seed(C * 1000 + D)
     feats = torch.randn(1, V, C, H, W, generator=g)
-    sc = {8: 1, 16: 2, 32: 4, 64: 8}[C]
-    pm = synth.make_proj_matrices(V, H * sc, W * sc, theta_step=th)[f"stage{ {1: 4, 2: 3, 4: 2, 8: 1}[sc] }"]
-    dv = synth.make_depth_values(192)
-    dvals = O.init_inverse_range(dv, D, H, W) * (1.0 + jit * torch.rand(1, D, H, W, generator=g))
+    if th == "grazing":
+        pm = R.grazing_projections(H, W)[None]
+        dvals = R.grazing_depth(D, H, W, seed=C + D)[None]
+    else:
+        sc = {8: 1, 16: 2, 32: 4, 64: 8}[C]
+        pm = synth.make_proj_matrices(V, H * sc, W * sc, theta_step=th)[f"stage{ {1: 4, 2: 3, 4: 2, 8: 1}[sc] }"]
+        dv = synth.make_depth_values(192)
+        dvals = O.init_inverse_range(dv, D, H, W) * (1.0 + jit * torch.rand(1, D, H, W, generator=g))
     want = O.cost_volume(feats, pm, dvals, sd, "fusions.3.", 8)
     homs = torch.empty((V - 1) * 12, device=dev)
     kinv = torch.empty(9, device=dev)
@@ -166,6 +178,30 @@ def test_cost_volume_kernels(dev, C, D, H, W, V, th, jit):
     dd = dvals[0].contiguous().to(dev)
     wts = packing.pack_vis(sd, "fusions.3.vis.").to(dev)
     vol_scale = max(1.0, float(want["volume_mean"].abs().max()))
+
+    # fp64 reference at the library's coordinates
+    ref = R.CostVolumeRef(f, homs.view(V - 1, 12), dd)
+    corr64, ent64 = ref.pass_a()
+    sd64 = R.state_dict_fp64(sd, dev)
+    vis64 = R.vis_fp64(ent64.view(V - 1, H, W), sd64, "fusions.3.")
+    corr_scale = max(1.0, float(corr64.abs().max()))
+    if th == "grazing":   # both kinds of tap the geometry is there for
+        finite = torch.isfinite(ref.ix) & torch.isfinite(ref.iy)
+        behind_in_image = R.in_bounds(ref.ix, ref.iy, H, W) & (ref.Z <= 0)
+        assert bool((~finite).any()) and bool(behind_in_image.any())
+    e64 = {}
+
+    def check64(tag, ent_k, vis_k, vol_k, corr_k=None):
+        """one organisation's outputs against the reference; pass B fed the organisation's own vis"""
+        vis_k = vis_k.reshape(V - 1, H * W)
+        own = R.vis_fp64(ent_k, sd64, "fusions.3.").reshape(V - 1, H * W)
+        vol64 = R.aggregate(corr64, vis_k)
+        e = {f"{tag}_entropy64": max_abs(ent_k.reshape(V - 1, -1), ent64),
+             f"{tag}_vis64": max_abs(vis_k, own), f"{tag}_vis64_chain": max_abs(vis_k, vis64.reshape(V - 1, -1)),
+             f"{tag}_volume64": max_abs(vol_k.reshape(D, H * W, 8), vol64) / max(1.0, float(vol64.abs().max()))}
+        if corr_k is not None:
+            e[f"{tag}_corr64"] = max_abs(corr_k.reshape(V - 1, D, H * W, 8), corr64) / corr_scale
+        e64.update(e)
 
     def run_two_gathers():
         ent = torch.empty(V - 1, H, W, device=dev)
@@ -187,6 +223,8 @@ def test_cost_volume_kernels(dev, C, D, H, W, V, th, jit):
         _lib.call("mvsf_corr_aggregate", corr, vis, vol_s, V, 8, D, H, W)
     finally:
         _lib.call("mvsf_warp_corr_set_tile_path", 1)
+    check64("l1", ent, vis, vol)
+    check64("l1_spill", ent_s, vis, vol_s, corr)
     assert torch.equal(ent_s, ent)
     e_paths = max_abs(vol_s.cpu(), vol.cpu())
     assert e_paths <= 2e-6 * vol_scale, e_paths   # identical up to the pair sum of 8-channel groups
@@ -196,6 +234,7 @@ def test_cost_volume_kernels(dev, C, D, H, W, V, th, jit):
     e_tile = {}
     if tiled:   # window kernels: the two-gather plan ...
         ent_t, vis_t, vol_t = run_two_gathers()
+        check64("tile", ent_t, vis_t, vol_t)
         e_tile = dict(tile_vs_l1_entropy=max_abs(ent_t.cpu(), ent.cpu()), tile_vs_l1_volume=max_abs(vol_t.cpu(), vol_s.cpu()))
         assert e_tile["tile_vs_l1_entropy"] < 2e-5 and e_tile["tile_vs_l1_volume"] < 1e-5 * vol_scale, e_tile
         # ... and the spill plan: forced through the persistent TMA pipeline kernel where it exists (C = 8, D = 4; mode 2,
@@ -214,6 +253,7 @@ def test_cost_volume_kernels(dev, C, D, H, W, V, th, jit):
             _lib.call("mvsf_vis_cnn", ent_p, wts, vis_p, V - 1, H, W)
             _lib.call("mvsf_corr_aggregate", corr_p, vis_p, vol_p, V, 8, D, H, W)
             tag = "pipe" if mode == 2 else "adaptive"
+            check64(tag, ent_p, vis_p, vol_p, corr_p)
             e_tile.update({f"{tag}_vs_l1_entropy": max_abs(ent_p.cpu(), ent.cpu()), f"{tag}_vs_l1_corr": max_abs(corr_p.cpu(), corr.cpu()),
                            f"{tag}_vs_l1_volume": max_abs(vol_p.cpu(), vol_s.cpu())})
             assert bool(torch.isfinite(corr_p).all())
@@ -229,30 +269,34 @@ def test_cost_volume_kernels(dev, C, D, H, W, V, th, jit):
     e_ent = max_abs(ent.cpu(), want["entropy"][0])
     e_vis = max_abs(vis.cpu(), want["vis_weight"][0])
     e_vol = max_abs(vol.cpu().permute(3, 0, 1, 2), want["volume_mean"][0])
-    # vis CNN in isolation on the oracle's entropy (removes the entropy noise from the comparison)
+    # vis CNN in isolation on the oracle's entropy
     vis2 = torch.empty(V - 1, H, W, device=dev)
     ent_o = want["entropy"][0].contiguous().to(dev)
     _lib.call("mvsf_vis_cnn", ent_o, wts, vis2, V - 1, H, W)
     e_vis2 = max_abs(vis2.cpu(), want["vis_weight"][0])
     rec(f"cost_volume_C{C}_D{D}_{H}x{W}_V{V}_th{th}_j{jit}", entropy=e_ent, vis=e_vis, vis_isolated=e_vis2, volume=e_vol,
-        vol_scale=float(want["volume_mean"].abs().max()), tiled=int(tiled), **e_tile)
-    assert e_ent < 5e-4 and e_vis < 5e-4 and e_vis2 < 2e-5 and e_vol < 1e-3
+        vol_scale=float(want["volume_mean"].abs().max()), corr64_scale=corr_scale, tiled=int(tiled), **e_tile, **e64)
+    for k, e in e64.items():
+        kind = k.rsplit("_", 1)[1] if not k.endswith("_chain") else "chain"
+        lim = {"entropy64": R.ENT_TOL, "vis64": R.VIS_TOL, "chain": R.VIS_CHAIN_TOL, "volume64": R.VOL_TOL, "corr64": R.CORR_TOL}[kind]
+        assert e < lim, f"{k}: {e:.3e} against fp64, limit {lim:.1e}"
 
 
 def test_vis_cnn_tile_borders(dev):
+    """the fused vis CNN (wgmma on fp16 hi|lo operands) against the vis CNN in fp64, at sizes that cut its 14 x 30 tiles"""
     from mvsformerplusplus_b200 import packing
-    from oracle import hotpath as O
     sd = _rand_vis_sd(9)
+    sd64 = R.state_dict_fp64(sd, "cpu")
     g = torch.Generator().manual_seed(3)
     for (N, H, W) in [(1, 30, 30), (2, 61, 95), (3, 7, 5), (1, 1, 1), (2, 64, 128)]:
-        ent = 3.0 * torch.rand(1, N, H, W, generator=g)
-        want = torch.cat([O.vis_cnn(ent[:, i:i + 1], sd, "fusions.1.") for i in range(N)], 1)[0]
+        ent = 3.0 * torch.rand(N, H, W, generator=g)
+        want = R.vis_fp64(ent, sd64, "fusions.1.")
         vis = torch.empty(N, H, W, device=dev)
-        ent_d, wts = ent[0].contiguous().to(dev), packing.pack_vis(sd, "fusions.1.vis.").to(dev)
+        ent_d, wts = ent.contiguous().to(dev), packing.pack_vis(sd, "fusions.1.vis.").to(dev)
         _lib.call("mvsf_vis_cnn", ent_d, wts, vis, N, H, W)
         e = max_abs(vis.cpu(), want)
         rec(f"vis_cnn_{N}x{H}x{W}", abs=e)
-        assert e < 2e-5
+        assert e < R.VIS_TOL, f"{e:.3e} against fp64"
 
 
 # ----------------------------------------------------------------------------------------------- regularisers
@@ -540,8 +584,9 @@ def test_full_size_properties(dev, hp):
 
 
 def test_identity_homography_property(dev):
-    """src camera == ref camera: the warp must return the source itself, so pass B equals the closed form
-    vol[g] = mean_{c in g} ref*src (all views weighted alike) at full DTU stage-4 size."""
+    """src camera == ref camera at full DTU stage-4 size: pass B (window kernel) against the fp64 reference at the
+    library's own coordinates, which sit within fp32 normalisation rounding of the pixel centres, so the volume is
+    vol[g] = mean_{c in g} ref * src (all views weighted alike) up to that rounding"""
     from mvsformerplusplus_b200 import synth
     H, W, C, D, V = 1152, 1536, 8, 4, 2
     pm = synth.make_proj_matrices(1, H, W)["stage4"][0]
@@ -555,10 +600,13 @@ def test_identity_homography_property(dev):
     vis = torch.full((1, H, W), 0.7, device=dev)
     vol = torch.empty(D, H, W, C, device=dev)
     _lib.call("mvsf_warp_corr_aggregate", f, homs, dd, vis, vol, V, C, 8, D, H, W)
-    want = (f[0] * f[1]) * (0.7 / (0.7 + 1e-6))
-    e = float((vol - want[None]).abs().max())
-    rec("identity_homography", abs=e)
-    assert e < 5e-3  # coordinates round-trip through fp32 normalisation (<=1e-4 px) on white-noise features
+    corr64, _ = R.CostVolumeRef(f, homs.view(1, 12), dd).view(0)
+    want = R.aggregate(corr64[None], vis.view(1, -1))
+    scale = max(1.0, float(want.abs().max()))
+    e = max_abs(vol.view(D, H * W, 8), want) / scale
+    e_closed = float((vol - (f[0] * f[1])[None] * (0.7 / (0.7 + 1e-6))).abs().max())
+    rec("identity_homography", abs64=e, scale=scale, closed_form_abs=e_closed)
+    assert e < R.VOL_TOL, f"{e:.3e} against fp64"
 
 
 # ----------------------------------------------------------------------------------------------- tensor-core attention
