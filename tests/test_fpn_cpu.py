@@ -173,3 +173,37 @@ def test_plain_install_leaves_the_fpn_untouched():
         assert torch.equal(model.encoder.state_dict()[k], v), k
     for k, v in sub_sd(sd, "decoder.").items():
         assert torch.equal(model.decoder.state_dict()[k], v), k
+
+
+def _source(name):
+    return " ".join(open(os.path.join(ROOT, "mvsformerplusplus_b200", "csrc", name)).read().split())
+
+
+def test_fpn_tile_coverage_restates_the_layer_table():
+    """tests/fpn_common.py restates the tiling of the 13 tensor-core layers; a retiling of csrc/fpn.cu or a change of
+    conv2d_tc.cuh's shared-memory layout fails here until the restatement follows it"""
+    from tests.fpn_common import FPN_TC_LAYERS, fpn_coverage
+    src = _source("fpn.cu")
+    enc = src[src.index("constexpr LayerDesc kEnc[11] = {"):]
+    enc = [tuple(int(v) for v in t.split(",")) for t in enc[enc.index("{") + 2:enc.index("}};")].split("}, {")]
+    dec = src[src.index("constexpr LayerDesc kDec[3] = {"):]
+    dec = [tuple(int(v) for v in t.split(",")) for t in dec[dec.index("{") + 2:dec.index("}};")].split("}, {")]
+    mine = [(ci, co, ks, ns) for _, ci, co, ks, _, _, ns, _, _ in FPN_TC_LAYERS]
+    assert mine == enc[1:] + [(64, co, 3, ns) for _, co, _, ns in dec]
+    assert ("using EncL = Conv<kEnc[I].ci, kEnc[I].co, kEnc[I].ks, (I == 2 || I == 5 || I == 8) ? 2 : 1, "
+            "(I >= 8) ? 8 : 16, kEnc[I].ns>;") in src
+    assert "using DecL = Conv<64, kDec[K].co, 3, 1, K == 0 ? 8 : 16, kDec[K].ns>;" in src
+    assert "constexpr int kLat[3] = {32, 16, 8};" in src
+    conv = _source("conv2d_tc.cuh")
+    for line in ("PAD = (KS - 1) / 2, HALO = (KS - 1) / S;", "PR = TR + HALO, PC = 32 + HALO;",
+                 "NO = CI / 8, NP = S * S, NG = CI < 16 ? 1 : CI / 16, NB = CO / NS;",
+                 "PLANE = PR * PC * 16, PITCH = PC * 16;", "BT = 64 * NS;", "WBYTES = KS * KS * NG * BT;",
+                 "OFF_W = NP * NO * 2 * PLANE, SMEM = OFF_W + WBYTES;",
+                 "long long cap = (long long)per_sm * device_sm_count(dev) / L::NB;"):
+        assert line in conv, line
+    assert "IR = L::PR + 6, IC = L::PC + 6, NW = 49 * 3 * 8 + 8;" in src and "EXTRA = (3 * IR * IC + NW) * 4;" in src
+    assert "EXTRA = (CL * 64 + 64) * 4;" in src
+    # an H100 SXM (132 SMs, 228 KB of shared memory per SM): 14 x 264 x 456 loops and is ragged in every layer
+    cov = fpn_coverage(14, 264, 456, 132, 228 * 1024)
+    assert all(t > b and rx and ry for t, b, rx, ry in cov.values()), cov
+    assert cov["downsample2"][:2] == (280, 132) and cov["conv20"][:2] == (280, 264) and cov["conv30"][:2] == (140, 66)

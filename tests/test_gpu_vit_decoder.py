@@ -1,7 +1,20 @@
 """GPU tests of the ViT feature decoder (csrc/vit_decoder.cu through hotpath.CrossVITDecoder) and of the streamed-weight
 GEMM it runs on (csrc/linear_tc.cu, mvsf_linear_tc_streamed_epilogue) against fp64 references, the reference-executed
-fixtures, the fp32 restatement at full size, and through install() with the reference's glue.
-Bar: every output within 1e-4 * max(1, max|ref|); errors go to rec()."""
+fixtures, and through install() with the reference's glue.  Errors go to rec().
+
+Bars, relative to max(1, max|fp64|), from the worst errors measured on an H100 SXM (132 SMs, 700 W power limit) and the
+value mutations of the kernels (dropping the a_lo x w_hi product, every CTA's second tile, the last image column of
+the convolutions' taps, or the lo half of the proj GEMMs' input):
+  * streamed GEMM: gemm_bar(K) = 2e-6 + 5e-9 K.  The tensor core's fp32 accumulation truncates, a biased error that
+    grows with the chain: measured 1.4e-6 .. 1.8e-6 at K <= 1024, 6.5e-6 at 3072, 1.45e-5 at 6912 (about 2.1e-9 K,
+    GEMM_WORST_MEASURED), so the bar is 2.5 .. 3.4x the worst at each K.  A dropped lo product costs 1.6e-4 .. 2.2e-4
+    at every K, 4x the bar or more.
+  * decoder: DECODER_BAR.  Its error, 1.6e-5 .. 3.0e-5 (DECODER_WORST_MEASURED), is ten times the fp32 torch
+    restatement's own (1.4e-6 .. 2.7e-6 at 1x3x4x6, 2x3x9x11 and the harsh case), about what the GEMM measures at the
+    head convolution's K = 6912.  Losing the lo half of every proj input adds about as much (4.1e-5 .. 6.5e-5; 1.7e-4
+    in the harsh case), so the bar sits at 1.7x the worst measured rather than 3x: the harsh case fails it 3x over.  A
+    skipped tile or a lost image column costs 0.4 or more.
+The reference-executed fixtures measure parity with the fp32 reference, not the kernels' arithmetic, and keep 1e-4."""
 
 import pytest
 import torch
@@ -12,10 +25,23 @@ from oracle import vit_decoder as OV
 from tests.common import load_golden, max_abs, rec
 from tests.fpn_common import fpn_state_dict
 from tests.vit_decoder_common import (CASES, OracleFPNDecoder, OracleFPNEncoder, OracleViTDecoder, cuda_decoder,
-                                      make_tokens, shipped_args, vit_state_dict)
+                                      decoder_gemm_tiles, make_tokens, shipped_args, vit_state_dict)
 
 pytestmark = pytest.mark.gpu
 BIAS, GELU, ELU1, RES, SILU = 0, 1, 2, 3, 6
+GEMM_WORST_MEASURED = {512: 1.4e-6, 768: 1.8e-6, 1024: 1.7e-6, 3072: 6.5e-6, 6912: 1.45e-5}
+DECODER_BAR = 5e-5
+DECODER_WORST_MEASURED = dict(harsh=3.0e-5, other=2.3e-5)   # 1x3x8x8 harsh; 10 x 34 x 60, bf16 inputs
+# (B, V, h, w, harsh) of the fp64 cases.  V = 10 at 34 x 60 and V = 5 at 36 x 48 are the shipped sizes (1152 x 1536 and
+# 1088 x 1920 images through the ViT's 14-pixel patches at 0.5 scale): there the head convolution, each transposed-conv
+# parity class and the source-view token linears run more tiles than the grid has CTAs, and the rows V h w are not a
+# multiple of 128, so tiles straddle images (test_vit_decoder_fp64_cases_loop_every_gemm)
+DECODER_FP64_CASES = [(1, 3, 4, 6, False), (1, 2, 5, 7, False), (2, 2, 3, 5, False), (1, 5, 12, 16, False),
+                      (2, 3, 9, 11, False), (1, 3, 8, 8, True), (1, 10, 34, 60, False), (1, 5, 36, 48, False)]
+
+
+def gemm_bar(K):
+    return 2e-6 + 5e-9 * K
 
 
 @pytest.fixture(scope="module")
@@ -68,23 +94,37 @@ def test_streamed_gemm_vs_fp64(dev, epi, M, N, K, elu_cols, c2):
         assert bool(torch.isnan(C2[:, 2 * N:]).all())
         e["C2"] = float((hi.double() + lo.double() - t).abs().max()) / scale
     rec(f"streamed_gemm_epi{epi}_{M}x{N}x{K}", **e)
-    assert max(e.values()) < 1e-4, e
+    assert max(e.values()) < gemm_bar(K), e
 
 
 def _run(dec, x, B, V, h, w):
     return dec(x, vit_shape=(B, V, h, w, 768))
 
 
-@pytest.mark.parametrize("B,V,h,w,harsh", [(1, 3, 4, 6, False), (1, 2, 5, 7, False), (2, 2, 3, 5, False),
-                                           (1, 5, 12, 16, False), (2, 3, 9, 11, False), (1, 3, 8, 8, True)])
+def test_vit_decoder_fp64_cases_loop_every_gemm(dev):
+    """on this device, some fp64 case runs more tiles than CTAs (one CTA per SM) in the head convolution, in every
+    parity class of both transposed convolutions and in each token linear of the source views"""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    most = {}
+    for B, V, h, w, _ in DECODER_FP64_CASES:
+        for k, t in decoder_gemm_tiles(B, V, h, w).items():
+            most[k] = max(most.get(k, 0), t)
+    short = {k: t for k, t in most.items() if t <= sms}
+    assert not short, (sms, short)
+
+
+@pytest.mark.parametrize("B,V,h,w,harsh", DECODER_FP64_CASES)
 def test_vit_decoder_vs_fp64_oracle(dev, B, V, h, w, harsh):
     sd = vit_state_dict(31)
-    x = make_tokens(dict(B=B, V=V, h=h, w=w, xseed=B * 100 + V * 10 + h + w, harsh=harsh))
-    got = _run(cuda_decoder(sd, dev), [t.to(dev) for t in x], B, V, h, w)
-    want = OV.vit_decoder([t.to(dev).double() for t in x], sd, (B, V, h, w, 768))
+    x = [t.to(dev) for t in make_tokens(dict(B=B, V=V, h=h, w=w, xseed=B * 100 + V * 10 + h + w, harsh=harsh))]
+    got = _run(cuda_decoder(sd, dev), x, B, V, h, w)
+    assert got.shape == (B * V, 64, 4 * h, 4 * w) and got.permute(0, 2, 3, 1).is_contiguous()
+    with torch.no_grad():
+        want = OV.vit_decoder([t.double() for t in x], sd, (B, V, h, w, 768))
     e = float((got.double() - want).abs().max()) / max(1.0, float(want.abs().max()))
+    e = e if bool(torch.isfinite(got).all()) else float("inf")
     rec(f"vit_decoder_fp64_{B}x{V}x{h}x{w}{'_harsh' if harsh else ''}", rel=e, max_ref=float(want.abs().max()))
-    assert e < 1e-4
+    assert e < DECODER_BAR, e
 
 
 @pytest.mark.parametrize("name", sorted(CASES))
@@ -96,26 +136,6 @@ def test_vit_decoder_vs_reference_fixture(dev, name):
     want = gold["out"]
     e = max_abs(got, want) / max(1.0, float(want.abs().max()))
     rec(f"vit_decoder_fixture_{name}", rel=e)
-    assert e < 1e-4
-
-
-@pytest.mark.parametrize("V,h,w", [(5, 36, 48), (10, 34, 60)])
-def test_vit_decoder_full_size_vs_fp32_torch(dev, V, h, w):
-    sd = vit_state_dict(32)
-    sd_dev = {k: v.to(dev) for k, v in sd.items()}
-    g = torch.Generator(device=dev).manual_seed(V)
-    x = [torch.randn(1, V, h * w, 768, device=dev, generator=g) for _ in range(3)]
-    got = _run(cuda_decoder(sd, dev), x, 1, V, h, w)
-    tf32 = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
-    try:
-        with torch.no_grad():
-            want = OV.vit_decoder(x, sd_dev, (1, V, h, w, 768))
-    finally:
-        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = tf32
-    e = float((got - want).abs().max()) / max(1.0, float(want.abs().max()))
-    rec(f"vit_decoder_fullsize_{V}x{h}x{w}", rel=e, max_ref=float(want.abs().max()))
-    assert got.shape == (V, 64, 4 * h, 4 * w) and got.permute(0, 2, 3, 1).is_contiguous()
     assert e < 1e-4
 
 
@@ -134,7 +154,7 @@ def test_vit_decoder_bf16_and_strided_inputs(dev):
         want = OV.vit_decoder([t.double() for t in x], sd, (B, V, h, w, 768))
         e[tag] = float((got.double() - want).abs().max()) / max(1.0, float(want.abs().max()))
     rec("vit_decoder_input_dtypes_strides", **e)
-    assert max(e.values()) < 1e-4, e
+    assert max(e.values()) < DECODER_BAR, e
 
 
 def test_install_vit_decoder_and_fpn_under_bf16_autocast(dev):

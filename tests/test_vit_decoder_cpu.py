@@ -193,3 +193,21 @@ def test_install_vit_decoder_keeps_the_checkpoint_contract():
     model.load_state_dict(before, strict=True)
     with pytest.raises(RuntimeError, match="no CPU fallback"):
         model.decoder_vit([torch.zeros(1, 2, 4, 768)] * 3, vit_shape=(1, 2, 2, 2, 768))
+
+
+def test_decoder_gemm_tiles_restate_the_streamed_launch():
+    """tests/vit_decoder_common.decoder_gemm_tiles restates how the streamed GEMM tiles the decoder's products; a change
+    of the tile shape, the grid or the head's GEMM shapes fails here until the restatement follows it"""
+    from tests.vit_decoder_common import decoder_gemm_tiles
+    src = lambda n: " ".join(open(os.path.join(ROOT, "mvsformerplusplus_b200", "csrc", n)).read().split())
+    lin, dec = src("linear_tc.cu"), src("vit_decoder.cu")
+    assert "const int ntiles = cdiv(a.M, TC_BM) * (a.N / BN), num_sms = device_sm_count(dev);" in lin
+    assert "<<<ntiles < num_sms ? ntiles : num_sms, TC_THREADS, smem, s>>>(a);" in lin
+    assert "return a.N % 128 == 0 ? launch_tcs_bn<128>(a, epi, s) : launch_tcs_bn<64>(a, epi, s);" in lin
+    for shape in ("a.M = imgs * L; a.N = 256; a.K = 9 * D;", "a.M = imgs * L; a.N = 128; a.K = 1024;",
+                  "a.M = imgs * 4 * L; a.N = 64; a.K = 512;", "TcsArgs a = gemm(ws, ws.xn2, 2 * D, D, wb + G_QKV, D, M);",
+                  "TcsArgs f1 = gemm(ws, ws.xn2, 2 * D, D, wb + G_FC1, HID, M);"):
+        assert shape in dec, shape
+    # V = 10 views of 34 x 60 tokens on an H100 SXM's 132 SMs: upsampler0 is the GEMM with the fewest tiles
+    t = decoder_gemm_tiles(1, 10, 34, 60)
+    assert min(t.values()) == t["upsampler0_class0"] == 160 and t["head_conv"] == 320

@@ -41,6 +41,25 @@ def sub_sd(sd, prefix):
     return {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
 
 
+def tcs_tiles(M, N):
+    """tiles of one streamed-weight GEMM: 128-row M tiles x N tiles of 128 columns (64 when N % 128 != 0), walked by
+    min(tiles, SMs) persistent CTAs (csrc/linear_tc.cu:749-750, :796)"""
+    return -(-M // 128) * (N // (128 if N % 128 == 0 else 64))
+
+
+def decoder_gemm_tiles(B, V, h, w):
+    """tiles of the streamed GEMMs of one ViT-decoder forward (csrc/vit_decoder.cu:236-266 head, :95-116 token linears
+    of the source-view batch, M = (V - 1) h w tokens)"""
+    L, D = h * w, 768
+    t = {"head_conv": tcs_tiles(B * V * L, 256)}
+    for cls in range(4):
+        t[f"upsampler0_class{cls}"] = tcs_tiles(B * V * L, 128)
+        t[f"upsampler1_class{cls}"] = tcs_tiles(B * V * 4 * L, 64)
+    for name, n in (("q", D), ("proj", D), ("fc1", 4 * D), ("fc2", D)):
+        t[f"source_{name}"] = tcs_tiles((V - 1) * L, n)
+    return t
+
+
 def cuda_decoder(sd, dev):
     from mvsformerplusplus_b200.hotpath import CrossVITDecoder
     m = CrossVITDecoder(shipped_args())
