@@ -319,6 +319,31 @@ int mvsf_fusion_extract(const unsigned char* mask, const float* depth_avg, const
                         const float* cam_inv, const float* image, float* xyz, unsigned char* rgb, long long capacity, int H,
                         int W, mvsf_stream_t stream);
 
+/* ---- gipuma fusion: probability_filter (misc/gipuma.py:160-177) and fusibile's cross-view voting and point averaging
+ *      at normal_thresh = 360 (test.py's default filter_method).  Reference views are stepped one at a time, in index
+ *      order: mvsf_fusion_gipuma_vote then mvsf_fusion_gipuma_emit per view, with one used-mark map for the scene.
+ * depth [N][H][W] (filtered), used [N][H][W] u8 (zero before view 0), cam_table [N][32] fp32; the workspace is that of
+ * mvsf_fusion_workspace_bytes.  N is bounded only by memory: the table is read from global memory with 64-bit offsets.
+ * Bad arguments (null pointer, H W outside [1, 2^31), ref outside [0, N), num_consistent < 0): -1; short workspace: -3;
+ * nothing launched. */
+/* depth = depths where conf > prob_threshold and depth_min <= depths <= depth_max, else 0; cam_table per view: P = K E[:3]
+ * (12, row-major), M^-1 of M = P[:, :3] (9, row-major), f b (f = K[0][0] / K[2][2], b = 0.54), padding; fp64 rounded once. */
+int mvsf_fusion_gipuma_prepare(const float* depths, const float* confs, const float* cams, int N, int H, int W,
+                               float prob_threshold, float depth_min, float depth_max, float* depth, float* cam_table,
+                               mvsf_stream_t stream);
+/* Reference view ref: a valid, unused pixel survives when at least num_consistent other views are consistent with it
+ * (the pixel's world point lands on a valid source pixel within disp_threshold in disparity).  -> mask u8 [H][W] and the
+ * workspace's scanned survivor counts, the view's survivor count in its last int. */
+int mvsf_fusion_gipuma_vote(const float* depth, const unsigned char* used, const float* cam_table, int N, int ref, int H, int W,
+                            float disp_threshold, int num_consistent, unsigned char* mask, void* workspace,
+                            size_t workspace_bytes, mvsf_stream_t stream);
+/* The survivors of the vote, in row-major pixel order: xyz [capacity][3] the mean of the pixel's world point and those of
+ * its consistent source pixels, rgb [capacity][3] the integer mean of round(255 image) over the same pixels (images
+ * [N][3][H][W] fp32 in [0, 1]); each consistent source pixel is marked used.  Survivors beyond capacity write no point. */
+int mvsf_fusion_gipuma_emit(const float* depth, const float* cam_table, const float* images, int N, int ref, int H, int W,
+                            float disp_threshold, const unsigned char* mask, const void* workspace, size_t workspace_bytes,
+                            unsigned char* used, float* xyz, unsigned char* rgb, long long capacity, mvsf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

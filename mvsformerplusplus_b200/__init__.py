@@ -4,7 +4,8 @@ from .config import default_args, load_args, validate_args  # noqa: F401
 
 __all__ = ["default_args", "load_args", "validate_args", "StageNet", "FMT_with_pathway", "HotPathNet", "install",
            "cascade_forward", "homo_warping_3D_with_mask", "FPNEncoder", "FPNDecoder", "CrossVITDecoder",
-           "DinoVisionTransformer", "vit_base", "DINOv2MVSNet", "filter_view", "fuse_scene", "write_ply", "read_pair_file"]
+           "DinoVisionTransformer", "vit_base", "DINOv2MVSNet", "filter_view", "fuse_scene", "fuse_scene_gipuma", "write_ply",
+           "read_pair_file"]
 
 
 def __getattr__(name):  # hotpath imports torch + ctypes; keep `import mvsformerplusplus_b200` light
@@ -13,7 +14,7 @@ def __getattr__(name):  # hotpath imports torch + ctypes; keep `import mvsformer
                 "CrossVITDecoder", "DinoVisionTransformer", "vit_base", "DINOv2MVSNet"):
         from . import hotpath
         return getattr(hotpath, name)
-    if name in ("filter_view", "fuse_scene", "write_ply", "read_pair_file"):
+    if name in ("filter_view", "fuse_scene", "fuse_scene_gipuma", "write_ply", "read_pair_file"):
         from . import fusion
         return getattr(fusion, name)
     raise AttributeError(name)

@@ -316,6 +316,164 @@ fusion_extract_kernel(const unsigned char* __restrict__ mask, const float* __res
 
 static size_t fusion_ws_bytes(int H, int W) { return ((size_t)cdiv((long long)H * W, FUSION_BLOCK) + 1) * sizeof(int); }
 
+// ------------------------------------------------------------------------------------------------
+// gipuma: the cross-view voting and point averaging of fusibile, the fusion misc/gipuma.py:208-228 runs as an external
+// binary (probability_filter, P = [K|0] E, fusibile at normal_thresh = 360 with constant normals, which makes the
+// normal test vacuous).  Reference views are processed one at a time in index order; a view's step reads only its own
+// used marks and sets only other views' marks, so every step is race-free and deterministic.
+//
+// Camera table: GIPUMA_CAM floats per view (128 bytes, 64-bit offsets, read through the L1 from global memory, so the
+// number of views is bounded only by int N and memory): [0, 12) P = K E[:3, :] row-major, [12, 21) M^-1 (M = P[:, :3])
+// row-major, [21] f b with f = K[0][0] / K[2][2] and b = 0.54; all computed in fp64 and rounded once.
+// ------------------------------------------------------------------------------------------------
+constexpr int GIPUMA_CAM = 32;
+constexpr double GIPUMA_BASELINE = 0.54;   // fusibile's fixed baseline
+
+__global__ void gipuma_cameras_kernel(const float* __restrict__ cams, int N, float* __restrict__ table) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  const float* E = cams + (size_t)n * 32;
+  const float* K = E + 16;
+  float* t = table + (size_t)n * GIPUMA_CAM;
+  const double nanv = __longlong_as_double(0x7ff8000000000000LL);
+  double P[12], A[16], B[16];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 4; ++c)
+      P[r * 4 + c] = __dadd_rn(__dadd_rn(__dmul_rn(K[r * 4], E[c]), __dmul_rn(K[r * 4 + 1], E[4 + c])), __dmul_rn(K[r * 4 + 2], E[8 + c]));
+  for (int r = 0; r < 4; ++r)
+    for (int c = 0; c < 4; ++c) A[r * 4 + c] = (r < 3 && c < 3) ? P[r * 4 + c] : (r == c ? 1.0 : 0.0);
+  const bool ok = invert4(A, B);
+  for (int i = 0; i < 12; ++i) t[i] = (float)P[i];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) t[12 + r * 3 + c] = (float)(ok ? B[r * 4 + c] : nanv);
+  t[21] = (float)__dmul_rn(__ddiv_rn(K[0], K[10]), GIPUMA_BASELINE);
+  for (int i = 22; i < GIPUMA_CAM; ++i) t[i] = 0.0f;
+}
+
+// probability_filter (misc/gipuma.py:160-177) and fusibile's depth range: depth where conf > prob_threshold and
+// depth_min <= depth <= depth_max, else 0 (a NaN fails every comparison)
+__global__ void gipuma_depth_kernel(const float* __restrict__ depths, const float* __restrict__ confs, long long n, float prob,
+                                    float dmin, float dmax, float* __restrict__ out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float d = __ldg(depths + i);
+    out[i] = (__ldg(confs + i) > prob && d >= dmin && d <= dmax) ? d : 0.0f;
+  }
+}
+
+// pixel (x, y) at depth d -> world point X = M^-1 (d x - p4.x, d y - p4.y, d - p4.z)
+__device__ __forceinline__ void gipuma_unproject(const float* __restrict__ cam, float x, float y, float d, float X[3]) {
+  const float a0 = sub(mul(d, x), __ldg(cam + 3)), a1 = sub(mul(d, y), __ldg(cam + 7)), a2 = sub(d, __ldg(cam + 11));
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+    X[i] = add(add(mul(__ldg(cam + 12 + i * 3), a0), mul(__ldg(cam + 13 + i * 3), a1)), mul(__ldg(cam + 14 + i * 3), a2));
+}
+
+// One probe: world point X of the reference pixel into source view s.  True iff it lands in the image on a valid source
+// pixel q whose disparity f_r b / D_s(q) is within disp of f_r b / z; q and D_s(q) are returned.
+__device__ __forceinline__ bool gipuma_probe(const float* __restrict__ cam_s, const float* __restrict__ depth_s, const float X[3],
+                                             float fb, float disp, int H, int W, int& q, float& ds) {
+  float t[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+    t[i] = add(add(add(mul(__ldg(cam_s + i * 4), X[0]), mul(__ldg(cam_s + i * 4 + 1), X[1])), mul(__ldg(cam_s + i * 4 + 2), X[2])),
+               __ldg(cam_s + i * 4 + 3));
+  const float xs = dvd(t[0], t[2]), ys = dvd(t[1], t[2]);
+  if (!(xs >= 0.0f && xs < (float)W && ys >= 0.0f && ys < (float)H)) return false;
+  q = (int)floorf(ys) * W + (int)floorf(xs);
+  ds = __ldg(depth_s + q);
+  return ds > 0.0f && fabsf(sub(dvd(fb, t[2]), dvd(fb, ds))) < disp;
+}
+
+// vote: the number of consistent source views of every valid, unused pixel of reference view r -> mask (n >= num_consistent)
+// and the block survivor counts
+__global__ void __launch_bounds__(FUSION_BLOCK)
+gipuma_vote_kernel(const float* __restrict__ depth, const unsigned char* __restrict__ used, const float* __restrict__ table, int N,
+                   int ref, int H, int W, float disp, int num_consistent, unsigned char* __restrict__ mask,
+                   int* __restrict__ block_counts) {
+  const int HW = H * W;
+  const int p = blockIdx.x * FUSION_BLOCK + threadIdx.x;
+  const bool inside = p < HW;
+  bool keep = false;
+  if (inside) {
+    const float d = __ldg(depth + (size_t)ref * HW + p);
+    if (d > 0.0f && __ldg(used + (size_t)ref * HW + p) == 0) {
+      const float* cam_r = table + (size_t)ref * GIPUMA_CAM;
+      const int py = p / W, px = p - py * W;
+      float X[3];
+      gipuma_unproject(cam_r, (float)px, (float)py, d, X);
+      const float fb = __ldg(cam_r + 21);
+      int n = 0;
+      for (int s = 0; s < N; ++s) {
+        if (s == ref) continue;
+        int q;
+        float ds;
+        n += gipuma_probe(table + (size_t)s * GIPUMA_CAM, depth + (size_t)s * HW, X, fb, disp, H, W, q, ds) ? 1 : 0;
+      }
+      keep = n >= num_consistent;
+    }
+    mask[p] = keep ? 1 : 0;
+  }
+  const int c = __syncthreads_count(keep);
+  if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
+}
+
+// emit: the survivors of the vote again, now averaging the world points and colours of the consistent source pixels and
+// marking those pixels used; the point goes to offsets[block] + rank, so a view's points are in row-major pixel order.
+// Survivors beyond capacity set their used marks but write no point.
+__global__ void __launch_bounds__(FUSION_BLOCK)
+gipuma_emit_kernel(const float* __restrict__ depth, const float* __restrict__ table, const float* __restrict__ images, int N,
+                   int ref, int H, int W, float disp, const unsigned char* __restrict__ mask, const int* __restrict__ offsets,
+                   unsigned char* __restrict__ used, float* __restrict__ xyz, unsigned char* __restrict__ rgb,
+                   long long capacity) {
+  __shared__ int warp_base[FUSION_BLOCK / 32];
+  const int HW = H * W;
+  const int p = blockIdx.x * FUSION_BLOCK + threadIdx.x;
+  const bool keep = p < HW && mask[p] != 0;
+  const unsigned bal = __ballot_sync(0xffffffffu, keep);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) warp_base[warp] = __popc(bal);
+  __syncthreads();
+  if (!keep) return;
+  long long pos = offsets[blockIdx.x] + __popc(bal & ((1u << lane) - 1u));
+  for (int w = 0; w < warp; ++w) pos += warp_base[w];
+  const float* cam_r = table + (size_t)ref * GIPUMA_CAM;
+  const int py = p / W, px = p - py * W;
+  float X[3], sum[3];
+  gipuma_unproject(cam_r, (float)px, (float)py, __ldg(depth + (size_t)ref * HW + p), X);
+  const float fb = __ldg(cam_r + 21);
+  int col[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    sum[k] = X[k];
+    col[k] = __float2int_rn(mul(__ldg(images + ((size_t)ref * 3 + k) * HW + p), 255.0f));
+  }
+  int n = 0;
+  for (int s = 0; s < N; ++s) {
+    if (s == ref) continue;
+    const float* cam_s = table + (size_t)s * GIPUMA_CAM;
+    int q;
+    float ds;
+    if (!gipuma_probe(cam_s, depth + (size_t)s * HW, X, fb, disp, H, W, q, ds)) continue;
+    const int qy = q / W, qx = q - qy * W;
+    float Xs[3];
+    gipuma_unproject(cam_s, (float)qx, (float)qy, ds, Xs);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      sum[k] = add(sum[k], Xs[k]);
+      col[k] += __float2int_rn(mul(__ldg(images + ((size_t)s * 3 + k) * HW + q), 255.0f));
+    }
+    used[(size_t)s * HW + q] = 1;
+    ++n;
+  }
+  if (pos >= capacity) return;
+  const float cnt = (float)(n + 1);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    xyz[pos * 3 + k] = dvd(sum[k], cnt);
+    rgb[pos * 3 + k] = (unsigned char)(col[k] / (n + 1));
+  }
+}
+
 }  // namespace mvsf
 
 extern "C" {
@@ -378,6 +536,58 @@ int mvsf_fusion_extract(const unsigned char* mask, const float* depth_avg, const
   mvsf::fusion_extract_kernel<<<mvsf::cdiv((long long)H * W, mvsf::FUSION_BLOCK), mvsf::FUSION_BLOCK, 0, (cudaStream_t)stream>>>(
       mask, depth_avg, (const int*)workspace, cam_inv, image, xyz, rgb, capacity, H, W);
   MVSF_LAUNCH_CHECK("fusion_extract");
+  return MVSF_OK;
+}
+
+int mvsf_fusion_gipuma_prepare(const float* depths, const float* confs, const float* cams, int N, int H, int W,
+                               float prob_threshold, float depth_min, float depth_max, float* depth, float* cam_table,
+                               mvsf_stream_t stream) {
+  MVSF_REQUIRE(depths && confs && cams && depth && cam_table, "fusion_gipuma_prepare: null pointer");
+  MVSF_REQUIRE(N > 0, "fusion_gipuma_prepare: N = %d < 1", N);
+  MVSF_REQUIRE(H > 0 && W > 0 && (long long)H * W < (1ll << 31), "fusion_gipuma_prepare: H x W = %d x %d outside [1, 2^31)", H, W);
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long n = (long long)N * H * W;
+  const int blocks = mvsf::cdiv(n, 256) < 65536 ? mvsf::cdiv(n, 256) : 65536;   // grid-stride beyond
+  mvsf::gipuma_depth_kernel<<<blocks, 256, 0, st>>>(
+      depths, confs, n, prob_threshold, depth_min, depth_max, depth);
+  MVSF_LAUNCH_CHECK("fusion_gipuma_prepare (depth)");
+  mvsf::gipuma_cameras_kernel<<<mvsf::cdiv(N, 64), 64, 0, st>>>(cams, N, cam_table);
+  MVSF_LAUNCH_CHECK("fusion_gipuma_prepare (cameras)");
+  return MVSF_OK;
+}
+
+int mvsf_fusion_gipuma_vote(const float* depth, const unsigned char* used, const float* cam_table, int N, int ref, int H, int W,
+                            float disp_threshold, int num_consistent, unsigned char* mask, void* workspace,
+                            size_t workspace_bytes, mvsf_stream_t stream) {
+  MVSF_REQUIRE(depth && used && cam_table && mask && workspace, "fusion_gipuma_vote: null pointer");
+  MVSF_REQUIRE(H > 0 && W > 0 && (long long)H * W < (1ll << 31), "fusion_gipuma_vote: H x W = %d x %d outside [1, 2^31)", H, W);
+  MVSF_REQUIRE(N > 0 && ref >= 0 && ref < N, "fusion_gipuma_vote: reference view %d outside the scene's %d views", ref, N);
+  MVSF_REQUIRE(num_consistent >= 0, "fusion_gipuma_vote: num_consistent = %d < 0", num_consistent);
+  if (workspace_bytes < mvsf::fusion_ws_bytes(H, W))
+    return mvsf::fail(MVSF_ERR_WORKSPACE, "fusion_gipuma_vote: workspace %zu < %zu bytes", workspace_bytes, mvsf::fusion_ws_bytes(H, W));
+  const int blocks = mvsf::cdiv((long long)H * W, mvsf::FUSION_BLOCK);
+  int* counts = (int*)workspace;
+  cudaStream_t st = (cudaStream_t)stream;
+  mvsf::gipuma_vote_kernel<<<blocks, mvsf::FUSION_BLOCK, 0, st>>>(depth, used, cam_table, N, ref, H, W, disp_threshold,
+                                                                  num_consistent, mask, counts);
+  MVSF_LAUNCH_CHECK("fusion_gipuma_vote");
+  mvsf::fusion_scan_kernel<<<1, mvsf::FUSION_SCAN_THREADS, 0, st>>>(counts, blocks);
+  MVSF_LAUNCH_CHECK("fusion_scan");
+  return MVSF_OK;
+}
+
+int mvsf_fusion_gipuma_emit(const float* depth, const float* cam_table, const float* images, int N, int ref, int H, int W,
+                            float disp_threshold, const unsigned char* mask, const void* workspace, size_t workspace_bytes,
+                            unsigned char* used, float* xyz, unsigned char* rgb, long long capacity, mvsf_stream_t stream) {
+  MVSF_REQUIRE(depth && cam_table && images && mask && workspace && used, "fusion_gipuma_emit: null pointer");
+  MVSF_REQUIRE(capacity >= 0 && (capacity == 0 || (xyz && rgb)), "fusion_gipuma_emit: no output for %lld points", capacity);
+  MVSF_REQUIRE(H > 0 && W > 0 && (long long)H * W < (1ll << 31), "fusion_gipuma_emit: H x W = %d x %d outside [1, 2^31)", H, W);
+  MVSF_REQUIRE(N > 0 && ref >= 0 && ref < N, "fusion_gipuma_emit: reference view %d outside the scene's %d views", ref, N);
+  if (workspace_bytes < mvsf::fusion_ws_bytes(H, W))
+    return mvsf::fail(MVSF_ERR_WORKSPACE, "fusion_gipuma_emit: workspace %zu < %zu bytes", workspace_bytes, mvsf::fusion_ws_bytes(H, W));
+  mvsf::gipuma_emit_kernel<<<mvsf::cdiv((long long)H * W, mvsf::FUSION_BLOCK), mvsf::FUSION_BLOCK, 0, (cudaStream_t)stream>>>(
+      depth, cam_table, images, N, ref, H, W, disp_threshold, mask, (const int*)workspace, used, xyz, rgb, capacity);
+  MVSF_LAUNCH_CHECK("fusion_gipuma_emit");
   return MVSF_OK;
 }
 }

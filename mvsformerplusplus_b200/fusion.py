@@ -3,14 +3,17 @@ the model (test.py:552-560).
 
   filter_view(ref_idx, src_idx, depths, confs, cams, method, ...)     <- one iteration of test.py:395-408 / :453-480
   fuse_scene(depths, confs, cams, images, pairs, method, ...)         <- filter_depth / dynamic_filter_depth, test.py:387-517
+  fuse_scene_gipuma(depths, confs, cams, images, ...)                 <- gipuma_filter, misc/gipuma.py:208-228 (fusibile)
+  gipuma_prepare(...) / gipuma_step(scene, ref, ...)                  <- one reference view of fuse_scene_gipuma
   write_ply(path, xyz, rgb)                                           <- test.py:431-441
   read_pair_file(path)                                                <- test.py:136-146
 
-`method` is "pcd" or "dpcd" (test.py:61).  A scene is depths [N,H,W], confs [N,H,W] (fp32 in [0,1], what the model
+`method` is "pcd" or "dpcd" (test.py:61); the third method, "gipuma", has its own entry point.  A scene is depths [N,H,W], confs [N,H,W] (fp32 in [0,1], what the model
 returns), cams [N,2,4,4] (slot 0 extrinsic, slot 1 [:3,:3] intrinsic) and images [N,3,H,W] (fp32 in [0,1]), all on the
 device; the views a pair names are read in place through their indices.
 """
 import ctypes
+import math
 
 import numpy as np
 import torch
@@ -152,3 +155,84 @@ def fuse_scene(depths, confs, cams, images, pairs, method, n_src_views=10, conf=
                       rgb[base:], counts[k], H, W)
         base += counts[k]
     return xyz, rgb
+
+
+GIPUMA_CAM = 32   # floats per view of the gipuma camera table (csrc/fusion.cu)
+
+
+class GipumaScene:
+    """The state of a gipuma fusion between reference views: depth [N,H,W] (filtered), cams [N,32] (the camera table:
+    P = K E[:3] row-major, M^-1 of M = P[:, :3] row-major, f b, padding), used [N,H,W] uint8 (the source pixels earlier
+    views consumed), images [N,3,H,W], and the per-view mask and workspace the steps reuse."""
+
+    def __init__(self, depth, cams, used, images):
+        self.depth, self.cams, self.used, self.images = depth, cams, used, images
+        N, H, W = depth.shape
+        self.mask = torch.empty(H, W, dtype=torch.uint8, device=depth.device)
+        self.ws = torch.empty(_workspace_ints(H, W), dtype=torch.int32, device=depth.device)
+
+
+def _finite(name, x):
+    x = float(x)
+    if not math.isfinite(x):
+        raise ValueError(f"fusion: {name} = {x} is not finite")
+    return x
+
+
+def gipuma_prepare(depths, confs, cams, images, prob_threshold=0.5, depth_min=0.001, depth_max=100000.0):
+    """-> GipumaScene with no used marks: probability_filter (misc/gipuma.py:160-177; depth 0 where conf is not
+    > prob_threshold) and fusibile's depth range (depth 0 outside [depth_min, depth_max]), and the camera table."""
+    prob, dmin, dmax = (_finite(n, x) for n, x in (("prob_threshold", prob_threshold), ("depth_min", depth_min),
+                                                      ("depth_max", depth_max)))
+    if dmin <= 0:
+        raise ValueError(f"fusion: depth_min = {dmin} must be > 0")
+    N, H, W = _check_scene(depths, confs, cams, images)
+    depth = torch.empty_like(depths)
+    table = torch.empty(N, GIPUMA_CAM, dtype=torch.float32, device=depths.device)
+    _lib.call("mvsf_fusion_gipuma_prepare", depths, confs, cams, N, H, W, prob, dmin, dmax, depth, table)
+    return GipumaScene(depth, table, torch.zeros(N, H, W, dtype=torch.uint8, device=depths.device), images)
+
+
+def _num_consistent(n):
+    if isinstance(n, bool) or float(n) != int(n) or int(n) < 0:
+        raise ValueError(f"fusion: num_consistent = {n!r} must be a whole number >= 0")
+    return int(n)
+
+
+def gipuma_step(scene, ref, disp_threshold=0.2, num_consistent=3):
+    """-> (xyz [M,3] float32, rgb [M,3] uint8) of reference view `ref` on the device, in row-major pixel order, and
+    scene.used updated: a valid pixel not yet used emits a point when at least num_consistent other views are consistent
+    with it (its world point lands on a valid source pixel whose disparity f b / depth is within disp_threshold); the
+    point and colour are the means over the pixel and those source pixels, which become used.  The view's point count
+    crosses to the host in one 4-byte read, which sizes the output."""
+    N, H, W = scene.depth.shape
+    if not 0 <= int(ref) < N:
+        raise ValueError(f"fusion: view {ref} outside the scene's {N} views")
+    disp, nc = _finite("disp_threshold", disp_threshold), _num_consistent(num_consistent)
+    nbytes = scene.ws.numel() * 4
+    _lib.call("mvsf_fusion_gipuma_vote", scene.depth, scene.used, scene.cams, N, int(ref), H, W, disp, nc, scene.mask, scene.ws,
+              nbytes)
+    M = int(scene.ws[-1])   # the one synchronisation of a view
+    xyz = torch.empty(M, 3, dtype=torch.float32, device=scene.depth.device)
+    rgb = torch.empty(M, 3, dtype=torch.uint8, device=scene.depth.device)
+    if M:
+        _lib.call("mvsf_fusion_gipuma_emit", scene.depth, scene.cams, scene.images, N, int(ref), H, W, disp, scene.mask, scene.ws,
+                  nbytes, scene.used, xyz, rgb, M)
+    return xyz, rgb
+
+
+def fuse_scene_gipuma(depths, confs, cams, images, prob_threshold=0.5, disp_threshold=0.2, num_consistent=3, depth_min=0.001,
+                      depth_max=100000.0):
+    """-> (xyz [M,3] float32, rgb [M,3] uint8) on the device: the gipuma fusion of gipuma_filter (misc/gipuma.py:208-228,
+    which runs the external fusibile at normal_thresh = 360), every view a reference view, in index order, and every other
+    view its source.  The defaults are those of test.py:71-73 and misc/gipuma.py:187-188.  Points come out view by view
+    and, within a view, in row-major pixel order, in world coordinates; rgb is the integer mean of round(255 image) over
+    the fused pixels.  To threshold confidences saved as uint8 exactly as the reference does, pass conf_u8.float() / 255.
+
+    The views are sequential (each consumes source pixels the next ones no longer fuse): one gipuma_step per view, each
+    with one 4-byte read of its point count."""
+    _finite("disp_threshold", disp_threshold)
+    _num_consistent(num_consistent)
+    scene = gipuma_prepare(depths, confs, cams, images, prob_threshold, depth_min, depth_max)
+    parts = [gipuma_step(scene, r, disp_threshold, num_consistent) for r in range(depths.shape[0])]
+    return torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts])
