@@ -344,6 +344,20 @@ int mvsf_fusion_gipuma_emit(const float* depth, const float* cam_table, const fl
                             float disp_threshold, const unsigned char* mask, const void* workspace, size_t workspace_bytes,
                             unsigned char* used, float* xyz, unsigned char* rgb, long long capacity, mvsf_stream_t stream);
 
+/* ---- image preparation of the eval loader, datasets/general_eval.py:112-131 (read_img's edge pad, scale_mvs_input's
+ *      cv2.resize) and :210-211 (ToTensor + Normalize), bit-exact.  Images are uint8 RGB, channels-last [H][W][3].
+ * src [N][h][w][3] (one source size) -> dst [N][H][W][3]: pad_rows rows repeated at the top and the bottom (the edge pad
+ * of np.pad), then cv2.resize(img, (W, H)) with INTER_LINEAR as cv2 computes it for uint8 (equal sizes: a copy).
+ * Bad arguments (null pointer, a size < 1, pad_rows < 0, 2^31 pixels or more per image): -1; nothing launched. */
+int mvsf_image_resize_u8(const unsigned char* src, int N, int h, int w, int pad_rows, unsigned char* dst, int H, int W,
+                         mvsf_stream_t stream);
+/* The V images views[0..V) (indices in HOST memory, V in [1, 64]) of scene [N][H][W][3] -> norm [V][3][H][W] =
+ * (u8 / 255 - mean) / std with the ImageNet mean and std, and colour [V][3][H][W] = trunc(clip((norm std + mean) 255, 0,
+ * 255)) / 255, the colour test.py:287-292 saves for fusion before its JPEG encode.  Either output may be NULL, not both.
+ * Bad arguments (null pointer, V outside [1, 64], a view outside [0, N), H W outside [1, 2^31)): -1; nothing launched. */
+int mvsf_image_normalize(const unsigned char* scene, int N, const int* views, int V, int H, int W, float* norm,
+                         float* colour, mvsf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,7 +5,7 @@ from .config import default_args, load_args, validate_args  # noqa: F401
 __all__ = ["default_args", "load_args", "validate_args", "StageNet", "FMT_with_pathway", "HotPathNet", "install",
            "cascade_forward", "homo_warping_3D_with_mask", "FPNEncoder", "FPNDecoder", "CrossVITDecoder",
            "DinoVisionTransformer", "vit_base", "DINOv2MVSNet", "filter_view", "fuse_scene", "fuse_scene_gipuma", "write_ply",
-           "read_pair_file"]
+           "read_pair_file", "load_scene", "reconstruct_scene"]
 
 
 def __getattr__(name):  # hotpath imports torch + ctypes; keep `import mvsformerplusplus_b200` light
@@ -17,4 +17,7 @@ def __getattr__(name):  # hotpath imports torch + ctypes; keep `import mvsformer
     if name in ("filter_view", "fuse_scene", "fuse_scene_gipuma", "write_ply", "read_pair_file"):
         from . import fusion
         return getattr(fusion, name)
+    if name in ("load_scene", "reconstruct_scene"):
+        from . import scene
+        return getattr(scene, name)
     raise AttributeError(name)

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmvsf_b200.so")
 STAMP = os.path.join(HERE, ".libmvsf_b200.stamp")
-SOURCES = ["api.cu", "geometry.cu", "warp_corr.cu", "warp_tile.cu", "vis_cnn.cu", "costreg_unet.cu", "costreg_tr.cu", "fmt.cu", "linear_tc.cu", "conv3d_tc.cu", "fpn.cu", "vit_decoder.cu", "vit.cu", "fusion.cu"]
+SOURCES = ["api.cu", "geometry.cu", "warp_corr.cu", "warp_tile.cu", "vis_cnn.cu", "costreg_unet.cu", "costreg_tr.cu", "fmt.cu", "linear_tc.cu", "conv3d_tc.cu", "fpn.cu", "vit_decoder.cu", "vit.cu", "fusion.cu", "image_prep.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "--extended-lambda"] + os.environ.get("MVSF_EXTRA_NVCC_FLAGS", "").split()
 
