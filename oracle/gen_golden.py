@@ -1,33 +1,23 @@
 """ORACLE - TEST INFRASTRUCTURE ONLY.  Generates tests/golden/*.npz by executing the REFERENCE's own
-modules (imported read-only from /root/reference, which exists only in the build container) on seeded
-synthetic inputs.  The fixtures pin oracle/hotpath.py (tests/test_oracle_golden.py) and, on the GPU box,
-the CUDA path (tests/test_gpu_parity.py).  Re-run:  python oracle/gen_golden.py
+modules (found and imported read-only by oracle/reference.py) on seeded synthetic inputs.  The fixtures pin
+oracle/hotpath.py (tests/test_oracle_golden.py) and, on the GPU box, the CUDA path (tests/test_gpu_parity.py).
+Re-run:  python oracle/gen_golden.py
 
 The reference has no tests/golden vectors of its own (SURVEY.md §4), so these reference-executed outputs
 are the pin.  Reference code is imported, never copied.
 """
-import json
 import os
 import sys
 
-import numpy as np
 import torch
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("MVSF_REFERENCE", "/root/reference")
 sys.path.insert(0, REPO)
-sys.path.insert(0, REF)
 
 from mvsformerplusplus_b200 import synth  # noqa: E402
 from mvsformerplusplus_b200.config import default_args  # noqa: E402
-
-
-from oracle.ref_hotpath import RefHotPath, import_reference as _import_reference, reference_hotpath  # noqa: E402
-
-
-def import_reference():
-    return _import_reference(REF)
-
+from oracle import fixture  # noqa: E402
+from oracle.ref_hotpath import RefHotPath, import_reference, reference_hotpath  # noqa: E402
 
 CASES = {
     # name: (V, H, W, feature seed, weight seed)
@@ -72,8 +62,7 @@ def main():
         # full-resolution FMT outputs are large: keep view 1 (first source view) of stages 2-4 only
         for k in ("stage2", "stage3", "stage4"):
             blob[f"fmt.{k}.view1"] = out["features"][k][0, 1].numpy()
-        blob["meta"] = np.frombuffer(json.dumps(c).encode(), dtype=np.uint8)
-        np.savez_compressed(os.path.join(out_dir, name + ".npz"), **blob)
+        fixture.save(os.path.join(out_dir, name + ".npz"), blob, c)
         print(name, "refined_depth range", float(out["refined_depth"].min()), float(out["refined_depth"].max()),
               "stage4 conf mean", float(out["stage4"]["photometric_confidence"].mean()))
 
@@ -86,8 +75,8 @@ def main():
     refp, srcp = compose_projection(pm[:, 0]), compose_projection(pm[:, 2])
     dvals = 425.0 + 500.0 * torch.rand(1, D, H, W, generator=g)
     warped, mask = R["homo_warp"](src, srcp, refp, dvals)
-    np.savez_compressed(os.path.join(out_dir, "warp_seam.npz"), src=src.numpy(), src_proj=srcp.numpy(),
-                        ref_proj=refp.numpy(), depth_values=dvals.numpy(), warped=warped.numpy(), mask=mask.numpy())
+    fixture.save(os.path.join(out_dir, "warp_seam.npz"), dict(src=src.numpy(), src_proj=srcp.numpy(), ref_proj=refp.numpy(),
+                                                              depth_values=dvals.numpy(), warped=warped.numpy(), mask=mask.numpy()))
     print("warp_seam: fraction masked", float(mask.float().mean()))
 
 

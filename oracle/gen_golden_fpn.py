@@ -9,7 +9,6 @@ and leaves every other fixture alone.  Re-run:  python oracle/gen_golden_fpn.py
 Weights: synth.randomize_state_dict(seed=wseed) over a module with `encoder` and `decoder` children (tests rebuild them
 from the seed stored in each fixture's meta).
 """
-import json
 import os
 import sys
 
@@ -21,7 +20,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from mvsformerplusplus_b200 import synth  # noqa: E402
-from oracle.ref_hotpath import reference_root  # noqa: E402
+from oracle import fixture, reference  # noqa: E402
 
 CASES = {
     "fpn_n2_64x96": dict(N=2, H=64, W=96, iseed=31, vseed=32, wseed=33),
@@ -47,12 +46,7 @@ def make_inputs(c):
 
 
 def main():
-    root = reference_root()
-    if root is None:
-        raise SystemExit("reference sources not found")
-    sys.path.insert(0, root)
-    import models.dino.layers.attention as A
-    A.FLASH_AVAILABLE = False
+    reference.import_models()
     from models.module import FPNDecoder, FPNEncoder
     torch.set_num_threads(max(1, os.cpu_count() or 1))
     out_dir = os.path.join(REPO, "tests", "golden")
@@ -69,13 +63,11 @@ def main():
         # vit_feat is a plain torch.randn draw (bit-reproducible from vseed); x involves CPU convolutions, so it is stored
         full = dict(conv01=c01, conv11=c11, conv21=c21, conv31=c31, **{f"out{k}": o for k, o in enumerate(outs)})
         blob = dict(x=x.numpy(), **{k: fixture_crop(k, v).contiguous().numpy() for k, v in full.items()})
-        blob["meta"] = np.frombuffer(json.dumps(c).encode(), dtype=np.uint8)
-        np.savez_compressed(os.path.join(out_dir, name + ".npz"), **blob)
-        print(name, {k: float(np.abs(v).max()) for k, v in blob.items() if k != "meta"})
+        fixture.save(os.path.join(out_dir, name + ".npz"), blob, c)
+        print(name, {k: float(np.abs(v).max()) for k, v in blob.items()})
 
     from models.networks.DINOv2_mvsformer_model import DINOv2MVSNet
-    cfg = json.load(open(os.path.join(root, "config", "mvsformer++.json")))["arch"]["args"]
-    model = DINOv2MVSNet(cfg)
+    model = DINOv2MVSNet(reference.config())
     with open(os.path.join(out_dir, "fpn_state_dict_keys.txt"), "w") as f:
         for k, v in model.state_dict().items():
             if k.startswith("encoder.") or k.startswith("decoder."):

@@ -1,5 +1,5 @@
 """ORACLE - TEST INFRASTRUCTURE ONLY.  Generates the depth-map fusion fixtures by executing the REFERENCE's own
-misc/fusion.py (imported read-only; oracle/_ref/misc/fusion.py where build() copied it) on the seeded synthetic scenes of
+misc/fusion.py (loaded read-only by oracle/reference.py) on the seeded synthetic scenes of
 synth.make_fusion_scene.  The glue between its functions (test.py:395-412 for pcd, :453-483 for dpcd) is restated in
 reference_filter below, because test.py parses the command line on import.  Writes only
 
@@ -14,8 +14,6 @@ misc/fusion.py builds its pixel grid with `.cuda()` (fusion.py:9-10).  To run it
 replaces torch.Tensor.cuda by the identity for the duration of the call and restores it afterwards.
 """
 import contextlib
-import importlib.util
-import json
 import os
 import sys
 
@@ -26,6 +24,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from mvsformerplusplus_b200 import synth  # noqa: E402
+from oracle import fixture, reference  # noqa: E402
 
 CASES = {
     "fusion_n6_40x72": dict(N=6, H=40, W=72, n_src=4, seed=77, refs=[0, 5]),
@@ -36,14 +35,7 @@ DEFAULTS = dict(conf=0.5, thres_view=2, thres_disp=1.0, dist_base=4.0, rel_diff_
 
 def reference_fusion_module():
     """The reference's misc/fusion.py as a module, or None where the reference is not available."""
-    for root in (os.environ.get("MVSF_REFERENCE"), os.path.join(REPO, "oracle", "_ref"), "/root/reference"):
-        path = os.path.join(root, "misc", "fusion.py") if root else None
-        if path and os.path.isfile(path):
-            spec = importlib.util.spec_from_file_location("mvsf_reference_fusion", path)
-            mod = importlib.util.module_from_spec(spec)
-            spec.loader.exec_module(mod)
-            return mod
-    return None
+    return reference.module("misc/fusion.py") if reference.root("misc/fusion.py") else None
 
 
 @contextlib.contextmanager
@@ -106,8 +98,7 @@ def main():
                 blob[f"{method}_depth_{r}"] = avg.numpy()
                 blob[f"{method}_points_{r}"] = pts.permute(1, 2, 0)[mask].numpy()
                 print(name, method, r, "kept", float(mask.float().mean()))
-        blob["meta"] = np.frombuffer(json.dumps(meta).encode(), dtype=np.uint8)
-        np.savez_compressed(os.path.join(out_dir, name + ".npz"), **blob)
+        fixture.save(os.path.join(out_dir, name + ".npz"), blob, meta)
         print(name, os.path.getsize(os.path.join(out_dir, name + ".npz")), "bytes")
 
 

@@ -1,5 +1,5 @@
 """ORACLE - TEST INFRASTRUCTURE ONLY.  Generates the gipuma fusion fixture by executing the REFERENCE's own input stage of
-gipuma_filter (misc/gipuma.py and datasets/data_io.py, imported read-only from the reference or from oracle/_ref/) on a
+gipuma_filter (misc/gipuma.py and datasets/data_io.py, loaded read-only by oracle/reference.py) on a
 seeded scene of synth.make_fusion_scene, written to disk the way test.py saves a scan:
 
   depth_est/<view>.pfm          datasets/data_io.save_pfm (test.py:278)
@@ -17,12 +17,9 @@ so the fixture holds the inputs it would get.  Writes only
 
 Re-run:  python oracle/gen_golden_gipuma.py
 """
-import importlib.util
-import json
 import os
 import sys
 import tempfile
-import types
 
 import numpy as np
 import torch
@@ -31,6 +28,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from mvsformerplusplus_b200 import synth  # noqa: E402
+from oracle import fixture, reference  # noqa: E402
 
 NAME = "gipuma_n8_40x72"
 # f b / depth is ~0.108 at this size (f ~ 130 px, depth ~ 650), so a disparity threshold of the order of the synthetic
@@ -38,36 +36,11 @@ NAME = "gipuma_n8_40x72"
 CASE = dict(N=8, H=40, W=72, seed=81, n_src=7, prob_threshold=0.5, disp_threshold=0.0015, num_consistent=2)
 
 
-def _load(name, path):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    sys.modules[name] = mod
-    spec.loader.exec_module(mod)
-    return mod
-
-
 def reference_gipuma_modules():
-    """(misc/gipuma.py, datasets/data_io.py) of the reference as modules, or None where the reference is not available.
-    data_io is registered as datasets.data_io without running the reference's datasets/__init__.py (its data loaders)."""
-    for root in (os.environ.get("MVSF_REFERENCE"), os.path.join(REPO, "oracle", "_ref"), "/root/reference"):
-        if not root:
-            continue
-        g, d = os.path.join(root, "misc", "gipuma.py"), os.path.join(root, "datasets", "data_io.py")
-        if os.path.isfile(g) and os.path.isfile(d):
-            saved = {k: sys.modules.get(k) for k in ("datasets", "datasets.data_io")}
-            try:
-                sys.modules["datasets"] = types.ModuleType("datasets")
-                data_io = _load("datasets.data_io", d)
-                sys.modules["datasets"].data_io = data_io
-                gipuma = _load("mvsf_reference_gipuma", g)
-            finally:
-                for k, v in saved.items():
-                    if v is None:
-                        sys.modules.pop(k, None)
-                    else:
-                        sys.modules[k] = v
-            return gipuma, data_io
-    return None
+    """(misc/gipuma.py, datasets/data_io.py) of the reference as modules, or None where the reference is not available"""
+    if reference.root("misc/gipuma.py", "datasets/data_io.py") is None:
+        return None
+    return reference.module("misc/gipuma.py"), reference.module("datasets/data_io.py")
 
 
 def write_cam(path, cam):
@@ -119,10 +92,8 @@ def main():
     depths, conf_u8, cams, images = scene()
     filtered, P = reference_inputs(*mods, depths, conf_u8, cams, CASE["prob_threshold"])
     print(NAME, "valid after probability_filter", float((filtered > 0).mean()))
-    blob = dict(depths=depths, conf_u8=conf_u8, cams=cams, images=images, filtered=filtered, P=P,
-                meta=np.frombuffer(json.dumps(CASE).encode(), dtype=np.uint8))
     path = os.path.join(REPO, "tests", "golden", NAME + ".npz")
-    np.savez_compressed(path, **blob)
+    fixture.save(path, dict(depths=depths, conf_u8=conf_u8, cams=cams, images=images, filtered=filtered, P=P), CASE)
     print(NAME, os.path.getsize(path), "bytes")
 
 

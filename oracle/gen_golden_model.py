@@ -13,19 +13,17 @@ re-created from the seeds in each fixture's meta (make_inputs), so only outputs 
 photometric_confidence, per-stage depth and confidence, a seeded sample of each stage's prob_volume, and the stage-1
 features before FMT.
 """
-import json
 import os
 import sys
 
-import numpy as np
 import torch
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from mvsformerplusplus_b200 import synth  # noqa: E402
+from oracle import fixture, reference  # noqa: E402
 from oracle.gen_golden_vit import vit_weights  # noqa: E402
-from oracle.ref_hotpath import reference_root  # noqa: E402
 
 CASES = {
     "model_b1v3_96x128": dict(B=1, V=3, H=96, W=128, numdepth=192, iseed=301, wseed=302),
@@ -63,22 +61,16 @@ def fixture_outputs(c, out, features_fpn):
     return blob
 
 
-def reference_model(root):
-    sys.path.insert(0, root)
-    import models.dino.layers.attention as A
-    A.FLASH_AVAILABLE = False
-    A.XFORMERS_AVAILABLE = False
+def reference_model():
+    reference.import_models()
     from models.networks.DINOv2_mvsformer_model import DINOv2MVSNet
-    cfg = json.load(open(os.path.join(root, "config", "mvsformer++.json")))["arch"]["args"]
+    cfg = reference.config()
     cfg["vit_path"] = ""   # the weights are seeded; nothing is read
     return DINOv2MVSNet, cfg
 
 
 def main():
-    root = reference_root()
-    if root is None:
-        raise SystemExit("reference sources not found")
-    DINOv2MVSNet, cfg = reference_model(root)
+    DINOv2MVSNet, cfg = reference_model()
     torch.set_num_threads(max(1, os.cpu_count() or 1))
     out_dir = os.path.join(REPO, "tests", "golden")
     for name, c in CASES.items():
@@ -95,8 +87,7 @@ def main():
         with torch.no_grad():
             out = model(imgs, proj, dv, tmp=TMP)
         blob = {k: v.contiguous().numpy() for k, v in fixture_outputs(c, out, cap["fpn"]).items()}
-        blob["meta"] = np.frombuffer(json.dumps(c).encode(), dtype=np.uint8)
-        np.savez_compressed(os.path.join(out_dir, name + ".npz"), **blob)
+        fixture.save(os.path.join(out_dir, name + ".npz"), blob, c)
         print(name, "refined_depth", float(out["refined_depth"].min()), float(out["refined_depth"].max()),
               "confidence mean", float(out["photometric_confidence"].mean()))
 

@@ -1,5 +1,5 @@
 """ORACLE - TEST INFRASTRUCTURE ONLY.  Generates the scene fixtures by executing the REFERENCE's own eval loader
-(datasets/general_eval.MVSDataset, imported read-only from the reference or from oracle/_ref/) on small seeded scene
+(datasets/general_eval.MVSDataset, loaded read-only by oracle/reference.py) on small seeded scene
 folders in the MVSNet layout, and the reference's own file writers (datasets/data_io.save_pfm, and write_cam as test.py
 and test_tt.py define it, taken from their source at run time) on a fixed depth map and camera.
 
@@ -22,13 +22,10 @@ Writes tests/golden/scene_<case>.npz:
 
 Re-run:  python oracle/gen_golden_scene.py
 """
-import ast
 import io
-import json
 import os
 import sys
 import tempfile
-import types
 
 import numpy as np
 
@@ -36,6 +33,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from mvsformerplusplus_b200 import synth  # noqa: E402
+from oracle import fixture, reference  # noqa: E402
 
 # sizes are (h, w) of the source JPEGs and (max_h, max_w) of the prepared images, multiples of 32 so that the model runs
 CASES = {
@@ -109,41 +107,11 @@ def write_files(root, files):
     return os.path.join(root, "test")
 
 
-def _reference_root():
-    for root in (os.environ.get("MVSF_REFERENCE"), os.path.join(REPO, "oracle", "_ref"), "/root/reference"):
-        if root and all(os.path.isfile(os.path.join(root, "datasets", n)) for n in ("general_eval.py", "data_io.py")):
-            return root
-    return None
-
-
 def reference_datasets():
-    """(general_eval, data_io) of the reference as modules, or None.  `datasets` is registered as a bare package so that
-    its __init__ (the training loaders) does not run."""
-    import importlib.util
-    root = _reference_root()
-    if root is None:
+    """(general_eval, data_io) of the reference as modules, or None where the reference is not available"""
+    if reference.root("datasets/general_eval.py", "datasets/data_io.py") is None:
         return None
-    pkg = types.ModuleType("datasets")
-    pkg.__path__ = [os.path.join(root, "datasets")]
-    sys.modules["datasets"] = pkg
-    mods = []
-    for name in ("data_io", "general_eval"):
-        spec = importlib.util.spec_from_file_location(f"datasets.{name}", os.path.join(root, "datasets", name + ".py"))
-        mod = importlib.util.module_from_spec(spec)
-        sys.modules[f"datasets.{name}"] = mod
-        spec.loader.exec_module(mod)
-        mods.append(mod)
-    return mods[1], mods[0]
-
-
-def reference_function(script, name):
-    """a top-level function of one of the reference's scripts (which parse arguments at import), compiled from its source"""
-    with open(os.path.join("/root/reference" if os.path.isdir("/root/reference") else os.environ["MVSF_REFERENCE"], script)) as f:
-        tree = ast.parse(f.read())
-    fn = next(n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name == name)
-    ns = {"np": np}
-    exec(compile(ast.Module(body=[fn], type_ignores=[]), script, "exec"), ns)
-    return ns[name]
+    return reference.module("datasets/general_eval.py"), reference.module("datasets/data_io.py")
 
 
 def generate(name, case, ge, data_io):
@@ -178,9 +146,9 @@ def generate(name, case, ge, data_io):
         cam = blob["proj_0_stage4"][0]
         if case["dataset"] == "tt":
             dv = blob["dv_0"]
-            reference_function("test_tt.py", "write_cam")(os.path.join(d, "c.txt"), cam, [dv[0], dv[-1]])
+            reference.function("test_tt.py", "write_cam")(os.path.join(d, "c.txt"), cam, [dv[0], dv[-1]])
         else:
-            reference_function("test.py", "write_cam")(os.path.join(d, "c.txt"), cam)
+            reference.function("test.py", "write_cam")(os.path.join(d, "c.txt"), cam)
         blob["pfm_depth"] = depth
         blob["pfm_bytes"] = np.frombuffer(open(os.path.join(d, "d.pfm"), "rb").read(), np.uint8)
         blob["cam_bytes"] = np.frombuffer(open(os.path.join(d, "c.txt"), "rb").read(), np.uint8)
@@ -188,9 +156,8 @@ def generate(name, case, ge, data_io):
     for i, rel in enumerate(names):
         blob[f"file_{i}"] = np.frombuffer(files[rel], np.uint8)
     meta = dict(case, pairs={str(k): v for k, v in case["pairs"].items()}, files=names, items=items)
-    blob["meta"] = np.frombuffer(json.dumps(meta).encode(), np.uint8)
     path = os.path.join(REPO, "tests", "golden", f"scene_{name}.npz")
-    np.savez_compressed(path, **blob)
+    fixture.save(path, blob, meta)
     print(name, len(items), "items", os.path.getsize(path), "bytes")
 
 

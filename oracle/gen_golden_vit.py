@@ -11,11 +11,9 @@ pos_embed and cls_token at O(0.5) (synth gives them ~1e-3 / ~0.04) and, for the 
 (DINOv2-style massive activations) and sharpens one block's attention.  Images are synth.make_images draws re-created
 from the seeds in each fixture's meta, so only outputs are stored.
 """
-import json
 import os
 import sys
 
-import numpy as np
 import torch
 import torch.nn as nn
 
@@ -23,7 +21,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from mvsformerplusplus_b200 import synth  # noqa: E402
-from oracle.ref_hotpath import reference_root  # noqa: E402
+from oracle import fixture, reference  # noqa: E402
 
 CASES = {
     "vit_n2_3x4": dict(n=2, gh=3, gw=4, xseed=81, wseed=82, harsh=False),          # 42 x 56, H != W
@@ -54,21 +52,16 @@ def make_images(c):
     return synth.make_images(c["n"], 14 * c["gh"], 14 * c["gw"], seed=c["xseed"])
 
 
-def reference_vit_base(root):
-    sys.path.insert(0, root)
-    import models.dino.layers.attention as A
-    A.FLASH_AVAILABLE = False
-    A.XFORMERS_AVAILABLE = False
+def reference_vit_base(root=None):
+    """the reference's vit_base, from the models/ package under root (default: the one reference.root finds), and the
+    shipped arch.args"""
+    reference.import_models(root)
     from models.dino.dinov2 import vit_base
-    cfg = json.load(open(os.path.join(root, "config", "mvsformer++.json")))["arch"]["args"]
-    return vit_base, cfg
+    return vit_base, reference.config()
 
 
 def main():
-    root = reference_root()
-    if root is None:
-        raise SystemExit("reference sources not found")
-    vit_base, cfg = reference_vit_base(root)
+    vit_base, cfg = reference_vit_base()
     torch.set_num_threads(max(1, os.cpu_count() or 1))
     out_dir = os.path.join(REPO, "tests", "golden")
     for name, c in CASES.items():
@@ -80,8 +73,7 @@ def main():
         with torch.no_grad():
             outs = m.vit.forward_interval_features(make_images(c))
         blob = {f"out{i}": o.contiguous().numpy() for i, o in enumerate(outs)}
-        blob["meta"] = np.frombuffer(json.dumps(c).encode(), dtype=np.uint8)
-        np.savez_compressed(os.path.join(out_dir, name + ".npz"), **blob)
+        fixture.save(os.path.join(out_dir, name + ".npz"), blob, c)
         print(name, [tuple(o.shape) for o in outs], [float(o.abs().max()) for o in outs])
 
     from models.networks.DINOv2_mvsformer_model import DINOv2MVSNet

@@ -8,11 +8,9 @@ and leaves every other fixture alone.  Re-run:  python oracle/gen_golden_vit_dec
 Weights: synth.randomize_state_dict(seed=wseed) over a module whose child `decoder_vit` is the decoder.  Inputs are
 torch.randn draws re-drawn bit for bit from the seeds in each fixture's meta (make_tokens), so only outputs are stored.
 """
-import json
 import os
 import sys
 
-import numpy as np
 import torch
 import torch.nn as nn
 
@@ -20,7 +18,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from mvsformerplusplus_b200 import synth  # noqa: E402
-from oracle.ref_hotpath import reference_root  # noqa: E402
+from oracle import fixture, reference  # noqa: E402
 
 CASES = {
     "vit_decoder_b1v3_4x6": dict(B=1, V=3, h=4, w=6, xseed=51, wseed=52, harsh=False),
@@ -43,20 +41,14 @@ def make_tokens(c):
     return x
 
 
-def reference_decoder_cls(root):
-    sys.path.insert(0, root)
-    import models.dino.layers.attention as A
-    A.FLASH_AVAILABLE = False
+def reference_decoder_cls():
+    reference.import_models()
     from models.module import CrossVITDecoder
-    cfg = json.load(open(os.path.join(root, "config", "mvsformer++.json")))["arch"]["args"]
-    return CrossVITDecoder, cfg
+    return CrossVITDecoder, reference.config()
 
 
 def main():
-    root = reference_root()
-    if root is None:
-        raise SystemExit("reference sources not found")
-    CrossVITDecoder, cfg = reference_decoder_cls(root)
+    CrossVITDecoder, cfg = reference_decoder_cls()
     torch.set_num_threads(max(1, os.cpu_count() or 1))
     out_dir = os.path.join(REPO, "tests", "golden")
     for name, c in CASES.items():
@@ -67,8 +59,7 @@ def main():
         x = make_tokens(c)
         with torch.no_grad():
             out = m.decoder_vit(x, vit_shape=[c["B"], c["V"], c["h"], c["w"], 768])
-        blob = dict(out=out.contiguous().numpy(), meta=np.frombuffer(json.dumps(c).encode(), dtype=np.uint8))
-        np.savez_compressed(os.path.join(out_dir, name + ".npz"), **blob)
+        fixture.save(os.path.join(out_dir, name + ".npz"), dict(out=out.contiguous().numpy()), c)
         print(name, tuple(out.shape), float(out.abs().max()))
 
     from models.networks.DINOv2_mvsformer_model import DINOv2MVSNet

@@ -1,42 +1,28 @@
 """ORACLE - TEST INFRASTRUCTURE ONLY.  Runs the REFERENCE's own modules (never this repo's kernels) through the glue of
 models/networks/DINOv2_mvsformer_model.py:117-179.  Used by
 
-  * oracle/gen_golden.py           - generates tests/golden/*.npz in the build container (reference at /root/reference)
+  * oracle/gen_golden.py           - generates the hot-path fixtures under tests/golden/
   * bench.py --impl reference      - times the reference's own CPU implementation of the hot path
                                      (cpu_baseline.kind = "reference") when a copy of the reference's models/ package
                                      is available
 
-The reference is located, in this order: $MVSF_REFERENCE, oracle/_ref/ (made by oracle/build_ref.py in the build
-container; git-ignored build output that travels to the GPU box with the repo snapshot), /root/reference.
-Reference code is imported from there, never copied into tracked files.  Only tests/, __graft_entry__ and bench.py's
-CPU legs may import this module.
+The reference is located and imported by oracle/reference.py, never copied into tracked files.  Only tests/,
+__graft_entry__ and bench.py's CPU legs may import this module.
 """
-import os
-import sys
-
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
+from oracle import reference
 
 
 def reference_root():
     """Directory that holds the reference's `models/` package, or None."""
-    for cand in (os.environ.get("MVSF_REFERENCE"), os.path.join(_HERE, "_ref"), "/root/reference"):
-        if cand and os.path.isfile(os.path.join(cand, "models", "cost_volume.py")):
-            return cand
-    return None
+    return reference.root("models")
 
 
 def import_reference(root=None):
-    root = root or reference_root()
-    if root is None:
-        raise RuntimeError("reference sources not found (oracle/_ref is built by oracle/build_ref.py in the build container)")
-    if root not in sys.path:
-        sys.path.insert(0, root)
-    import models.dino.layers.attention as A
-    A.FLASH_AVAILABLE = False  # CPU: SDPA fallback with the same scale (attention.py:82-96,144-146)
+    reference.import_models(root)  # CPU: SDPA fallback with the same scale (attention.py:82-96,144-146)
     from models.FMT import FMT_with_pathway
     from models.cost_volume import StageNet
     from models.module import init_inverse_range, schedule_inverse_range

@@ -2,22 +2,21 @@
 import json
 import os
 
-import numpy as np
 import torch
 
 from mvsformerplusplus_b200 import synth
 from mvsformerplusplus_b200.config import default_args
 from mvsformerplusplus_b200.params import build_hotpath_params
+from oracle import fixture
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 TMP = [5.0, 5.0, 5.0, 1.0]
 
 
 def load_golden(name):
-    z = np.load(os.path.join(GOLDEN, name + ".npz"))
-    d = {k: torch.from_numpy(z[k]) for k in z.files if k != "meta"}
-    meta = json.loads(bytes(z["meta"]).decode()) if "meta" in z.files else {}
-    return d, meta
+    """-> ({name: CPU tensor}, meta) of tests/golden/<name>.npz"""
+    arrays, meta = fixture.load(os.path.join(GOLDEN, name + ".npz"))
+    return {k: torch.from_numpy(v) for k, v in arrays.items()}, meta
 
 
 def build_case(meta, args=None):

@@ -1,10 +1,10 @@
 """Shared helpers of the depth-map fusion tests: fixture loading and the mask rule."""
-import json
 import os
 
 import numpy as np
 import torch
 
+from oracle import fixture
 from oracle import fusion as OF
 from tests.common import GOLDEN
 
@@ -15,8 +15,7 @@ MAX_DISAGREE = 1e-3  # and that may happen to this fraction of a view's pixels a
 
 def load_fixture(name):
     """-> scene dict (float32 CPU tensors, images back in [0,1]), meta, raw arrays"""
-    z = np.load(os.path.join(GOLDEN, name + ".npz"))
-    meta = json.loads(bytes(z["meta"]).decode())
+    z, meta = fixture.load(os.path.join(GOLDEN, name + ".npz"))
     scene = dict(depths=torch.from_numpy(z["depths"]), confs=torch.from_numpy(z["confs"]), cams=torch.from_numpy(z["cams"]),
                  images=torch.from_numpy(z["images"]).float() / 255.0, pairs=[(r, s) for r, s in meta["pairs"]])
     return scene, meta, z

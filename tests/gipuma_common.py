@@ -1,10 +1,9 @@
 """Shared helpers of the gipuma fusion tests: the reference-executed fixture and the per-view comparison rule."""
-import json
 import os
 
-import numpy as np
 import torch
 
+from oracle import fixture
 from oracle import gipuma as OG
 from tests.common import GOLDEN
 
@@ -14,9 +13,8 @@ MAX_DISAGREE = 1e-3    # ... and on fewer than this share of a view's pixels
 
 
 def load_fixture():
-    """-> scene dict (depths, confs = conf_u8 / 255 in fp32, cams, images in [0,1]), meta, the raw npz"""
-    z = np.load(os.path.join(GOLDEN, FIXTURE + ".npz"))
-    meta = json.loads(bytes(z["meta"]).decode())
+    """-> scene dict (depths, confs = conf_u8 / 255 in fp32, cams, images in [0,1]), meta, the raw arrays"""
+    z, meta = fixture.load(os.path.join(GOLDEN, FIXTURE + ".npz"))
     scene = dict(depths=torch.from_numpy(z["depths"]), confs=torch.from_numpy(z["conf_u8"]).float() / 255,
                  cams=torch.from_numpy(z["cams"]), images=torch.from_numpy(z["images"]).float() / 255)
     return scene, meta, z

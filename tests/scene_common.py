@@ -1,11 +1,11 @@
 """The scene fixtures tests/golden/scene_*.npz (oracle/gen_golden_scene.py: the reference's own eval loader and file
 writers on small seeded scene folders): the folder rebuilt from its stored bytes, and the reference's items."""
 import functools
-import json
 import os
 
 import numpy as np
 
+from oracle import fixture as F
 from tests.common import GOLDEN
 
 CASES = ("dtu", "tt_identity", "tt_short_range", "eth3d")
@@ -13,10 +13,8 @@ CASES = ("dtu", "tt_identity", "tt_short_range", "eth3d")
 
 @functools.lru_cache(maxsize=None)
 def fixture(name):
-    """-> (npz contents as a dict, meta)"""
-    with np.load(os.path.join(GOLDEN, f"scene_{name}.npz")) as z:
-        blob = {k: z[k] for k in z.files}
-    return blob, json.loads(blob["meta"].tobytes().decode())
+    """-> (arrays, meta)"""
+    return F.load(os.path.join(GOLDEN, f"scene_{name}.npz"))
 
 
 def write_folder(name, root):

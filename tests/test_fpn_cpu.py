@@ -2,7 +2,6 @@
 reference-executed fixtures, state-dict keys, BN folding of the packed weights, argument checks, loud failure on the CPU
 and the install() seam."""
 import ctypes
-import json
 import os
 
 import pytest
@@ -113,18 +112,13 @@ def test_fpn_modules_fail_loudly_on_cpu():
 
 
 def _reference_model():
-    import sys
-    from oracle import ref_hotpath as RH
-    root = RH.reference_root()
-    if root is None or not os.path.isfile(os.path.join(root, "config", "mvsformer++.json")):
+    from oracle import reference
+    if reference.root("models", reference.CONFIG) is None:
         pytest.skip("no reference sources (oracle/_ref is made by build() only where the reference is available)")
-    sys.path.insert(0, root)
-    import models.dino.layers.attention as A
-    A.FLASH_AVAILABLE = False
+    reference.import_models()
     from models.networks.DINOv2_mvsformer_model import DINOv2MVSNet
-    cfg = json.load(open(os.path.join(root, "config", "mvsformer++.json")))["arch"]["args"]
     torch.manual_seed(0)
-    model = DINOv2MVSNet(cfg).eval()
+    model = DINOv2MVSNet(reference.config()).eval()
     synth.randomize_state_dict(model.FMT_module, seed=3)
     synth.randomize_state_dict(model.fusions, seed=4)
     return model

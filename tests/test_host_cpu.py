@@ -186,20 +186,14 @@ def test_install_on_reference_constructed_model_keeps_the_checkpoint_contract():
     """test.py:209-220 on the real thing: init_model -> DINOv2MVSNet(arch.args); install() swaps FMT_module / fusions for
     this package's modules; every state-dict key and value of the model is unchanged, so a reference checkpoint loads with
     strict=True before or after install()."""
-    import json
-    import sys
-    from oracle import ref_hotpath as RH
-    root = RH.reference_root()
-    if root is None or not os.path.isfile(os.path.join(root, "config", "mvsformer++.json")):
+    from oracle import reference
+    if reference.root("models", reference.CONFIG) is None:
         pytest.skip("no reference sources (oracle/_ref is made by build() only where the reference is available)")
-    sys.path.insert(0, root)
-    import models.dino.layers.attention as A
-    A.FLASH_AVAILABLE = False
+    reference.import_models()
     from models.networks.DINOv2_mvsformer_model import DINOv2MVSNet
     from mvsformerplusplus_b200 import hotpath
-    cfg = json.load(open(os.path.join(root, "config", "mvsformer++.json")))["arch"]["args"]
     torch.manual_seed(0)
-    model = DINOv2MVSNet(cfg).eval()
+    model = DINOv2MVSNet(reference.config()).eval()
     synth.randomize_state_dict(model.FMT_module, seed=3)
     synth.randomize_state_dict(model.fusions, seed=4)
     before = {k: v.clone() for k, v in model.state_dict().items()}

@@ -218,16 +218,12 @@ def test_install_vit_keeps_the_checkpoint_contract():
 
 
 def test_install_vit_on_the_reference_model():
-    from oracle.ref_hotpath import reference_root
-    root = reference_root()
-    if root is None or not os.path.isdir(os.path.join(root, "config")):
+    from oracle import reference
+    if reference.root("models", reference.CONFIG) is None:
         pytest.skip("reference modules not available")
-    from oracle.gen_golden_vit import reference_vit_base
-    reference_vit_base(root)
-    import json
+    reference.import_models()
     from models.networks.DINOv2_mvsformer_model import DINOv2MVSNet
-    cfg = json.load(open(os.path.join(root, "config", "mvsformer++.json")))["arch"]["args"]
-    model = DINOv2MVSNet(cfg).eval()
+    model = DINOv2MVSNet(reference.config()).eval()
     wrap = torch.nn.Module()
     wrap.vit = model.vit
     sd = {k: v for k, v in vit_state_dict(10).items()}

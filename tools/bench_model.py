@@ -40,12 +40,11 @@ def card():
 
 def reference_model(sd, dev):
     """the reference's own DINOv2MVSNet (oracle/_ref) with the weights sd, or None"""
+    from oracle import reference
     from oracle.gen_golden_model import reference_model as ref_cls
-    from oracle.ref_hotpath import reference_root
-    root = reference_root()
-    if root is None or not os.path.isfile(os.path.join(root, "config", "mvsformer++.json")):
+    if reference.root("models", reference.CONFIG) is None:
         return None
-    cls, cfg = ref_cls(root)
+    cls, cfg = ref_cls()
     m = cls(cfg)
     m.load_state_dict(sd, strict=True)
     return m.to(dev).eval()
