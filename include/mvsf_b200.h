@@ -109,6 +109,13 @@ int mvsf_vis_cnn(const float* entropy, const float* wts, float* vis, int N, int 
  * models/cost_volume.py:72-101 -> volume [D][H][W][G] = sum_v w_v*inprod_v / (sum_v w_v + 1e-6) */
 int mvsf_warp_corr_aggregate(const float* feat, const float* homs, const float* depth, const float* vis,
                              float* volume, int V, int C, int G, int D, int H, int W, mvsf_stream_t stream);
+/* ---- adjoint of pass B (training): grad_volume = dL/dvolume [D][H][W][G], volume = pass B's output for the same
+ * feat / homs / depth / vis -> grad_feat [V][H][W][C] (reference view written, source views zeroed on the stream and then
+ * accumulated with atomics) and grad_vis [(V-1)][H][W] (written).  Same (C, G) as mvsf_warp_corr_aggregate; feat and
+ * grad_feat 16-byte aligned.  No gradient to homs or depth (the reference builds the grid under no_grad). */
+int mvsf_warp_corr_aggregate_backward(const float* feat, const float* homs, const float* depth, const float* vis,
+                                      const float* volume, const float* grad_volume, float* grad_feat, float* grad_vis,
+                                      int V, int C, int G, int D, int H, int W, mvsf_stream_t stream);
 /* Faster variant of the two calls above (the one hotpath.py uses): pass A additionally stores the per-view group
  * correlations corr [V-1][D][H*W][G] (G must be 8; 4*G*D*H*W*(V-1) bytes), the view aggregation then streams them
  * instead of gathering the source features a second time (the gather is L1-request bound, HBM has headroom). */
