@@ -12,6 +12,7 @@ import torch
 import torch.nn.functional as F
 
 from mvsformerplusplus_b200 import _lib
+from tests import conv3d_common as C3
 from tests import cost_volume_common as R
 from tests.common import ROOT, TMP, build_case, load_golden, max_abs, rec, rel_linf
 
@@ -309,51 +310,19 @@ def test_vis_cnn_tile_borders(dev):
 def test_conv3d_tensor_core_layer(dev, mode, sd, cin, cout, ID, IH, IW, skip):
     """One 3x3x3 layer of the wgmma implicit-GEMM path against torch's fp64 convolution (conv / strided conv /
     transposed conv with output_padding = stride - 1, bias, ReLU, skip added after the ReLU)."""
-    import torch.nn.functional as F
-    g = torch.Generator().manual_seed(mode * 100 + cin + ID)
-    x = torch.randn(ID, IH, IW, cin, generator=g)
-    w = torch.randn(27, cin, cout, generator=g) / (27 * cin) ** 0.5 * 1.7
-    b = torch.randn(cout, generator=g) * 0.2
-    xin = x.permute(3, 0, 1, 2)[None].double()
-    if mode == 2:
-        wt = w.reshape(3, 3, 3, cin, cout).permute(3, 4, 0, 1, 2).double()
-        y = F.conv_transpose3d(xin, wt, stride=(sd, 2, 2), padding=1, output_padding=(sd - 1, 1, 1))
-    else:
-        wt = w.reshape(3, 3, 3, cin, cout).permute(4, 3, 0, 1, 2).double()
-        y = F.conv3d(xin, wt, stride=(1, 1, 1) if mode == 0 else (sd, 2, 2), padding=1)
-    y = torch.relu(y + b.double().view(1, -1, 1, 1, 1))[0].permute(1, 2, 3, 0).contiguous()
-    sk = torch.randn(y.shape, generator=g) if skip else None
-    if skip:
-        y = y + sk.double()
-    x_d, wb_d = x.contiguous().to(dev), torch.cat([w.reshape(-1), b]).to(dev)
-    sk_d = sk.contiguous().to(dev) if skip else None
-    out = torch.empty(y.shape, device=dev)
-    ws = torch.empty((2 * x.numel() + 4 * y.numel()) // 2 + 27 * cin * max(cout, 16) * 4 + 1024, device=dev)
-    _lib.call("mvsf_conv3d_tc_layer", mode, sd, x_d, wb_d, sk_d, out, ws, ws.numel() * 4, cin, cout, ID, IH, IW)
-    e = float((out.cpu().double() - y).abs().max())
-    rec(f"conv3d_tc_mode{mode}_sd{sd}_{cin}to{cout}_{ID}x{IH}x{IW}_skip{int(skip)}", abs=e, scale=float(y.abs().max()))
-    assert e < 1e-5 * max(1.0, float(y.abs().max()))
+    e, scale = C3.layer_vs_fp64(dev, mode, sd, cin, cout, ID, IH, IW, skip, seed=mode * 100 + cin + ID)
+    rec(f"conv3d_tc_mode{mode}_sd{sd}_{cin}to{cout}_{ID}x{IH}x{IW}_skip{int(skip)}", abs=e, scale=scale)
+    assert e < C3.LAYER_TOL * max(1.0, scale)
 
 
 @pytest.mark.parametrize("stage,D,H,W", [(1, 16, 16, 24), (1, 8, 8, 40), (2, 8, 16, 24), (3, 4, 24, 40), (3, 3, 8, 8)])
 def test_costreg_unet_two_part(dev, stage, D, H, W):
-    from mvsformerplusplus_b200 import packing
-    from oracle import hotpath as O
-    sd = _rand_vis_sd(13)
-    g = torch.Generator().manual_seed(stage * 7 + D)
-    vol = torch.randn(1, 8, D, H, W, generator=g) * 0.5
-    p = f"fusions.{stage}.cost_reg."
-    want = O.costreg_unet(vol, sd, p)[0, 0]
-    kind, conv, small = packing.pack_costreg_unet(sd, p)
-    ws = _lib.workspace("mvsf_costreg_unet_workspace_bytes", kind, 8, D, H, W, device=dev)
-    logits = torch.empty(D, H, W, device=dev)
-    v = vol[0].permute(1, 2, 3, 0).contiguous().to(dev)
-    from mvsformerplusplus_b200.hotpath import pack_unet_tc
-    tc = pack_unet_tc(kind, conv.to(dev))
-    _lib.call("mvsf_costreg_unet_forward", kind, v, small.to(dev), tc, logits, ws, ws.numel() * 4, 8, D, H, W)
-    e = max_abs(logits.cpu(), want)
-    rec(f"costreg_unet_stage{stage}_{D}x{H}x{W}", abs=e, scale=float(want.abs().max()))
-    assert e < 2e-4 * max(1.0, float(want.abs().max()))
+    """Both parts of a U-Net (conv weights packed for the tensor cores, fp32 biases and `prob` conv) against the fp64
+    oracle; stage 1 is CostRegNet, stages 2 and 3 CostRegNet3D"""
+    e, scale = C3.unet_vs_fp64(dev, _rand_vis_sd(13), f"fusions.{stage}.cost_reg.", 0 if stage == 1 else 1, D, H, W,
+                               seed=stage * 7 + D)
+    rec(f"costreg_unet_stage{stage}_{D}x{H}x{W}", abs=e, scale=scale)
+    assert e < C3.UNET_TOL * max(1.0, scale)
 
 
 # |logits - fp64| <= COSTREG_TR_TOL * max(1, max|fp64|).  The attention's P is fp16, so the error grows as the token count
