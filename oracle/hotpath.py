@@ -215,10 +215,10 @@ def position_encoding_3d(position3d, C, rescale=4.0):
     """position_encoding.py:164-189 -> [B,3C,D,H,W]."""
     B, _, D, H, W = position3d.shape
     dt = position3d.dtype
-    div = torch.exp(torch.arange(0, C, 2).float() * (-math.log(10000.0) / C)).to(dt)[None, :, None]
+    div = torch.exp(torch.arange(0, C, 2).float() * (-math.log(10000.0) / C)).to(position3d.device, dt)[None, :, None]
     pes = []
     for a in range(3):
-        pe = torch.zeros(B, C, D * H * W, dtype=dt)
+        pe = torch.zeros(B, C, D * H * W, dtype=dt, device=position3d.device)
         pos = position3d[:, a].reshape(B, 1, -1)
         pe[:, 0::2] = torch.sin(pos * rescale * div)
         pe[:, 1::2] = torch.cos(pos * rescale * div)
